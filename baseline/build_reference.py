@@ -5,7 +5,7 @@ The reference is a CMake project whose configure step downloads pybind11 (`HugeC
 and links libaio / libnuma / tbb, none of which exist in this image, so `pip install /root/reference` and a
 stock `cmake` both fail (DESIGN.md section 4).  This script does what that CMake tree does, with nothing
 fetched: it globs the same source lists (`HugeCTR/core23/CMakeLists.txt`, `HugeCTR/embedding/CMakeLists.txt`,
-`gpu_cache/src/CMakeLists.txt`, `HugeCTR/src/CMakeLists.txt` with `-DDISABLE_CUDF=ON -DSM=100`), compiles them
+`gpu_cache/src/CMakeLists.txt`, `HugeCTR/src/CMakeLists.txt` with `-DDISABLE_CUDF=ON -DSM=90`), compiles them
 straight from the read-only tree with the same definitions and language flags, and links the same four
 libraries plus the `hugectr` pybind11 module into `baseline/_ref/`.  No reference source file is edited.
 Substitutions, all on the build side:
@@ -69,7 +69,7 @@ def main():
     incf = " ".join("-I" + i for i in inc)
     defs = "-DDISABLE_CUDF -DLIBCUDACXX_ENABLE_EXPERIMENTAL_MEMORY_RESOURCE -DNDEBUG"
     cxxflags = f"-std=c++17 -O3 -fPIC -fopenmp -Wno-sign-compare -Wno-deprecated-declarations {defs} {incf}"
-    cuflags = (f"-std=c++17 -O3 -gencode arch=compute_100,code=sm_100 --expt-extended-lambda "
+    cuflags = (f"-std=c++17 -O3 -gencode arch=compute_90,code=sm_90 --expt-extended-lambda "
                f"--expt-relaxed-constexpr -Xcompiler -fPIC,-fopenmp -Xcudafe --diag_suppress=177 "
                f"-w {defs} {incf}")
 

@@ -1,11 +1,13 @@
 #!/usr/bin/env python
 """Headline benchmark: DLRM-DCNv2 (MLPerf v3.1 config, Criteo-TB table sizes / multi-hot sizes,
 128-dim embeddings, bottom MLP 512-256-128, 3 x low-rank cross (p=512), top MLP 1024-1024-512-256-1,
-AdaGrad) training throughput in samples/s on N B200 GPUs of one node, bf16, synthetic power-law data.
+AdaGrad) training throughput in samples/s on N H100 GPUs of one node, bf16, synthetic power-law data.
 
   python bench.py --gpus N --steps K --warmup W            (N>1: launched by torch.distributed.run)
   python bench.py --impl reference ...                     (unmodified reference built by baseline/build_reference.py)
   python bench.py --impl nccl_cublas ...                   (stand-in baseline: our model on NCCL collectives + cuBLAS GEMMs)
+  python bench.py ... --dump-outputs DIR                   (loss, predictions and a sample of the dense weights
+                                                            after the last timed step, as DIR/<name>.npy)
 
 Prints ONE JSON line on rank 0 (contract in the task description).  Weak scaling: 6912 samples per
 GPU (the MLPerf 8-GPU global batch 55296 / 8).
@@ -24,7 +26,9 @@ import time
 
 PER_GPU_BATCH = 6912
 BASELINE_SAMPLES_PER_S = 14.7e6   # BASELINE.md: implied (derived) HugeCTR MLPerf v3.1 rate on 8 x H100
-ROW_CAP_1GPU = 22_000_000         # N == 1 only: fp32 tables + fp32 AdaGrad state must fit 180 GB (see run_arm)
+ROW_CAP_1GPU = 10_000_000         # N == 1 only: fp32 tables + fp32 AdaGrad state (55 GB) must fit 80 GB (see main)
+ROW_CAP_1GPU_BF16_STATE = 13_000_000   # N == 1 secondary arm: fp32 tables + bf16 AdaGrad state, 53 GB
+DUMP_DENSE_SAMPLE = 1 << 20       # dense weights written by --dump-outputs (fixed, seeded sample of the arena)
 HERE = os.path.dirname(os.path.abspath(__file__))
 
 # Schedules tried in order when the headline arm does not exist after --headline-timeout seconds (a multi-GPU
@@ -259,8 +263,25 @@ def _note(comm, msg):
         sys.stderr.flush()
 
 
-def run_arm(args, comm, *, standin=False, state="fp32", cap_rows=0, K=30, W=5, sustained_s=2.0, label="b200",
-            on_partial=None):
+def dump_outputs(model, out_dir):
+    """What the last training step computed, as float32 .npy files: the loss, the predicted probabilities of the
+    batch (sigmoid of the logits the loss layer consumed) and a fixed, seeded sample of the updated dense weights
+    (the same indices on every run and build)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    ll = model.net_train.loss_layers
+    logits = torch.cat([l.inputs[0].data.reshape(l.inputs[0].data.shape[0], -1) for l in ll], 1)
+    w = model.arena.weights
+    g = torch.Generator().manual_seed(12345)
+    idx = torch.randperm(w.numel(), generator=g)[:DUMP_DENSE_SAMPLE].sort().values.to(w.device)
+    arrays = {"loss": model.net_train.loss_value().reshape(-1), "predictions": torch.sigmoid(logits.float()), "dense_weights_sample": w[idx]}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
+
+
+def run_arm(args, comm, *, standin=False, state="fp32", cap_rows=0, K=30, W=5, sustained_s=0.0, label="b200",
+            on_partial=None, dump_dir=""):
     """Build the model for one configuration, time it, tear it down.  Returns the measurements (rank 0: dict)."""
     _note(comm, f"arm standin={standin} state={state} cap={cap_rows}: building")
     import gc
@@ -367,6 +388,8 @@ def run_arm(args, comm, *, standin=False, state="fp32", cap_rows=0, K=30, W=5, s
     ms_dev = timed(K)
     sync_all()
     _note(comm, f"device-timed done: {ms_dev / K:.3f} ms/step")
+    if dump_dir and rank == 0:
+        dump_outputs(model, dump_dir)
     ms_dev = maxr([ms_dev])[0]
     n_clk_short = len(samples)
     loss_trace.append(model.get_current_loss())
@@ -543,7 +566,7 @@ def _compose(args, n, K, W, r, secondary, standin):
                    "parallelism": f"dp{n} dense + model-parallel embeddings (plan={args.plan})",
                    "embedding_weights": "fp32", "embedding_opt_state": r["state"],
                    "row_cap": r["cap_rows"], "embedding_bytes_resident_per_gpu": r["table_bytes"],
-                   "l2_hygiene": "inputs_exceed_L2 (>=50 GB of tables per GPU under random access, "
+                   "l2_hygiene": "inputs_exceed_L2 (>=28 GB of tables per GPU under random access, "
                                  "~1 GB activations/step, a different batch every step)",
                    "synthetic_pool_batches": r["pool_batches"],
                    "cuda_graph": not args.no_graph, "small_tables_debug": bool(args.small or args.cap_rows),
@@ -577,7 +600,8 @@ def main():
     ap.add_argument("--profile", default="", help="dump a torch.profiler kernel table (rank 0) here")
     ap.add_argument("--no-standin", action="store_true", help="skip the NCCL+cuBLAS stand-in arm")
     ap.add_argument("--no-secondary", action="store_true", help="N=1: skip the bf16-state full-size run")
-    ap.add_argument("--sustained-sec", type=float, default=2.0)
+    ap.add_argument("--sustained-sec", type=float, default=0.0,
+                    help="after the --steps timed steps, time back-to-back steps for this many seconds more")
     ap.add_argument("--ref-timeout", type=int, default=1500)
     ap.add_argument("--headline-timeout", type=float, default=240.0,
                     help="seconds until the headline arm must exist; then the rank re-executes itself with the "
@@ -588,6 +612,8 @@ def main():
                     help="skip the end-to-end measurement through the RawAsync FILE reader")
     ap.add_argument("--fp8-mlp", action="store_true",
                     help="forward MLP GEMMs in MX block-scaled fp8 (Solver.use_fp8_mlp); reported in config.fp8_mlp")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the loss, predictions and a dense-weight sample of the last timed step to DIR/*.npy")
     ap.add_argument("--model", default="dlrm_dcnv2",
                     help="dlrm_dcnv2 (headline) | deepfm | dlrm | wdl_cache (secondary configurations)")
     args = ap.parse_args()
@@ -623,10 +649,10 @@ def main():
         faulthandler.dump_traceback_later(120, exit=True)
         comm.shutdown()
         return 0
-    # 104 GB of fp32 tables + 104 GB of fp32 AdaGrad state do not fit one 180 GB GPU.  N == 1 therefore runs
-    # fp32 state (the reference's precision) with the six 40 M-row tables capped at ROW_CAP_1GPU rows (declared
-    # in config.row_cap; same random-access pattern, 146 GB resident), and reports the full-size run with bf16
-    # AdaGrad accumulators as `secondary`.  N >= 2: full tables, fp32 state.
+    # 104 GB of fp32 tables + 104 GB of fp32 AdaGrad state do not fit one 80 GB H100.  N == 1 therefore runs
+    # fp32 state (the reference's precision) with the five 40 M-row tables capped at ROW_CAP_1GPU rows (declared
+    # in config.row_cap; same random-access pattern, 55 GB resident), and reports a run with bf16 AdaGrad
+    # accumulators and ROW_CAP_1GPU_BF16_STATE rows as `secondary`.  N >= 2: full tables, fp32 state.
     cap = args.cap_rows or (ROW_CAP_1GPU if (n == 1 and not args.small) else 0)
     standin_only = args.impl == "nccl_cublas"
     # As soon as the headline (K device-timed steps + the end-to-end loop) exists, a watchdog guards everything
@@ -659,17 +685,17 @@ def main():
         t.start()
         wd_box.append(t)
     main_res = run_arm(args, comm, standin=standin_only, state="fp32", cap_rows=cap, K=K, W=W,
-                       sustained_s=args.sustained_sec, on_partial=on_partial)
+                       sustained_s=args.sustained_sec, on_partial=on_partial, dump_dir=args.dump_outputs)
     extra["main"] = main_res
     secondary = None
     if n == 1 and not args.small and not args.cap_rows and not args.no_secondary and not standin_only:
         try:
-            r2 = run_arm(args, comm, state="bf16", cap_rows=0, K=K, W=W, sustained_s=0.0)
-            secondary = {"bf16_adagrad_state_full_tables": {
+            r2 = run_arm(args, comm, state="bf16", cap_rows=ROW_CAP_1GPU_BF16_STATE, K=K, W=W, sustained_s=0.0)
+            secondary = {"bf16_adagrad_state": {
                 "value": r2["value"], "ms_per_step": r2["ms_per_step"], "e2e": r2["e2e"]["value"],
-                "table_bytes": r2["table_bytes"], "final_loss": r2["final_loss"]}}
+                "row_cap": r2["cap_rows"], "table_bytes": r2["table_bytes"], "final_loss": r2["final_loss"]}}
         except Exception as e:       # noqa: BLE001 -- a secondary figure must not take the headline down
-            secondary = {"bf16_adagrad_state_full_tables": {"error": repr(e)[:300]}}
+            secondary = {"bf16_adagrad_state": {"error": repr(e)[:300]}}
     extra["secondary"] = secondary
     standin = None
     if not args.no_standin and not standin_only:

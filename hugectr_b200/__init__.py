@@ -1,4 +1,4 @@
-"""hugectr_b200 -- a Blackwell (sm_100a) native CTR training framework with HugeCTR's API.
+"""hugectr_b200 -- a Hopper (sm_90a, H100) native CTR training framework with HugeCTR's API.
 
 ``import hugectr`` resolves to this package (see the top-level ``hugectr`` shim): CreateSolver,
 DataReaderParams, CreateOptimizer, Model, Input, SparseEmbedding, DenseLayer,

@@ -10,15 +10,15 @@ from hugectr_b200 import _native
 
 def main():
     print(f"hugectr_b200 {h.__version__}  (python {sys.version.split()[0]}, torch {torch.__version__})")
-    for name, path in (("sm_100a kernels", _native.CUDA_SO), ("host runtime", _native.HOST_SO)):
+    for name, path in (("sm_90a kernels", _native.CUDA_SO), ("host runtime", _native.HOST_SO)):
         st = f"{os.path.getsize(path) / 1e6:.1f} MB" if os.path.exists(path) else "NOT BUILT (python __graft_entry__.py)"
         print(f"  {name:16s} {path}  {st}")
     if torch.cuda.is_available():
         p = torch.cuda.get_device_properties(0)
         print(f"  device 0         {p.name}, sm_{p.major}{p.minor}, {p.multi_processor_count} SMs, "
               f"{p.total_memory / 2**30:.0f} GiB, {torch.cuda.device_count()} visible")
-        if (p.major, p.minor) != (10, 0):
-            print("  WARNING: the kernels are compiled for sm_100a only")
+        if (p.major, p.minor) != (9, 0):
+            print("  WARNING: the kernels are compiled for sm_90a only")
     else:
         print("  device           none (CPU reference paths and gloo collectives only)")
     try:

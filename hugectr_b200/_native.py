@@ -1,13 +1,13 @@
 """Native code build + loader.
 
-All device code lives in ``hugectr_b200/csrc/*.cu`` and is compiled **only** for sm_100a
-(``-gencode arch=compute_100a,code=sm_100a``) into ``hugectr_b200/lib/libhctr_cuda.so``; host-side
+All device code lives in ``hugectr_b200/csrc/*.cu`` and is compiled **only** for sm_90a
+(``-gencode arch=compute_90a,code=sm_90a``, the H100) into ``hugectr_b200/lib/libhctr_cuda.so``; host-side
 native runtime pieces (readers, generators, host parameter server, thread pool) live in
 ``csrc/host/*.cpp`` -> ``lib/libhctr_host.so``.  Launchers are ``extern "C"`` and are called through
 ctypes with raw device pointers and the current torch CUDA stream, so the kernels run on torch's
 streams and are captured by CUDA graphs like any other launch.
 
-The shared objects are built in-tree (git-ignored, but they travel with ``gpurun`` snapshots).
+The shared objects are built in-tree (git-ignored) by ``build()``.
 """
 from __future__ import annotations
 
@@ -26,7 +26,7 @@ CUDA_SO = os.path.join(LIBDIR, "libhctr_cuda.so")
 HOST_SO = os.path.join(LIBDIR, "libhctr_host.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "--use_fast_math", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 CXX_FLAGS = ["-O3", "-std=c++17", "-fPIC", "-pthread", "-fopenmp", "-march=x86-64-v3"]
@@ -78,7 +78,7 @@ def build_cuda(force: bool = False, verbose: bool = False) -> str:
                 if verbose and out.strip():
                     print(out)
     if jobs or not os.path.exists(CUDA_SO):
-        _run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", CUDA_SO, *objs,
+        _run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", CUDA_SO, *objs,
               "-Xcompiler", "-fPIC"])
     return CUDA_SO
 
@@ -112,7 +112,7 @@ def _preload_cudart():
 
 
 def cuda_lib() -> ctypes.CDLL:
-    """ctypes handle on the sm_100a kernel library. Fails loudly when it is missing."""
+    """ctypes handle on the sm_90a kernel library. Fails loudly when it is missing."""
     global _cuda_lib
     if _cuda_lib is None:
         with _lock:

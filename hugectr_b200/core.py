@@ -13,7 +13,7 @@ they are and whom they talk to; two back-ends implement it:
   one-GPU proof of the peer kernels).
 
 ``KernelParams`` mirrors core23::KernelParams (SM count, warp size, max threads per block / SM) and is what
-launch-size decisions should read instead of a literal 148.
+launch-size decisions should read instead of a literal SM count (132 on an H100 SXM).
 """
 from __future__ import annotations
 
@@ -26,7 +26,7 @@ import torch
 
 @dataclass(frozen=True)
 class KernelParams:
-    num_sms: int = 148
+    num_sms: int = 132
     warp_size: int = 32
     max_threads_per_block: int = 1024
     max_threads_per_sm: int = 2048

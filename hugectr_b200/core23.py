@@ -30,7 +30,7 @@ ALIGN = 256
 class DeviceType(Enum):
     CPU = "cpu"
     GPU = "cuda"
-    UNIFIED = "managed"      # served from pinned host memory here (B200 reads it over C2C / PCIe)
+    UNIFIED = "managed"      # served from pinned host memory here (the GPU reads it over PCIe)
 
 
 @dataclass(frozen=True)

@@ -1,4 +1,4 @@
-// D4 elementwise / reduction family + fused dense optimizers + loss kernels (sm_100a).
+// D4 elementwise / reduction family + fused dense optimizers + loss kernels (sm_90a).
 //   fused optimizers over the flat parameter arena  (reference HugeCTR/src/optimizers/*.cu)
 //   BinaryCrossEntropy fwd+bwd in one pass           (reference HugeCTR/src/loss.cu:231-264)
 //   bias-grad column reduction, skinny (N==1) FC fwd/bwd, DCNv2 backward elementwise fusion
@@ -479,7 +479,7 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-static inline int grid_for(long long n, int threads, int max_blocks = 148 * 16) {
+static inline int grid_for(long long n, int threads, int max_blocks = num_sms() * 16) {
   long long b = (n + threads - 1) / threads;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;
@@ -497,7 +497,7 @@ extern "C" int hctr_abi_size_dense_opt() { return static_cast<int>(sizeof(DenseO
 extern "C" int hctr_dense_opt(const DenseOptArgs* a, int opt, void* stream) {
   if (a->n == 0) return 0;
   const int threads = 256;
-  const int blocks = grid_for((a->n + 3) / 4, threads, 148 * 8);
+  const int blocks = grid_for((a->n + 3) / 4, threads, num_sms() * 8);
   switch (opt) {
     case D_SGD: dense_opt_kernel<D_SGD><<<blocks, threads, 0, ST(stream)>>>(*a); break;
     case D_ADAGRAD: dense_opt_kernel<D_ADAGRAD><<<blocks, threads, 0, ST(stream)>>>(*a); break;
@@ -522,7 +522,7 @@ extern "C" int hctr_lr_step(unsigned int* step, float* lr, float base_lr, float 
 extern "C" int hctr_bce_loss(const void* x, const float* y, void* dx, float* loss_out, int n,
                              float grad_scale, float loss_scale, int is_train, int want_loss,
                              int is_bf16, void* stream) {
-  const int blocks = grid_for(n, 256, 148 * 4);
+  const int blocks = grid_for(n, 256, num_sms() * 4);
   if (is_bf16)
     bce_loss_kernel<bf16><<<blocks, 256, 0, ST(stream)>>>((const bf16*)x, y, (bf16*)dx, loss_out, n,
                                                           grad_scale, loss_scale, is_train, want_loss);
@@ -537,7 +537,7 @@ extern "C" int hctr_colsum(const void* x, float* out, int M, int N, long long ld
   const int cols_per_block = is_bf16 ? 256 : 128;
   const int gx = (N + cols_per_block - 1) / cols_per_block;
   int gy = 1;
-  while (gx * gy < 296 && M / (gy * 2) >= 64) gy *= 2;   // ~2 waves of blocks
+  while (gx * gy < 2 * num_sms() && M / (gy * 2) >= 64) gy *= 2;   // ~2 waves of blocks
   dim3 grid(gx, gy);
   if (is_bf16) colsum_kernel<bf16><<<grid, 256, 0, ST(stream)>>>((const bf16*)x, out, M, N, ld);
   else colsum_kernel<float><<<grid, 256, 0, ST(stream)>>>((const float*)x, out, M, N, ld);
@@ -603,7 +603,7 @@ extern "C" int hctr_cross_bwd_ew(const void* dy, const void* x0, const void* t, 
                                  int dx0_bf16, int row_splits, void* stream) {
   if (cols % 8) return -2;
   const int gx = (cols / 8 + 15) / 16;
-  int gy = row_splits > 0 ? row_splits : (148 * 4 + gx - 1) / gx;
+  int gy = row_splits > 0 ? row_splits : (num_sms() * 4 + gx - 1) / gx;
   if (gy * 16 > rows) gy = (rows + 15) / 16;
   if (gy < 1) gy = 1;
   if (dx0_bf16)

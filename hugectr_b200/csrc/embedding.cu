@@ -501,7 +501,7 @@ extern "C" int hctr_emb_backward_accum(const EmbParams* p, const UniqueTable* ut
       cudaFuncSetAttribute(emb_dp_wgrad_kernel<long long, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
       attr_set = true;
     }
-    int chunks = (2 * 148 + p->num_lookups - 1) / p->num_lookups;
+    int chunks = (2 * num_sms() + p->num_lookups - 1) / p->num_lookups;
     if (chunks > 64) chunks = 64;
     if (chunks * 8 > p->batch) chunks = (p->batch + 7) / 8;
     if (chunks < 1) chunks = 1;

@@ -524,10 +524,14 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       load_a(i + groups, 1, 1);
       const unsigned int uid = rec[0].x;
       const long long base = static_cast<long long>(row[0]) * ev;
-      float4 wv[NC], sv[NC], acc[NC];
+      // the row in passes of at most 4 chunks: weights, state and sums of one pass stay within the
+      // 128 registers of two resident blocks per SM for G == 32 (8 chunks per lane)
 #pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        const int col = (c * G + gl) * 4;
+      for (int c0 = 0; c0 < NC; c0 += 4) {
+      float4 wv[4], sv[4], acc[4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) {
+        const int col = ((c0 + c) * G + gl) * 4;
         wv[c] = sv[c] = acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (col < ev) {
           wv[c] = *reinterpret_cast<const float4*>(p.table + base + col);
@@ -535,8 +539,8 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
         }
       }
 #pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        const int col = (c * G + gl) * 4;
+      for (int c = 0; c < 4; ++c) {
+        const int col = ((c0 + c) * G + gl) * 4;
         if (col < ev) {
           float4 g[4];
 #pragma unroll
@@ -551,8 +555,8 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
         }
       }
 #pragma unroll
-      for (int c = 0; c < NC; ++c) {
-        const int col = (c * G + gl) * 4;
+      for (int c = 0; c < 4; ++c) {
+        const int col = ((c0 + c) * G + gl) * 4;
         if (col < ev) {
           float4 w = wv[c];
           apply_opt4_pre<OPT, StateT>(w, make_float4(acc[c].x * inv_scaler, acc[c].y * inv_scaler,
@@ -560,6 +564,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
                                       sv[c], s0, s1, base + col, hp, lr, bc1, bc2);
           *reinterpret_cast<float4*>(p.table + base + col) = w;
         }
+      }
       }
       if (gl == 0) {
         const unsigned int slot = ut.slots[uid];
@@ -745,7 +750,7 @@ extern "C" int hctr_emb_bwd_index(const EmbParams* p, const UniqueTable* ut, con
                                        ix->heavy_slot, ix->class_count);
   scan_apply_kernel<<<nb, 1024, 0, st>>>(ix->count, ix->block_sums, ix->offsets, ut->counter,
                                          ut->max_unique);
-  emb_bwd_classify_kernel<<<148, 1024, 0, st>>>(*ut, *ix);
+  emb_bwd_classify_kernel<<<num_sms(), 1024, 0, st>>>(*ut, *ix);
   emb_bwd_fill_kernel<<<blocks, kIdxThreads, 0, st>>>(*p, *ix, total_pairs);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -1,4 +1,4 @@
-// Shared declarations + the fused epilogue of the tcgen05 GEMM kernels (gemm_tc.cu, gemm_tc2.cu).
+// Shared declarations + the fused epilogue of the wgmma GEMM kernels (gemm_tc.cu, gemm_mxfp8.cu).
 #pragma once
 #include "ptx.cuh"
 
@@ -32,13 +32,11 @@ struct GemmParams {
   int flags;
   const float* addf;
   long long ldaddf;
-  float* colsum;   // optional fp32 [N]: += column sums of the (bf16-rounded) output -- the bias gradient
-                   // of the layer that consumes this GEMM's output as its dY (TMA epilogue only)
 };
 
 
-// One thread owns row `m`, columns [n0, n0+32) of the tile: r[] are the fp32 accumulators read from
-// TMEM with tcgen05.ld.32x32b.x32.
+// One thread owns row `m`, columns [n0, n0+32) of the tile: r[] are the fp32 accumulators (bit patterns)
+// read back from the kernel's staging slab.
 HCTR_DEVICE void epilogue_chunk(const GemmParams& p, const int flags, const int m, const bool row_ok,
                                 const int n0, const uint32_t (&r)[32]) {
         if (n0 >= p.N) return;  // warp-uniform
@@ -192,116 +190,49 @@ HCTR_DEVICE void epilogue_chunk(const GemmParams& p, const int flags, const int 
   }
 }
 
+
 // ---------------------------------------------------------------------------------------------
-// TMA-staged epilogue (gemm_tc2.cu).  The direct epilogue above is one thread per row: every 16-byte
-// global access of a warp touches 32 different cache lines, so operand-reading / large-N epilogues
-// are bound by L1TEX wavefronts, not by DRAM.  Here every epilogue warp owns a [32 rows x 64 cols]
-// bf16 slab in shared memory (128-byte rows, SWIZZLE_128B): outputs are written to the slab and
-// leave through cp.async.bulk.tensor stores, the x0 / xl / mask operands arrive in such slabs through
-// TMA loads issued one tile ahead.  Out-of-range rows / columns are clipped (stores) or zero filled
-// (loads) by the TMA unit, so there is no ragged-edge code at all.
-//   EK_GENERIC: out = act(alpha * acc + bias)                       act in {id, relu, sigmoid}
-//   EK_CROSS:   aux = alpha * acc + bias ; out = x0 * aux + xl      (aux store optional)
-//   EK_ADD:     out = alpha * acc + bias + xl
-//   EK_MASK:    out = (alpha * acc + bias) * (mask > 0)
-enum EpiKind : int { EK_GENERIC = 0, EK_CROSS = 1, EK_ADD = 2, EK_MASK = 3 };
+// Epilogue of one warpgroup's m64 x BN wgmma accumulator tile (layout in wgmma.cuh): 64-column groups go
+// through a [64 x kStagePitch] fp32 staging slab in shared memory so that every thread then owns one row
+// x 32 consecutive columns for epilogue_chunk.  `slab` is private to the warpgroup (named barrier 1 + wg).
+constexpr int kStagePitch = 64 + 4;  // fp32 words per staged row (+4: conflict-free 16-byte reads)
+constexpr int kEpiSlabBytes = 64 * kStagePitch * 4;
 
-// host-side classification of a flag word; -1: not expressible by the TMA epilogue
-inline int epi_kind_of(int flags, const void* addf) {
-  if (flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)) return -1;
-  if (addf != nullptr) return -1;
-  const int op = flags & (EPI_CROSS | EPI_ADD | EPI_MASK);
-  const int act = flags & (EPI_RELU | EPI_SIGMOID);
-  if (op == 0) return EK_GENERIC;
-  if (act) return -1;
-  if (op == EPI_CROSS) return EK_CROSS;
-  if (op == EPI_ADD) return EK_ADD;
-  if (op == EPI_MASK) return EK_MASK;
-  return -1;
+HCTR_DEVICE void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
-// 16-byte chunk k (0..7) of row `row` inside a 128B-swizzled slab
-HCTR_DEVICE uint32_t slab_off(int row, int k) { return row * 128 + ((k ^ (row & 7)) << 4); }
-
-HCTR_DEVICE uint4 lds_v4(uint32_t addr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr));
-  return v;
-}
-HCTR_DEVICE void sts_v4(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-// One 32-column chunk: accumulators r[] -> slab `st_out` (and `st_aux` for the cross pre-activation),
-// operands from slabs `ld_a` / `ld_b`.  `half` selects the 64-byte half of the 128-byte slab row.
-template <int KIND>
-HCTR_DEVICE void epilogue_chunk_tma(const GemmParams& p, const int flags, const int lane, const int n0,
-                                    const int half, const uint32_t (&r)[32], const uint32_t st_out,
-                                    const uint32_t st_aux, const uint32_t ld_a, const uint32_t ld_b) {
-  float v[32];
+template <int BN>
+HCTR_DEVICE void epilogue_tile_wg(const GemmParams& p, const int flags, const float (&acc)[BN / 2], uint32_t* slab,
+                                  const int m_base, const int n_base, const int wg) {
+  const int w4 = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int erow = (w4 & 1) * 32 + lane;
+  const int m = m_base + erow;
+  const bool row_ok = m < p.M;
+  const int r0 = w4 * 16 + (lane >> 2);
+  const int c = w4 >> 1;
 #pragma unroll
-  for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) * p.alpha;
-  if (p.bias != nullptr) {
-    if (n0 + 32 <= p.N) {
+  for (int g = 0; g < BN / 64; ++g) {
+    named_bar_sync(1 + wg, 128);  // the slab's previous readers are done
 #pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + j));
-        v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (n0 + j < p.N) v[j] += __ldg(p.bias + n0 + j);
+    for (int j = 0; j < 8; ++j) {
+      const int col = 8 * j + 2 * (lane & 3);
+      const float* a4 = acc + (8 * g + j) * 4;
+      *reinterpret_cast<uint2*>(slab + r0 * kStagePitch + col) =
+          make_uint2(__float_as_uint(a4[0]), __float_as_uint(a4[1]));
+      *reinterpret_cast<uint2*>(slab + (r0 + 8) * kStagePitch + col) =
+          make_uint2(__float_as_uint(a4[2]), __float_as_uint(a4[3]));
     }
+    named_bar_sync(1 + wg, 128);
+    uint32_t r[32];
+    const uint4* src = reinterpret_cast<const uint4*>(slab + erow * kStagePitch + c * 32);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+      const uint4 v = src[q];
+      r[4 * q] = v.x; r[4 * q + 1] = v.y; r[4 * q + 2] = v.z; r[4 * q + 3] = v.w;
+    }
+    epilogue_chunk(p, flags, m, row_ok, n_base + g * 64 + c * 32, r);
   }
-  if constexpr (KIND == EK_CROSS) {
-    if (st_aux != 0) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        sts_v4(st_aux + slab_off(lane, half * 4 + j),
-               make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                          pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7])));
-    }
-  }
-  if constexpr (KIND != EK_GENERIC) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint4 a = make_uint4(0, 0, 0, 0), b = make_uint4(0, 0, 0, 0);
-      if constexpr (KIND == EK_CROSS || KIND == EK_MASK) a = lds_v4(ld_a + slab_off(lane, half * 4 + j));
-      if constexpr (KIND == EK_CROSS || KIND == EK_ADD) b = lds_v4(ld_b + slab_off(lane, half * 4 + j));
-      const uint32_t aw[4] = {a.x, a.y, a.z, a.w};
-      const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float& lo = v[8 * j + 2 * q];
-        float& hi = v[8 * j + 2 * q + 1];
-        if constexpr (KIND == EK_CROSS) {
-          lo = bf16_lo(aw[q]) * lo + bf16_lo(bw[q]);
-          hi = bf16_hi(aw[q]) * hi + bf16_hi(bw[q]);
-        } else if constexpr (KIND == EK_ADD) {
-          lo += bf16_lo(bw[q]);
-          hi += bf16_hi(bw[q]);
-        } else {
-          if (!(bf16_lo(aw[q]) > 0.f)) lo = 0.f;
-          if (!(bf16_hi(aw[q]) > 0.f)) hi = 0.f;
-        }
-      }
-    }
-  } else {
-    if (flags & EPI_RELU) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-    }
-    if (flags & EPI_SIGMOID) {
-#pragma unroll
-      for (int j = 0; j < 32; ++j) v[j] = 1.f / (1.f + __expf(-v[j]));
-    }
-  }
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    sts_v4(st_out + slab_off(lane, half * 4 + j),
-           make_uint4(pack_bf16x2(v[8 * j], v[8 * j + 1]), pack_bf16x2(v[8 * j + 2], v[8 * j + 3]),
-                      pack_bf16x2(v[8 * j + 4], v[8 * j + 5]), pack_bf16x2(v[8 * j + 6], v[8 * j + 7])));
 }
 
 }  // namespace hctr

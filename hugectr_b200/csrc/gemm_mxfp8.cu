@@ -1,17 +1,16 @@
-// D1-fp8: block-scaled (MX) fp8 GEMM on the 5th-generation tensor cores.
+// D1-fp8: block-scaled (MX) fp8 GEMM on Hopper tensor cores.
 //   out[M, N] (bf16 / fp32) = epilogue( sum_k  (A_q[m, k] * 2^(SFA[m, k/32] - 127)) * (B_q[n, k] * 2^(SFB[n, k/32] - 127)) )
 // A_q [M, K], B_q [N, K]: e4m3, K-major.  SFA / SFB: one UE8M0 scale per 32 consecutive K elements (OCP MX
-// format), applied by the tensor core itself: `tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale` reads the
-// scales from TENSOR MEMORY next to the accumulator.  Pipeline per CTA (one 128 x 128 output tile):
-//   warp 0   TMA producer: A / B tiles (128 rows x 128 bytes, SWIZZLE_128B) + the 512-byte scale blocks of the
-//            k-block (1-D bulk copies) into a 4-stage ring, completion on the stage's mbarrier
-//   warp 1   one elected thread: `tcgen05.cp.32x128b.warpx4` moves the two scale blocks smem -> TMEM, then four
-//            K = 32 MMAs with scale-factor id 0..3 (the byte of the 32-bit TMEM column that holds the scale of this
-//            32-wide slice); tcgen05.commit releases the stage / publishes the accumulator
-//   warps 4-7 epilogue: tcgen05.ld 32 x 32 columns -> bias / ReLU / ... -> global
-// Scale layout in global memory = the layout the copy needs, so a k-block's scales are ONE contiguous 512-byte
-// block per 128 rows:  block (row / 128, k / 128), byte offset (row % 32) * 16 + ((row % 128) / 32) * 4 + (k % 128) / 32
-// (row r of the tile lands in TMEM lane r % 32 -- replicated to the 4 sub-partitions --, 32-bit column (r % 128) / 32).
+// format).  Hopper's fp8 wgmma has no block scaling, and one m64n128k32 wgmma covers exactly one 32-wide scale
+// slice, so every slice is accumulated into a temporary register tile and promoted into the fp32 accumulator
+// with the product of its row and column scales (powers of two: the promotion is exact up to fp32 rounding).
+// CTA (one 128 x 128 output tile) = three warpgroups:
+//   warpgroup 0   TMA producer: A / B tiles (128 rows x 128 bytes, SWIZZLE_128B) + the 512-byte scale blocks of
+//                 the k-block (1-D bulk copies) into a ring of stages, completion on the stage's mbarrier
+//   warpgroups 1-2  64 rows each: 4 slices per k-block (wgmma -> wait -> scaled promotion), then the fused
+//                 epilogue (bias / ReLU / ...) through the shared staging slab
+// Scale layout in global memory: a k-block's scales are ONE contiguous 512-byte block per 128 rows:
+//   block (row / 128, k / 128), byte offset (row % 32) * 16 + ((row % 128) / 32) * 4 + (k % 128) / 32
 // The quantiser (mx_quantize_kernel) writes exactly this; it is the reference's cublasLt path replaced
 // (HugeCTR/src/layers/functors/fused_gemm_functors.cu:21-289 has no fp8 at all).
 #include <cuda_fp8.h>
@@ -20,10 +19,10 @@
 
 namespace hctr {
 
-constexpr int MX_BM = 128, MX_BN = 128, MX_BK = 128, MX_STAGES = 4, MX_THREADS = 256;
+constexpr int MX_BM = 128, MX_BN = 128, MX_BK = 128, MX_STAGES = 4, MX_THREADS = 384;
 constexpr int MX_TILE_BYTES = MX_BM * MX_BK;          // 16 KB (fp8)
 constexpr int MX_SF_BYTES = 512;
-constexpr int MX_SMEM = MX_STAGES * (2 * MX_TILE_BYTES + 2 * MX_SF_BYTES) + 1024 + 1024;
+constexpr int MX_SMEM = MX_STAGES * (2 * MX_TILE_BYTES + 2 * MX_SF_BYTES) + 2 * kEpiSlabBytes + 1024 + 1024;
 
 HCTR_DEVICE void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
@@ -31,34 +30,8 @@ HCTR_DEVICE void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, 
                "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
-// shared-memory matrix descriptor without swizzle: 8-row x 16-byte core matrices, rows 16 bytes apart
-HCTR_DEVICE uint64_t make_smem_desc_none(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  return d;
-}
-HCTR_DEVICE void utccp_32x128b_warpx4(uint32_t tmem_dst, uint64_t smem_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(tmem_dst), "l"(smem_desc) : "memory");
-}
-HCTR_DEVICE void umma_mxf8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate,
-                           uint32_t sfa_tmem, uint32_t sfb_tmem) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(sfa_tmem), "r"(sfb_tmem)
-      : "memory");
-}
-// block-scaled instruction descriptor (kind::mxf8f6f4): [4,6) b_sf_id  [7,10) a_format  [10,13) b_format
-// [15] a_major  [16] b_major  [17,23) N >> 3  [23] scale format (1 = UE8M0)  [24,29) M >> 4  [29,31) a_sf_id
-__host__ __device__ constexpr uint32_t make_idesc_mx(uint32_t M, uint32_t N) {
-  return (kFmtE4M3 << 7) | (kFmtE4M3 << 10) | ((N >> 3) << 17) | (1u << 23) | ((M >> 4) << 24);
-}
+// UE8M0 byte -> 2^(e - 127) (e = 0, i.e. 2^-127, flushes to zero)
+HCTR_DEVICE float ue8m0_to_float(uint32_t e) { return __uint_as_float(e << 23); }
 
 __global__ void __launch_bounds__(MX_THREADS, 1)
     gemm_mxfp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -69,12 +42,11 @@ __global__ void __launch_bounds__(MX_THREADS, 1)
   uint8_t* smem_b = smem + MX_STAGES * MX_TILE_BYTES;
   uint8_t* smem_sfa = smem + 2 * MX_STAGES * MX_TILE_BYTES;
   uint8_t* smem_sfb = smem_sfa + MX_STAGES * MX_SF_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem_sfb + MX_STAGES * MX_SF_BYTES);
+  uint32_t* epi = reinterpret_cast<uint32_t*>(smem_sfb + MX_STAGES * MX_SF_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi) + 2 * kEpiSlabBytes);
   uint64_t* empty_bar = full_bar + MX_STAGES;
-  uint64_t* tmem_full = empty_bar + MX_STAGES;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_full + 1);
 
-  const int warp_idx = threadIdx.x >> 5;
+  const int wg = threadIdx.x >> 7, warp_idx = threadIdx.x >> 5;
   const int n_blk = blockIdx.x, m_blk = blockIdx.y;
   const int k_blocks = p.k_blocks;
 
@@ -85,23 +57,15 @@ __global__ void __launch_bounds__(MX_THREADS, 1)
   if (warp_idx == 1 && elect_one()) {
     for (int i = 0; i < MX_STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);   // every consumer warp
     }
-    mbar_init(tmem_full, 1);
     fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    tmem_alloc(tmem_ptr, 256);       // 128 accumulator columns + 2 x 4 scale columns
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t tmem_sfa = tmem_base + 128, tmem_sfb = tmem_base + 132;
 
-  if (warp_idx == 0) {
-    if (elect_one()) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp_idx == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int kb = 0; kb < k_blocks; ++kb) {
@@ -119,53 +83,52 @@ __global__ void __launch_bounds__(MX_THREADS, 1)
         }
       }
     }
-  } else if (warp_idx == 1) {
-    constexpr uint32_t idesc0 = make_idesc_mx(MX_BM, MX_BN);
+  } else {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;
+    const int w4 = warp_idx & 3, lane = threadIdx.x & 31;
+    const int row0 = cw * 64 + w4 * 16 + (lane >> 2);   // tile rows row0 and row0 + 8
+    float acc[64], part[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
     int stage = 0;
     uint32_t phase = 0;
     for (int kb = 0; kb < k_blocks; ++kb) {
       mbar_wait(&full_bar[stage], phase);
-      tc_fence_after();
-      if (elect_one()) {
-        utccp_32x128b_warpx4(tmem_sfa, make_smem_desc_none(smem_u32(smem_sfa + stage * MX_SF_BYTES), 16, 128));
-        utccp_32x128b_warpx4(tmem_sfb, make_smem_desc_none(smem_u32(smem_sfb + stage * MX_SF_BYTES), 16, 128));
-        const uint64_t a_desc = make_smem_desc_sw128(smem_u32(smem_a + stage * MX_TILE_BYTES), 16, 1024);
-        const uint64_t b_desc = make_smem_desc_sw128(smem_u32(smem_b + stage * MX_TILE_BYTES), 16, 1024);
+      const uint64_t a_desc = make_smem_desc_sw128(smem_u32(smem_a + stage * MX_TILE_BYTES) + cw * (64 * 128), 16, 1024);
+      const uint64_t b_desc = make_smem_desc_sw128(smem_u32(smem_b + stage * MX_TILE_BYTES), 16, 1024);
+      const uint8_t* sa = smem_sfa + stage * MX_SF_BYTES;
+      const uint8_t* sb = smem_sfb + stage * MX_SF_BYTES;
 #pragma unroll
-        for (int k = 0; k < MX_BK / 32; ++k) {
-          const uint32_t idesc = idesc0 | (static_cast<uint32_t>(k) << 4) | (static_cast<uint32_t>(k) << 29);
-          umma_mxf8(tmem_base, a_desc + static_cast<uint64_t>(k * 2), b_desc + static_cast<uint64_t>(k * 2), idesc,
-                    (kb > 0 || k > 0) ? 1u : 0u, tmem_sfa, tmem_sfb);
+      for (int k = 0; k < MX_BK / 32; ++k) {
+        wgmma_fence_regs(part);
+        wgmma_fence();
+        wgmma_e4m3_n128(part, a_desc + static_cast<uint64_t>(k * 2), b_desc + static_cast<uint64_t>(k * 2), 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(part);
+        const float s0 = ue8m0_to_float(sa[(row0 & 31) * 16 + (row0 >> 5) * 4 + k]);
+        const float s1 = ue8m0_to_float(sa[((row0 + 8) & 31) * 16 + ((row0 + 8) >> 5) * 4 + k]);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * j + 2 * (lane & 3) + e;
+            const float sc = ue8m0_to_float(sb[(col & 31) * 16 + (col >> 5) * 4 + k]);
+            acc[4 * j + e] = fmaf(part[4 * j + e], s0 * sc, acc[4 * j + e]);
+            acc[4 * j + 2 + e] = fmaf(part[4 * j + 2 + e], s1 * sc, acc[4 * j + 2 + e]);
+          }
         }
-        umma_commit(&empty_bar[stage]);
-        if (kb == k_blocks - 1) umma_commit(tmem_full);
       }
       __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
       if (++stage == MX_STAGES) {
         stage = 0;
         phase ^= 1;
       }
     }
-  } else if (warp_idx >= 4) {
-    const int ew = warp_idx - 4;
-    const int lane = threadIdx.x & 31;
-    const int m = m_blk * MX_BM + ew * 32 + lane;
-    const bool row_ok = m < p.M;
-    mbar_wait(tmem_full, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c = 0; c < MX_BN / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_base + c * 32 + (static_cast<uint32_t>(ew * 32) << 16), r);
-      tmem_ld_wait();
-      epilogue_chunk(p, p.flags, m, row_ok, n_blk * MX_BN + c * 32, r);
-    }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
+    epilogue_tile_wg<MX_BN>(p, p.flags, acc, epi + cw * (kEpiSlabBytes / 4), m_blk * MX_BM + cw * 64,
+                            n_blk * MX_BN, cw);
   }
 }
 
@@ -255,7 +218,7 @@ extern "C" int hctr_mx_quantize(const void* x, long long ldx, void* q, void* sf,
   const int rows_pad = (rows + 127) / 128 * 128;
   const long long total = static_cast<long long>(rows_pad) * (cols / 32);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > num_sms() * 16) blocks = num_sms() * 16;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
   if (is_bf16)
     mx_quantize_kernel<__nv_bfloat16><<<static_cast<unsigned>(blocks), 256, 0, st>>>(

@@ -1,4 +1,4 @@
-// D1 / D3: persistent warp-specialised bf16 GEMM on 5th-gen tensor cores (tcgen05.mma, TMEM
+// D1 / D3: persistent warp-specialised bf16 GEMM on Hopper tensor cores (wgmma.mma_async, register
 // accumulators, TMA operand staging, mbarrier pipelines) with fused epilogues:
 //   bias + ReLU            (MLP fprop;       replaces cuBLASLt RELU_AUX_BIAS epilogue,
 //                           reference HugeCTR/src/layers/functors/fused_gemm_functors.cu:21-289)
@@ -7,6 +7,11 @@
 //   x0 * (acc + b) + xl    (DCNv2 cross;     reference HugeCTR/src/layers/multi_cross_layer.cu:625-672)
 // Operands may be K-major or MN-major, so fprop (X*W, W=[in,out]), dgrad (dY*W^T) and wgrad
 // (X^T*dY) all run from the same row-major tensors without any transposed copies.
+//
+// CTA = three warpgroups: warpgroup 0 is the TMA producer, warpgroups 1 and 2 each own 64 rows of the
+// 128 x BN tile (one m64nBNk16 wgmma per 16-wide K step) and run the epilogue of their rows.  The
+// accumulators leave the registers through a per-warpgroup [64 x 64] fp32 staging slab, so the fused
+// epilogue works on one row x 32 columns per thread with vectorised global accesses.
 #include <cstdio>
 
 #include "gemm_epilogue.cuh"
@@ -15,23 +20,31 @@ namespace hctr {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one SWIZZLE_128B row
-constexpr int UMMA_K = 16;
-constexpr int kNumThreads = 256;
-constexpr int kEpiWarp0 = 4;
+constexpr int WG_K = 16;
+constexpr int kNumThreads = 384;
+constexpr int kSmemLimit = 232448;  // 227 KB opt-in shared memory per block on sm_90
 
 template <int BN>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BN * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
+  static constexpr int kEpiBytes = 2 * kEpiSlabBytes;
   static constexpr int kBarBytes = 1024;
-  static constexpr int kTotal = kStages * kStageBytes + kBarBytes + 1024;  // +1024 align slack
+  static constexpr int kFit = (kSmemLimit - kEpiBytes - kBarBytes - 1024) / kStageBytes;
+  static constexpr int kStages = kFit < 8 ? kFit : 8;
+  static constexpr int kTotal = kStages * kStageBytes + kEpiBytes + kBarBytes + 1024;  // +1024 align slack
 };
 
+template <int BN, int TA, int TB>
+HCTR_DEVICE void wgmma_tile(float (&acc)[BN / 2], uint64_t a, uint64_t b, uint32_t accumulate) {
+  if constexpr (BN == 64) wgmma_bf16_n64<TA, TB>(acc, a, b, accumulate);
+  else if constexpr (BN == 128) wgmma_bf16_n128<TA, TB>(acc, a, b, accumulate);
+  else wgmma_bf16_n256<TA, TB>(acc, a, b, accumulate);
+}
+
 // MC == 2: thread-block cluster of two CTAs stacked along M that share the B tile -- each CTA loads
-// half of it and TMA-multicasts it into both shared memories (halves the L2->SM operand traffic of
-// B; the kernel is L2-bandwidth bound at CTR shapes, see profiles/).
+// half of it and TMA-multicasts it into both shared memories (halves the L2->SM operand traffic of B).
 template <int BN, bool A_MN, bool B_MN, int MC>
 __global__ void __launch_bounds__(kNumThreads, 1)
     gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -43,13 +56,12 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * L::kABytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * L::kStageBytes);
+  uint32_t* epi = reinterpret_cast<uint32_t*>(smem + kStages * L::kStageBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * L::kStageBytes + L::kEpiBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
-  uint64_t* tmem_full = bars + 2 * kStages;
-  uint64_t* tmem_empty = bars + 2 * kStages + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * kStages + 4);
 
+  const int wg = threadIdx.x >> 7;
   const int warp_idx = threadIdx.x >> 5;
   // work items are (m-group of MC tiles, n tile, k split); the CTAs of a cluster take the MC
   // consecutive m tiles of one item
@@ -66,27 +78,17 @@ __global__ void __launch_bounds__(kNumThreads, 1)
   if (warp_idx == 1 && elect_one()) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], MC);   // every CTA of the cluster must have drained the slot
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[i], 8 * MC);  // every consumer warp of every CTA of the cluster
     }
     fence_barrier_init();
   }
-  if (warp_idx == 2) {
-    tmem_alloc(tmem_ptr, 2 * BN);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (MC > 1) cluster_sync_all();   // peers' barriers are initialised before any remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  if constexpr (MC > 1) cluster_sync_all();  // peers' barriers are initialised before any remote arrive
 
-  if (warp_idx == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (elect_one()) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp_idx == 0 && elect_one()) {
       int stage = 0;
       uint32_t phase = 0;
       for (int t = cluster_id; t < total_tiles; t += num_clusters) {
@@ -122,10 +124,14 @@ __global__ void __launch_bounds__(kNumThreads, 1)
             constexpr uint16_t kMask = (1u << MC) - 1;
             if constexpr (B_MN) {
               constexpr int kChunks = BN / 64 / MC;
+              if constexpr (kChunks > 0) {
 #pragma unroll
-              for (int c = 0; c < kChunks; ++c) {
-                const int cc = cta_rank * kChunks + c;
-                tma_load_2d_mc(sb + cc * (BLOCK_K * 128), &tmB, &full_bar[stage], n0 + cc * 64, k0, kMask);
+                for (int c = 0; c < kChunks; ++c) {
+                  const int cc = cta_rank * kChunks + c;
+                  tma_load_2d_mc(sb + cc * (BLOCK_K * 128), &tmB, &full_bar[stage], n0 + cc * 64, k0, kMask);
+                }
+              } else if (cta_rank == 0) {  // BN == 64: one chunk, fetched by the first CTA
+                tma_load_2d_mc(sb, &tmB, &full_bar[stage], n0, k0, kMask);
               }
             } else {
               constexpr int kRowsPer = BN / MC;
@@ -140,96 +146,71 @@ __global__ void __launch_bounds__(kNumThreads, 1)
         }
       }
     }
-  } else if (warp_idx == 1) {
-    // ===================== MMA issuer (single elected thread) =====================
-    constexpr uint32_t idesc =
-        make_idesc(kFmtBF16, kFmtBF16, A_MN ? 1u : 0u, B_MN ? 1u : 0u, BLOCK_M, BN);
+  } else {
+    // ===================== wgmma consumers + epilogue (64 rows each) =====================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int cw = wg - 1;                       // 0 / 1: rows [64 cw, 64 cw + 64) of the tile
+    const int lane = threadIdx.x & 31;
+    uint32_t* slab = epi + cw * (kEpiSlabBytes / 4);
+    const int flags = p.flags;
     int stage = 0;
     uint32_t phase = 0;
-    int as = 0;
-    uint32_t aphase = 0;
+    float acc[BN / 2];
     for (int t = cluster_id; t < total_tiles; t += num_clusters) {
+      const int n_blk = t % p.n_tiles;
+      const int m_blk = ((t / p.n_tiles) % m_groups) * MC + cta_rank;
       const int split = t / (p.n_tiles * m_groups);
       const int kb0 = split * p.kb_per_split;
       const int kb1 = min(p.k_blocks, kb0 + p.kb_per_split);
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + as * BN;
+      int prev = -1;
       for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a_addr = smem_u32(smem_a + stage * L::kABytes);
-          const uint32_t b_addr = smem_u32(smem_b + stage * L::kBBytes);
-          // K-major SW128 : 8-row atoms of 1024 B ; MN-major SW128: 64-wide chunks BLOCK_K*128 B
-          // apart (LBO), 8-k-row groups 1024 B apart (SBO)
-          const uint64_t a_desc = A_MN ? make_smem_desc_sw128(a_addr, BLOCK_K * 128, 1024)
-                                       : make_smem_desc_sw128(a_addr, 16, 1024);
-          const uint64_t b_desc = B_MN ? make_smem_desc_sw128(b_addr, BLOCK_K * 128, 1024)
-                                       : make_smem_desc_sw128(b_addr, 16, 1024);
-          constexpr uint32_t a_step = A_MN ? (UMMA_K * 128) >> 4 : (UMMA_K * 2) >> 4;
-          constexpr uint32_t b_step = B_MN ? (UMMA_K * 128) >> 4 : (UMMA_K * 2) >> 4;
+        const uint32_t a_addr = smem_u32(smem_a + stage * L::kABytes) + cw * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem_b + stage * L::kBBytes);
+        // K-major SW128 : 8-row atoms of 1024 B ; MN-major SW128: 64-wide chunks BLOCK_K*128 B
+        // apart (LBO), 8-k-row groups 1024 B apart (SBO)
+        const uint64_t a_desc = A_MN ? make_smem_desc_sw128(a_addr, BLOCK_K * 128, 1024)
+                                     : make_smem_desc_sw128(a_addr, 16, 1024);
+        const uint64_t b_desc = B_MN ? make_smem_desc_sw128(b_addr, BLOCK_K * 128, 1024)
+                                     : make_smem_desc_sw128(b_addr, 16, 1024);
+        constexpr uint32_t a_step = A_MN ? (WG_K * 128) >> 4 : (WG_K * 2) >> 4;
+        constexpr uint32_t b_step = B_MN ? (WG_K * 128) >> 4 : (WG_K * 2) >> 4;
+        wgmma_fence_regs(acc);
+        wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            umma_f16(d_tmem, a_desc + static_cast<uint64_t>(k * a_step),
-                     b_desc + static_cast<uint64_t>(k * b_step), idesc,
-                     (kb > kb0 || k > 0) ? 1u : 0u);
+        for (int k = 0; k < BLOCK_K / WG_K; ++k)
+          wgmma_tile<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, a_desc + static_cast<uint64_t>(k * a_step),
+                                                      b_desc + static_cast<uint64_t>(k * b_step),
+                                                      (kb > kb0 || k > 0) ? 1u : 0u);
+        wgmma_commit();
+        wgmma_fence_regs(acc);
+        if (prev >= 0) {
+          wgmma_wait<1>();  // the previous k block's wgmma has finished reading its slot
+          if (lane == 0) {
+            if constexpr (MC == 1) mbar_arrive(&empty_bar[prev]);
+            else
+              for (int r = 0; r < MC; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
           }
-          if constexpr (MC == 1) umma_commit(&empty_bar[stage]);   // frees the smem slot
-          else umma_commit_mc(&empty_bar[stage], (1u << MC) - 1);  // ... in every CTA of the cluster
-          if (kb == kb1 - 1) umma_commit(&tmem_full[as]);   // accumulator ready
         }
-        __syncwarp();
+        prev = stage;
         if (++stage == kStages) {
           stage = 0;
           phase ^= 1;
         }
       }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && lane == 0) {
+        if constexpr (MC == 1) mbar_arrive(&empty_bar[prev]);
+        else
+          for (int r = 0; r < MC; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
       }
-    }
-  } else if (warp_idx >= kEpiWarp0) {
-    // ===================== epilogue: TMEM -> regs -> fused math -> global =====================
-    const int ew = warp_idx - kEpiWarp0;  // == warp_idx % 4 : TMEM lane quarter
-    const int lane = threadIdx.x & 31;
-    int as = 0;
-    uint32_t aphase = 0;
-    const int flags = p.flags;
-    for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-      const int n_blk = t % p.n_tiles;
-      const int m_blk = ((t / p.n_tiles) % m_groups) * MC + cta_rank;
-      const int m = m_blk * BLOCK_M + ew * 32 + lane;
-      const bool row_ok = m < p.M;
-      mbar_wait(&tmem_full[as], aphase);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        const int n0 = n_blk * BN + c * 32;
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + as * BN + c * 32 + (static_cast<uint32_t>(ew * 32) << 16), r);
-        tmem_ld_wait();
-        epilogue_chunk(p, flags, m, row_ok, n0, r);
-      }
-      // all TMEM reads of this accumulator stage are complete -> hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[as]);
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
+      epilogue_tile_wg<BN>(p, flags, acc, slab, m_blk * BLOCK_M + cw * 64, n_blk * BN, cw);
     }
   }
 
-  tc_fence_before();
   __syncthreads();
-  if constexpr (MC > 1) cluster_sync_all();   // no CTA may exit while a peer can still multicast into it
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 2 * BN);
-  }
+  if constexpr (MC > 1) cluster_sync_all();  // no CTA may exit while a peer can still multicast into it
 }
 
 // ------------------------------------------------------------------ host side
@@ -267,8 +248,6 @@ static int make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t inner, uint6
   return r == CUDA_SUCCESS ? 0 : -2;
 }
 
-static int g_num_sms = 0;
-
 template <int BN, bool A_MN, bool B_MN, int MC>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
                   cudaStream_t stream) {
@@ -283,7 +262,7 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams
   }
   const int m_groups = (p.m_tiles + MC - 1) / MC;
   const int total = m_groups * p.n_tiles * p.splits;       // cluster work items
-  int clusters = g_num_sms / MC;
+  int clusters = num_sms() / MC;
   if (total < clusters) clusters = total;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(clusters * MC);
@@ -308,6 +287,8 @@ using namespace hctr;
 // A: a_mn ? [K, M] row-major (lda) : [M, K] row-major (lda)
 // B: b_mn ? [K, N] row-major (ldb) : [N, K] row-major (ldb)
 // out: [M, N] row-major (ldo) bf16 (default) or fp32 (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)
+// block_n: BN in {64, 128, 256} (one CTA per tile) or 1000 + BN (2-CTA cluster sharing the B tile); other codes
+// >= 1000 are rejected (rc -11)
 extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
                               long long lda, long long ldb, long long ldo, int a_mn, int b_mn,
                               const float* bias, const void* mask, long long ldmask,
@@ -315,14 +296,10 @@ extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, in
                               long long ldaux, float alpha, int flags, int splits, int block_n,
                               const float* addf, long long ldaddf, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (g_num_sms == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&g_num_sms, cudaDevAttrMultiProcessorCount, dev);
-  }
   if (M <= 0 || N <= 0 || K <= 0) return 0;
-  const int mc = (block_n >= 1000) ? 2 : 1;   // block_n = 1000 + BN selects the 2-CTA multicast kernel
-  if (block_n >= 1000) block_n -= 1000;
+  if (block_n >= 2000) return -11;
+  const int mc = (block_n >= 1000) ? 2 : 1;
+  block_n %= 1000;
   const int BN = (block_n == 256 || block_n == 64) ? block_n : 128;
   GemmParams p;
   p.M = M; p.N = N; p.K = K;
@@ -339,7 +316,6 @@ extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, in
   p.x0 = reinterpret_cast<const __nv_bfloat16*>(x0);
   p.xl = reinterpret_cast<const __nv_bfloat16*>(xl); p.ldx = ldx;
   p.alpha = alpha; p.flags = flags; p.addf = addf; p.ldaddf = ldaddf;
-  p.colsum = nullptr;
 
   CUtensorMap ta, tb;
   int rc;
@@ -360,6 +336,7 @@ extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, in
   }
   if (mc == 2) {
     if (BN == 256) { HCTR_DISPATCH(256, 2) }
+    if (BN == 64) { HCTR_DISPATCH(64, 2) }
     HCTR_DISPATCH(128, 2)
   }
   if (BN == 256) { HCTR_DISPATCH(256, 1) }

@@ -1,12 +1,13 @@
-// D2: DLRM dot-product interaction on tcgen05 (fwd + bwd), bf16, n <= 32 rows, D <= 128, D % 16 == 0.
+// D2: DLRM dot-product interaction on Hopper wgmma (fwd + bwd), bf16, n <= 32 rows, D <= 128, D % 16 == 0.
 //   fwd : out[s] = [ mlp[s] | strict lower triangle of X X^T (row-major) | 0 ],  X = [mlp[s]; emb[s]]
 //   bwd : dX = (G + G^T) X  with G the lower-triangular gradient matrix;  dmlp += dout[:, :D]
 // Reference: HugeCTR/src/layers/interaction_layer.cu:47-596 (Volta wmma 16x16x16, one warp per
-// sample).  Here FOUR samples share one UMMA tile: their (zero padded) 32-row blocks are stacked
-// into a 128-row operand that sits in shared memory in the canonical SWIZZLE_128B layout; one
-// 128x128xD tcgen05.mma produces all four 32x32 Gram blocks on the TMEM diagonal, the epilogue
-// warps read their own block with tcgen05.ld and store the triangle.  The backward builds a
-// block-diagonal (G+G^T) operand and multiplies it with the same X tile used as an MN-major B.
+// sample).  Here FOUR samples share one tile: their (zero padded) 32-row blocks are stacked into a
+// 128-row operand that sits in shared memory in the canonical SWIZZLE_128B layout.  Each of the two
+// warpgroups owns two samples (64 rows): one m64n64 wgmma chain with A = B = its 64 rows produces both
+// 32x32 Gram blocks on the diagonal, and the triangle is stored straight from the accumulator
+// fragments.  The backward builds a block-diagonal (G+G^T) operand and multiplies it with the same X
+// tile used as an MN-major B (m64n128 per warpgroup).
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -49,78 +50,62 @@ __global__ void __launch_bounds__(256, 2)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem_x = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                                ~static_cast<uintptr_t>(1023));
-  __shared__ uint64_t mma_bar;
-  __shared__ uint32_t tmem_slot;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0) {
-    tmem_alloc(&tmem_slot, 128);
-    tmem_relinquish();
-  }
-  if (threadIdx.x == 32) {
-    mbar_init(&mma_bar, 1);
-    fence_barrier_init();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  const uint32_t idesc = make_idesc(kFmtBF16, kFmtBF16, 0, 0, 128, 128);
+  const int wg = threadIdx.x >> 7, w4 = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int ntiles = (B + kSPT - 1) / kSPT;
   const int ntri = n * (n - 1) / 2;
-  uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int s0 = tile * kSPT;
     fill_x_tile(smem_x, mlp, emb, s0, B, n, D);
     fence_proxy_async();   // generic-proxy smem writes -> visible to the tensor-core (async) proxy
     __syncthreads();
-    if (warp == 1) {
-      if (elect_one()) {
-        const uint32_t base = smem_u32(smem_x);
-        for (int k = 0; k < (D >> 4); ++k) {
-          const uint32_t a = base + (k >> 2) * kHalfBytes + (k & 3) * 32;
-          const uint64_t d = make_smem_desc_sw128(a, 16, 1024);
-          umma_f16(tmem, d, d, idesc, k > 0 ? 1u : 0u);   // Z = X X^T : A and B are the same tile
-        }
-        umma_commit(&mma_bar);
+    // passthrough of the bottom-MLP output + zero pad column
+    for (int t = threadIdx.x; t < kSPT * D; t += blockDim.x) {
+      const int i = t / D, c = t - i * D, s = s0 + i;
+      if (s >= B) continue;
+      bf16* o = out + static_cast<long long>(s) * out_w;
+      if ((out_w & 7) == 0) {
+        if ((c & 7) == 0)
+          reinterpret_cast<int4*>(o)[c >> 3] =
+              ld_nc_v4(reinterpret_cast<const int4*>(mlp + static_cast<long long>(s) * D) + (c >> 3));
+      } else {
+        o[c] = mlp[static_cast<long long>(s) * D + c];
       }
-      __syncwarp();
+      if (c == 0) o[D + ntri] = __float2bfloat16(0.f);
     }
-    // warps 4..7: passthrough of the bottom-MLP output + zero pad column (overlaps the MMA)
-    if (warp >= 4) {
-      const int i = warp - 4, s = s0 + i;
-      if (s < B) {
-        const int4* src = reinterpret_cast<const int4*>(mlp + static_cast<long long>(s) * D);
-        bf16* o = out + static_cast<long long>(s) * out_w;
-        if ((out_w & 7) == 0) {
-          for (int c = lane; c < (D >> 3); c += 32) reinterpret_cast<int4*>(o)[c] = ld_nc_v4(src + c);
-        } else {
-          const bf16* sm = mlp + static_cast<long long>(s) * D;
-          for (int c = lane; c < D; c += 32) o[c] = sm[c];
-        }
-        if (lane == 0) o[D + ntri] = __float2bfloat16(0.f);
-      }
-    }
-    mbar_wait(&mma_bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    if (warp < 4) {
-      // TMEM lanes 32*warp.. hold sample `warp`; its Gram block is at columns 32*warp..
-      uint32_t r[32];
-      tmem_ld_32x32(tmem + (static_cast<uint32_t>(warp * 32) << 16) + warp * 32, r);
-      tmem_ld_wait();
-      const int s = s0 + warp, j = lane;
-      if (s < B && j < n && j > 0) {
-        bf16* o = out + static_cast<long long>(s) * out_w + D + j * (j - 1) / 2;
+    float acc[32];
+    {
+      const uint32_t base = smem_u32(smem_x) + wg * (64 * 128);
+      wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < 32; ++c)
-          if (c < j) o[c] = __float2bfloat16(__uint_as_float(r[c]));
+      for (int k = 0; k < 8; ++k) {              // D <= 128: at most 8 steps of 16
+        if (k >= (D >> 4)) break;
+        const uint64_t d = make_smem_desc_sw128(base + (k >> 2) * kHalfBytes + (k & 3) * 32, 16, 1024);
+        wgmma_bf16_n64<0, 0>(acc, d, d, k > 0 ? 1u : 0u);   // Z = X X^T : A and B are the same rows
+      }
+      wgmma_commit();
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    // rows 16 w4 + lane / 4 (+ 8) of this warpgroup's 64; the sample's Gram block is n8 blocks [4 h, 4 h + 4)
+    const int h = w4 >> 1, s = s0 + 2 * wg + h;
+    if (s < B) {
+      bf16* o = out + static_cast<long long>(s) * out_w + D;
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int i = (16 * w4 + (lane >> 2) + 8 * half) & 31;
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = 8 * jj + 2 * (lane & 3) + e;
+            const float v = h ? acc[16 + 4 * jj + 2 * half + e] : acc[4 * jj + 2 * half + e];
+            if (i < n && c < i) o[i * (i - 1) / 2 + c] = __float2bfloat16(v);
+          }
+        }
       }
     }
-    tc_fence_before();
-    __syncthreads();   // TMEM reads + smem tile consumed before the next tile overwrites them
-    tc_fence_after();
+    __syncthreads();   // smem tile consumed before the next tile overwrites it
   }
-  if (warp == 0) tmem_dealloc(tmem, 128);
 }
 
 __global__ void __launch_bounds__(256, 2)
@@ -131,25 +116,8 @@ __global__ void __launch_bounds__(256, 2)
   uint8_t* smem_x = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                                ~static_cast<uintptr_t>(1023));
   uint8_t* smem_g = smem_x + 2 * kHalfBytes;   // block-diagonal (G + G^T), K-major, 2 halves
-  __shared__ uint64_t mma_bar;
-  __shared__ uint32_t tmem_slot;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0) {
-    tmem_alloc(&tmem_slot, 128);
-    tmem_relinquish();
-  }
-  if (threadIdx.x == 32) {
-    mbar_init(&mma_bar, 1);
-    fence_barrier_init();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
-  // D[128, N=D] = A[128, K=128] (K-major) * B (MN-major: rows = K, 64-wide N chunks)
-  const uint32_t idesc = make_idesc(kFmtBF16, kFmtBF16, 0, 1, 128, static_cast<uint32_t>(D));
+  const int wg = threadIdx.x >> 7, w4 = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int ntiles = (B + kSPT - 1) / kSPT;
-  uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     const int s0 = tile * kSPT;
     fill_x_tile(smem_x, mlp, emb, s0, B, n, D);
@@ -185,60 +153,43 @@ __global__ void __launch_bounds__(256, 2)
     }
     fence_proxy_async();
     __syncthreads();
-    if (warp == 1) {
-      if (elect_one()) {
-        const uint32_t ga = smem_u32(smem_g), xb = smem_u32(smem_x);
-        for (int k = 0; k < 8; ++k) {            // K = 128 stacked rows
-          const uint64_t a = make_smem_desc_sw128(ga + (k >> 2) * kHalfBytes + (k & 3) * 32, 16, 1024);
-          const uint64_t b = make_smem_desc_sw128(xb + k * 2048, kHalfBytes, 1024);
-          umma_f16(tmem, a, b, idesc, k > 0 ? 1u : 0u);
-        }
-        umma_commit(&mma_bar);
+    // D[64 rows of this warpgroup, N = 128] = A[64, K = 128] (K-major) * B (MN-major: rows = K, 64-wide N chunks)
+    float acc[64];
+    {
+      const uint32_t ga = smem_u32(smem_g) + wg * (64 * 128), xb = smem_u32(smem_x);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {            // K = 128 stacked rows
+        const uint64_t a = make_smem_desc_sw128(ga + (k >> 2) * kHalfBytes + (k & 3) * 32, 16, 1024);
+        const uint64_t b = make_smem_desc_sw128(xb + k * 2048, kHalfBytes, 1024);
+        wgmma_bf16_n128<0, 1>(acc, a, b, k > 0 ? 1u : 0u);
       }
-      __syncwarp();
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
     }
-    mbar_wait(&mma_bar, phase);
-    phase ^= 1;
-    tc_fence_after();
-    if (warp < 4) {
-      const int s = s0 + warp, j = lane;
-      const bool ok = s < B && j < n;
-      bf16* dst = nullptr;
-      const bf16* pass = nullptr;
-      if (ok) {
-        if (j == 0) {
-          dst = dmlp + static_cast<long long>(s) * D;
-          pass = dout + static_cast<long long>(s) * out_w;
-        } else {
-          dst = demb + (static_cast<long long>(s) * (n - 1) + (j - 1)) * D;
-        }
-      }
-      for (int c0 = 0; c0 < D; c0 += 32) {
-        uint32_t r[32];
-        tmem_ld_32x32(tmem + (static_cast<uint32_t>(warp * 32) << 16) + c0, r);
-        tmem_ld_wait();
-        if (ok) {
 #pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            float v[8];
+    for (int half = 0; half < 2; ++half) {
+      const int row = 64 * wg + 16 * w4 + (lane >> 2) + 8 * half;
+      const int s = s0 + (row >> 5), j = row & 31;
+      if (s >= B || j >= n) continue;
+      bf16* dst = j == 0 ? dmlp + static_cast<long long>(s) * D
+                         : demb + (static_cast<long long>(s) * (n - 1) + (j - 1)) * D;
+      const bf16* pass = j == 0 ? dout + static_cast<long long>(s) * out_w : nullptr;
 #pragma unroll
-            for (int e = 0; e < 8; ++e) {
-              v[e] = __uint_as_float(r[q * 8 + e]);
-              if (pass) v[e] += __bfloat162float(pass[c0 + q * 8 + e]);
-            }
-            if (c0 + q * 8 < D)
-              *reinterpret_cast<uint4*>(dst + c0 + q * 8) =
-                  make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]),
-                             pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]));
-          }
+      for (int jj = 0; jj < 16; ++jj) {
+        const int c = 8 * jj + 2 * (lane & 3);
+        if (c >= D) continue;
+        float v0 = acc[4 * jj + 2 * half], v1 = acc[4 * jj + 2 * half + 1];
+        if (pass) {
+          v0 += __bfloat162float(pass[c]);
+          v1 += __bfloat162float(pass[c + 1]);
         }
+        *reinterpret_cast<uint32_t*>(dst + c) = pack_bf16x2(v0, v1);
       }
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
   }
-  if (warp == 0) tmem_dealloc(tmem, 128);
 }
 
 }  // namespace hctr
@@ -256,7 +207,7 @@ extern "C" int hctr_interaction_fwd(const void* mlp, const void* emb, void* out,
   }
   const int out_w = D + n * (n - 1) / 2 + 1;
   const int tiles = (B + kSPT - 1) / kSPT;
-  const int grid = tiles < 296 ? tiles : 296;
+  const int grid = tiles < 2 * num_sms() ? tiles : 2 * num_sms();
   interaction_fwd_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(
       (const bf16*)mlp, (const bf16*)emb, (bf16*)out, B, n, D, out_w);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
@@ -273,7 +224,7 @@ extern "C" int hctr_interaction_bwd(const void* mlp, const void* emb, const void
   }
   const int out_w = D + n * (n - 1) / 2 + 1;
   const int tiles = (B + kSPT - 1) / kSPT;
-  const int grid = tiles < 296 ? tiles : 296;
+  const int grid = tiles < 2 * num_sms() ? tiles : 2 * num_sms();
   interaction_bwd_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>(
       (const bf16*)mlp, (const bf16*)emb, (const bf16*)dout, (bf16*)dmlp, (bf16*)demb, B, n, D, out_w);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;

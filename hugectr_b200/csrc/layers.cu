@@ -11,6 +11,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ptx.cuh"
+
 namespace hctr {
 
 using bf16 = __nv_bfloat16;
@@ -433,7 +435,7 @@ __global__ void gru_gate_bwd_kernel(const float* __restrict__ dh, const float* _
 using namespace hctr;
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 #define OK() (cudaGetLastError() == cudaSuccess ? 0 : -1)
-static inline unsigned grid1(long long n, int threads = 256, long long cap = 148LL * 32) {
+static inline unsigned grid1(long long n, int threads = 256, long long cap = hctr::num_sms() * 32LL) {
   long long b = (n + threads - 1) / threads;
   if (b > cap) b = cap;
   return static_cast<unsigned>(b < 1 ? 1 : b);

@@ -1,5 +1,5 @@
 // Device side of the distributed exact AUC (hugectr_b200/metrics.py).  Pipeline per evaluation round, the
-// B200 reading of the reference's histogram -> pivots -> all-to-all -> local sort -> halo pipeline
+// GPU reading of the reference's histogram -> pivots -> all-to-all -> local sort -> halo pipeline
 // (HugeCTR/src/metrics.cu:1017-1240):
 //   1. auc_hist_kernel       every rank bins its (prediction, label) pairs by an order-preserving 20-bit key
 //                            of the fp32 prediction into positive / negative histograms (2 x 4 MB)
@@ -11,6 +11,8 @@
 // Memory per rank is O(N / W) + the histograms, never the whole evaluation set.
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "ptx.cuh"
 
 namespace hctr {
 
@@ -68,7 +70,7 @@ extern "C" int hctr_auc_hist(const float* pred, const float* label, long long n,
                              void* hist_neg, int bits, void* stream) {
   if (n <= 0) return 0;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > hctr::num_sms() * 16) blocks = hctr::num_sms() * 16;
   auc_hist_kernel<<<static_cast<unsigned>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       pred, label, n, reinterpret_cast<unsigned int*>(hist_pos), reinterpret_cast<unsigned int*>(hist_neg),
       32 - bits);
@@ -80,7 +82,7 @@ extern "C" int hctr_auc_partition(const float* pred, const float* label, long lo
                                   void* stream) {
   if (n <= 0) return 0;
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > hctr::num_sms() * 16) blocks = hctr::num_sms() * 16;
   auc_partition_kernel<<<static_cast<unsigned>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       pred, label, n, reinterpret_cast<const unsigned char*>(bin2dst), reinterpret_cast<unsigned int*>(cursors),
       send_pred, send_label, 32 - bits);

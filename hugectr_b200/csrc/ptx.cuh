@@ -1,4 +1,4 @@
-// Blackwell (sm_100a) PTX wrappers: mbarrier, TMA, tcgen05 (MMA / TMEM), peer-memory ld/st.
+// Hopper (sm_90a) PTX wrappers: mbarrier, TMA, clusters, wgmma (wgmma.cuh), peer-memory ld/st.
 // Hand-written inline PTX; no CUTLASS dependency.
 #pragma once
 #include <cuda.h>
@@ -30,6 +30,17 @@ HCTR_DEVICE bool elect_one() {
       "}\n"
       : "=r"(pred));
   return pred != 0;
+}
+
+// streaming multiprocessors of the current device: grid size of persistent / grid-stride kernels
+inline int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+  }
+  return n;
 }
 
 // ---------------------------------------------------------------- mbarrier
@@ -98,125 +109,17 @@ HCTR_DEVICE void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// tcgen05.commit that arrives on the mbarrier at the same offset in every CTA of cta_mask
-HCTR_DEVICE void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"(cta_mask)
-      : "memory");
-}
-
-HCTR_DEVICE void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-HCTR_DEVICE void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-HCTR_DEVICE void tma_store_wait_read() {
-  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
-}
-template <int N>
-HCTR_DEVICE void tma_store_wait() {
-  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
-}
-
-// ---------------------------------------------------------------- tcgen05 / TMEM
-HCTR_DEVICE void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-}
-HCTR_DEVICE void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-HCTR_DEVICE void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-HCTR_DEVICE void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-HCTR_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]   (kind::f16 : bf16/fp16 inputs, fp32 accumulate)
-HCTR_DEVICE void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                          uint32_t accumulate) {
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
+HCTR_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      ".reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
       : "memory");
 }
-// kind::f8f6f4 : e4m3/e5m2 inputs, fp32 accumulate (UMMA_K = 32)
-HCTR_DEVICE void umma_f8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t"
-      "}\n" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire
-HCTR_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-          smem_u32(bar))
-      : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns (one row per thread)
-HCTR_DEVICE void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-HCTR_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ------------------------------------------------------- UMMA descriptors
-// Shared-memory matrix descriptor, SWIZZLE_128B, sm_100 version field = 1.
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version (=1)
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-HCTR_DEVICE uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes,
-                                          uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 / kind::f8f6f4 (dense, fp32 accumulate)
-//   [4,6) c_format (1=F32)  [7,10) a_format  [10,13) b_format  [15] a_major  [16] b_major
-//   [17,23) N>>3   [24,29) M>>4           (major: 0 = K-major, 1 = MN-major)
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t a_fmt, uint32_t b_fmt, uint32_t a_mn,
-                                                   uint32_t b_mn, uint32_t M, uint32_t N) {
-  return (1u << 4) | (a_fmt << 7) | (b_fmt << 10) | (a_mn << 15) | (b_mn << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-constexpr uint32_t kFmtBF16 = 1;  // kind::f16 : 0 = F16, 1 = BF16, 2 = TF32
-constexpr uint32_t kFmtE4M3 = 0;  // kind::f8f6f4 : 0 = E4M3, 1 = E5M2
-constexpr uint32_t kFmtE5M2 = 1;
 
 // ------------------------------------------------------- misc
 HCTR_DEVICE uint32_t pack_bf16x2(float lo, float hi) {
@@ -257,3 +160,5 @@ HCTR_DEVICE void st_na_v4(void* p, const int4& v) {
 }
 
 }  // namespace hctr
+
+#include "wgmma.cuh"

@@ -9,6 +9,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "ptx.cuh"
+
 namespace hctr {
 
 struct SplitDesc {
@@ -83,7 +85,7 @@ extern "C" int hctr_raw_split(const void* raw, void* label, void* dense, void* k
                     dense_dim, sparse_cols, rec_bytes, key_bytes_in, key_bytes_out, dense_is_float};
   const long long total = static_cast<long long>(batch) * (label_dim + dense_dim + sparse_cols);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > hctr::num_sms() * 8) blocks = hctr::num_sms() * 8;
   hctr::raw_split_kernel<<<static_cast<unsigned>(blocks), 256, 2 * sparse_cols * sizeof(int),
                            reinterpret_cast<cudaStream_t>(stream)>>>(d);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;

@@ -566,7 +566,7 @@ class EmbeddingCollection:
                                           row_elems=b * H, src_stride=b * H, dst_stride=b * H, dst_rank=g))
         self._key_routes = routes
         self._key_routes_dev = E.routes_to_device(routes, self.device)
-        # bytes this rank stores into peers per step (roofline accounting, see profiles/)
+        # bytes this rank stores into peers per step (roofline accounting)
         kb = self._kb
         self.dispatch_key_bytes = sum(r.rows * r.row_elems * kb for r in routes if r.dst_rank != me)
 

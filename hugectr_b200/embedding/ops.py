@@ -484,7 +484,7 @@ def sparse_opt_reference(opt: Optimizer_t, w, s0, s1, g, hp, lr, step):
 
 
 def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: dict, lr_t, step_t,
-           num_sms: int = 148):
+           num_sms: int = 132):
     """Fused per-unique-row optimizer; consumes and clears the workspace."""
     if table.is_cuda:
         h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),
@@ -581,7 +581,7 @@ def bwd_index(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, ws, my_ran
 
 def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_pitch, key_bufs,
                       grad_bufs, batch, ws, hp: dict, lr_t, step_t, grad_scale=1.0, my_rank=0,
-                      nnz_bufs=None, num_sms: int = 148, key_bytes=4, act_bf16=True):
+                      nnz_bufs=None, num_sms: int = 132, key_bytes=4, act_bf16=True):
     """Fused gradient gather (local / peer loads) + duplicate reduction + optimizer."""
     p, kb, gbf = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch,
                               my_rank, nnz_bufs, key_bytes, act_bf16)

@@ -185,7 +185,7 @@ class DeviceLayout(Enum):
 class AllReduceAlgo(Enum):
     OneShot = 0
     NCCL = 1
-    # B200 extension: two-shot reduce-scatter/all-gather over peer memory (large buffers)
+    # extension: two-shot reduce-scatter/all-gather over peer memory (large buffers)
     TwoShot = 2
 
 

@@ -1,6 +1,6 @@
 """Layer / tensor / parameter-arena runtime.
 
-Design (B200-first, not a port of core23):
+Design (GPU-native, not a port of core23):
   * tensors are torch tensors with static shapes, pre-allocated at compile() so one training step
     is CUDA-graph capturable;
   * all trainable dense parameters live in ONE flat fp32 master buffer (+ flat fp32 wgrad, flat
@@ -9,7 +9,7 @@ Design (B200-first, not a port of core23):
     core23 "Weight"/"Wgrad" UnitaryBuffers, HugeCTR/include/network_buffer_channels.hpp and
     HugeCTR/src/pybind/model_compile.cpp:887-900);
   * every layer implements explicit fprop/bprop (reference Layer::fprop/bprop,
-    HugeCTR/include/layer.hpp:31-92); hot layers call the sm_100a kernels, the long tail derives
+    HugeCTR/include/layer.hpp:31-92); hot layers call the sm_90a kernels, the long tail derives
     bprop from torch autograd (``TorchLayer``).
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """The remaining dense layer inventory (SURVEY 2.2): shape ops, elementwise, reductions,
 normalisation, attention, GRU.  Views are zero-copy where the reference copies; elementwise hot
-ones (ReLU/Sigmoid/Concat) call the sm_100a kernels, the rest derive backward from autograd.
+ones (ReLU/Sigmoid/Concat) call the sm_90a kernels, the rest derive backward from autograd.
 File references are given per class.
 """
 from __future__ import annotations
@@ -16,7 +16,7 @@ from .base import Layer, TorchLayer, make_init
 
 
 class NativeTail(TorchLayer):
-    """Long-tail layer with hand-written sm_100a forward / backward kernels (csrc/layers.cu).  On CUDA the
+    """Long-tail layer with hand-written sm_90a forward / backward kernels (csrc/layers.cu).  On CUDA the
     native path runs (no at:: kernels, no autograd tape, graph capturable); on CPU -- and for inputs the
     kernels do not take (non-contiguous, integer) -- the PyTorch formulation of ``TorchLayer`` runs, which
     is also the oracle of the numerics tests."""

@@ -1,6 +1,6 @@
 """MultiCross (DCN v1 and low-rank DCN v2) and the DLRM dot Interaction layer.
 
-DCN v2 low-rank: x_{l+1} = x_0 * (x_l U_l V_l + b_l) + x_l   as two tcgen05 GEMMs per layer with the
+DCN v2 low-rank: x_{l+1} = x_0 * (x_l U_l V_l + b_l) + x_l   as two wgmma GEMMs per layer with the
 elementwise part fused into the second GEMM's epilogue (csrc/gemm_tc.cu EPI_CROSS); backward =
 4 GEMMs per layer + one fused elementwise kernel.  Reference: HugeCTR/src/layers/multi_cross_layer.cu
 (v1 :582-600/:698-731, v2 fwd :625-672, bwd :733-812, weights U[w,p],V[p,w],b per layer :857-886).

@@ -1,4 +1,4 @@
-"""MLP / InnerProduct / FusedInnerProduct on the tcgen05 GEMM with fused epilogues.
+"""MLP / InnerProduct / FusedInnerProduct on the wgmma GEMM with fused epilogues.
 
 Reference behaviour: HugeCTR/src/layers/mlp_layer.cu:25-298 (N x cuBLASLt matmul with bias+ReLU
 epilogue, DRELU_BGRAD dgrad, beta=1 wgrad on an overlap stream, skip_head_dgrad),
@@ -11,6 +11,7 @@ from typing import List
 
 import torch
 
+from ..core import KernelParams
 from ..enums import Activation_t
 from ..ops import dense as D
 from ..ops import gemm as G
@@ -62,7 +63,7 @@ class MLPLayer(Layer):
         self._out(0, self.lead + (self.dims_out[-1],))
         self._side = None
         # Solver.use_fp8_mlp: forward GEMMs in block-scaled fp8 (OCP MX: e4m3 values, one UE8M0 scale per 32
-        # K elements, applied inside tcgen05.mma.kind::mxf8f6f4.block_scale); backward stays bf16 on the
+        # K elements, applied per 32-wide K slice of the fp8 wgmma); backward stays bf16 on the
         # bf16 activations.  Layers whose K is not a multiple of 128 (or N == 1) keep the bf16 GEMM.
         self.fp8 = bool(getattr(ctx.solver, "use_fp8_mlp", False)) and ctx.mixed and ctx.native
 
@@ -198,8 +199,9 @@ class MLPLayer(Layer):
         K = x.shape[0]
         tiles = ((gW.shape[0] + 127) // 128) * ((gW.shape[1] + 127) // 128)
         splits = 1
-        if tiles < 148:
-            splits = max(1, min(8, 148 // max(tiles, 1), K // 512))
+        sms = KernelParams.init(x.device).num_sms
+        if tiles < sms:
+            splits = max(1, min(8, sms // max(tiles, 1), K // 512))
         G.gemm_bf16(x, dz, gW, a_mn=True, b_mn=True, flags=G.EPI_ATOMIC, splits=splits)
 
 

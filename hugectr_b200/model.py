@@ -452,8 +452,8 @@ class Model:
                 e.forward_begin()
             s_emb.wait_stream(main)
             s_idx.wait_stream(main)
-            # HCTR_BOTTOM_FIRST=1 enqueues the (tiny) bottom MLP before the embedding kernels; measured
-            # neutral on B200 (the block scheduler still runs the embedding forward first)
+            # HCTR_BOTTOM_FIRST=1 enqueues the (tiny) bottom MLP before the embedding kernels (the block
+            # scheduler may still run the embedding forward first)
             bottom_first = os.environ.get("HCTR_BOTTOM_FIRST", "0") == "1"
             if bottom_first:
                 net.fprop(True, "bottom")
@@ -578,7 +578,7 @@ class Model:
         self._graph.replay()
 
     def _aggressive_schedule(self) -> bool:
-        """Step-tail scheduling.  "aggressive" (validated on 1, 2 and 4 B200): bottom-network backward and the
+        """Step-tail scheduling.  "aggressive": bottom-network backward and the
         all-reduce buckets on streams above the embedding update's priority, no end-of-step device barrier
         (the next step's dispatch barrier orders the inbox reuse).  More than 4 ranks run the round-1 schedule
         (bottom backward on the main stream, default-priority communication streams, end-of-step barrier):

@@ -1,4 +1,4 @@
-"""bf16 tensor-core GEMM with fused epilogues (tcgen05/TMEM/TMA kernel in csrc/gemm_tc.cu).
+"""bf16 tensor-core GEMM with fused epilogues (wgmma/TMA kernel in csrc/gemm_tc.cu).
 
 ``gemm_bf16`` is the single entry point used by the MLP / InnerProduct / MultiCross layers for
 fprop, dgrad and wgrad.  On CPU (or for shapes TMA cannot address) it falls back to an fp32
@@ -37,8 +37,6 @@ def _lib():
             _c.c_void_p, _c.c_void_p, _c.c_longlong, _c.c_void_p, _c.c_void_p, _c.c_longlong,
             _c.c_void_p, _c.c_longlong, _c.c_float, _c.c_int, _c.c_int, _c.c_int, _c.c_void_p,
             _c.c_longlong, _c.c_void_p]
-        lib.hctr_gemm_bf16_2sm.restype = _c.c_int
-        lib.hctr_gemm_bf16_2sm.argtypes = lib.hctr_gemm_bf16.argtypes[:-1] + [_c.c_void_p, _c.c_void_p]
         _sig_set = True
     return lib
 
@@ -48,7 +46,7 @@ def _ptr(t):
 
 
 def tc_eligible(a: torch.Tensor, b: torch.Tensor, a_mn: bool, b_mn: bool) -> bool:
-    """TMA needs 16-byte aligned bases and row pitches; tcgen05 path is bf16 only."""
+    """TMA needs 16-byte aligned bases and row pitches; the wgmma path is bf16 only."""
     if not (a.is_cuda and a.dtype == torch.bfloat16 and b.dtype == torch.bfloat16):
         return False
     for t in (a, b):
@@ -91,7 +89,7 @@ def gemm_reference(a, b, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, 
 
 _bn_override = {}
 
-# "tc": the hand-written tcgen05 kernels (product path).  "library": bf16 GEMMs through torch.mm
+# "tc": the hand-written wgmma kernels (product path).  "library": bf16 GEMMs through torch.mm
 # (cuBLAS / cuBLASLt) with eager epilogues -- the stand-in baseline arm of bench.py, never a default.
 IMPL = "tc"
 _fallback_logged = set()
@@ -148,8 +146,8 @@ def gemm_library(a, b, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, xl
 
 
 def _pick_block_n(M, N, K, splits):
-    """Tile / cluster choice.  1000 + BN selects the 2-CTA cluster kernel that multicasts the B tile
-    (halves the L2->SM traffic of B; the GEMM is L2-bandwidth bound at these shapes)."""
+    """Tile / cluster choice.  1000 + BN selects the 2-CTA cluster kernel: the two CTAs take adjacent 128-row
+    tiles and multicast the shared B tile (halves the L2->SM traffic of B)."""
     import os
     ov = os.environ.get("HCTR_GEMM_BN")
     if ov:
@@ -159,15 +157,14 @@ def _pick_block_n(M, N, K, splits):
     m_t = (M + 127) // 128
     if m_t < 2:
         return 128
-    # Measured on B200 (profiles/gemm_microbench_*.jsonl): the cta_group::2 kernel (2000 + BN, one
-    # 256 x BN UMMA per CTA pair) beats the 1-SM kernel on every DLRM shape; the 256-wide pair tile
-    # is ~12 % more efficient per MAC but loses when it costs an extra wave.
+    # the 256-wide tile reads A half as often per MAC but loses when it costs an extra wave of the
+    # 66 cluster pairs of an H100 (132 SMs); the autotuner below times both on first sight of a shape
     def waves(bn):
         items = ((m_t + 1) // 2) * ((N + bn - 1) // bn) * max(1, splits)
-        return (items + 73) // 74
+        return (items + 65) // 66
     if N >= 256 and waves(256) * 2 * 0.88 <= waves(128):
-        return 2256
-    return 2128
+        return 1256
+    return 1128
 
 
 def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, xl=None,
@@ -175,8 +172,7 @@ def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x
     """out[M,N] = epilogue(alpha * op(a) @ op(b)).
 
     ``colsum`` (fp32 [N], optional): += column sums of the bf16 output, i.e. the bias gradient of the
-    layer that consumes ``out`` as its dY.  Fused into the TMA epilogue when possible, otherwise one
-    extra reduction kernel; either way ``colsum`` is up to date on return.
+    layer that consumes ``out`` as its dY (one reduction kernel after the GEMM).
 
     a: ``[M,K]`` (K-major) or ``[K,M]`` when ``a_mn``;  b: ``[N,K]`` or ``[K,N]`` when ``b_mn``.
     """
@@ -193,7 +189,7 @@ def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x
         return r
     if not tc_eligible(a, b, a_mn, b_mn) or out.stride(1) != 1:
         if a.is_cuda:
-            # never silent: a misaligned / non-bf16 operand moves this GEMM off the tcgen05 kernel
+            # never silent: a misaligned / non-bf16 operand moves this GEMM off the wgmma kernel
             sig = (M, N, K, str(a.dtype), tuple(a.stride()), tuple(b.stride()), a.data_ptr() % 16,
                    b.data_ptr() % 16)
             if sig not in _fallback_logged:
@@ -201,7 +197,7 @@ def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x
                 from ..utils import logger
                 logger.warning(f"gemm_bf16: M={M} N={N} K={K} dtype={a.dtype} strides a={tuple(a.stride())} "
                                f"b={tuple(b.stride())} is not TMA-addressable (16-byte base / pitch, bf16): "
-                               "running the library matmul instead of the tcgen05 kernel")
+                               "running the library matmul instead of the wgmma kernel")
         r = gemm_reference(a, b, a_mn, b_mn, bias, mask, x0, xl, alpha, flags, out, aux, addf)
         if colsum is not None:
             colsum.add_(out.float().sum(0))
@@ -211,35 +207,26 @@ def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x
     if block_n == 0:
         block_n = _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags,
                                  splits, addf)
-    fused = _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits,
-                    block_n, addf, colsum)
-    if colsum is not None and not fused:
+    _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, block_n, addf)
+    if colsum is not None:
         from . import dense as _D
         _D.colsum_accum(out, colsum)
     return out
 
 
-def _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, block_n, addf,
-            colsum=None):
-    """-> True when the kernel also accumulated the column sums into ``colsum``"""
+def _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, block_n, addf):
     stream = torch.cuda.current_stream(a.device).cuda_stream
     args = [a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0),
             out.stride(0), int(a_mn), int(b_mn), _ptr(bias), _ptr(mask),
             0 if mask is None else mask.stride(0), _ptr(x0), _ptr(xl),
             0 if xl is None else xl.stride(0), _ptr(aux), 0 if aux is None else aux.stride(0),
-            float(alpha), int(flags), int(splits), 0, _ptr(addf),
-            0 if addf is None else addf.stride(0)]
-    if block_n >= 2000:           # 2000 + BN : cta_group::2 kernel (CTA pair, 256 x BN tile)
-        args[22] = int(block_n - 2000)
-        rc = _lib().hctr_gemm_bf16_2sm(*args, _ptr(colsum), stream)
-    else:
-        args[22] = int(block_n)
-        rc = _lib().hctr_gemm_bf16(*args, stream)
-    if rc not in (0, 100):
+            float(alpha), int(flags), int(splits), int(block_n), _ptr(addf),
+            0 if addf is None else addf.stride(0), stream]
+    rc = _lib().hctr_gemm_bf16(*args)
+    if rc != 0:
         raise RuntimeError(f"hctr_gemm_bf16 failed rc={rc} M={M} N={N} K={K}")
     from . import dense as _D
     _D._count()
-    return rc == 100
 
 
 # ----------------------------------------------------------------------------- tile autotuner
@@ -253,7 +240,7 @@ _TUNE_CACHE = {}
 def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, addf):
     import os
     heur = _pick_block_n(M, N, K, splits)
-    if heur < 2000 or os.environ.get("HCTR_GEMM_AUTOTUNE", "1") == "0" or os.environ.get("HCTR_GEMM_BN"):
+    if heur < 1000 or os.environ.get("HCTR_GEMM_AUTOTUNE", "1") == "0" or os.environ.get("HCTR_GEMM_BN"):
         return heur
     key = (M, N, K, bool(a_mn), bool(b_mn), int(flags), int(splits), out.dtype, out.stride(0),
            aux is not None, bias is not None)
@@ -262,7 +249,7 @@ def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alph
         return hit
     if torch.cuda.is_current_stream_capturing():
         return heur
-    cands = [2128, 2256] if N >= 256 else [2128]
+    cands = [1128, 1256] if N >= 256 else [1128]
     if len(cands) == 1:
         _TUNE_CACHE[key] = cands[0]
         return cands[0]

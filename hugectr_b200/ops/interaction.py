@@ -3,7 +3,7 @@
 out[b] = [ mlp[b] (D) | strict lower triangle of X X^T, row-major (n(n-1)/2) | 0 ]  with
 X = [mlp[b]; emb[b,0]; ...; emb[b,n-2]]  (reference HugeCTR/src/layers/interaction_layer.cu:47-274,
 output width D + n(n-1)/2 + 1, :637).  The torch implementation below is the oracle and the CPU path;
-the sm_100a kernel (csrc/interaction.cu) is used on GPU for bf16 when available.
+the sm_90a kernel (csrc/interaction.cu) is used on GPU for bf16 when available.
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""Loader shim for the sm_100a interaction kernel (csrc/interaction.cu)."""
+"""Loader shim for the sm_90a interaction kernel (csrc/interaction.cu)."""
 from __future__ import annotations
 
 import ctypes as C

@@ -54,7 +54,7 @@ class Solver:
     drop_incomplete_batch: bool = True
     kafka_brockers: str = ""
     training_callbacks: list = field(default_factory=list)
-    # B200 extensions (ignored by reference scripts)
+    # extensions of this framework (ignored by reference scripts)
     use_fp8_mlp: bool = False
     fused_embedding_comm: bool = True
 

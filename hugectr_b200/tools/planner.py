@@ -4,7 +4,7 @@ Capabilities of the reference planner (samples/dlrm/sharding/planner.py:22-327,
 generate_plan.py:23-131): data-parallel threshold for tiny tables, hot-table split (row-wise over
 several GPUs) when one table's lookup cost exceeds the balanced share, memory-cap split, then
 greedy longest-processing-time placement by cost = hotness * (1 + comm/mem ratio).
-B200 numbers: HBM ~6.5 TB/s measured, NVLink ~770 GB/s per direction -> ratio ~8.5.
+H100 SXM data-sheet rates: HBM3 3.35 TB/s, NVLink 450 GB/s per direction -> ratio ~7.4 (not measured here).
 """
 from __future__ import annotations
 
@@ -13,7 +13,7 @@ from typing import List, Sequence, Tuple
 
 def generate_plan(table_sizes: Sequence[int], multi_hot: Sequence[int], num_gpus: int,
                   ev_size: int = 128, plan: str = "auto", dp_threshold_rows: int = 4096,
-                  mem_comm_bw_ratio: float = 6.5e12 / 770e9, mem_cap_gb: float = 150.0,
+                  mem_comm_bw_ratio: float = 3.35e12 / 450e9, mem_cap_gb: float = 70.0,
                   bytes_per_elem: int = 8, num_nodes: int = 1) -> Tuple[List[List[int]], list]:
     """``num_nodes`` > 1 (hier-auto of the reference planner): the shards of a row-split table are
     kept inside ONE node (the least loaded) so that the hierarchical exchange reduces their partial
@@ -71,13 +71,13 @@ def generate_plan(table_sizes: Sequence[int], multi_hot: Sequence[int], num_gpus
 # ------------------------------------------------------------------------------------------------
 # heterogeneous planner: per-table widths / combiners, row- AND column-wise splits, time-based costs
 class HardwareModel:
-    """Per-GPU rates the cost model divides by (defaults: this repo's measurements on B200,
-    MEASURED_PEAKS.json / profiles/README.md): random 512-byte row gathers run at ~0.8 of the 6.5 TB/s
-    copy bandwidth, the read-modify-write sparse update at ~0.55, one NVLink direction carries
-    ~770 GB/s of payload inside the fused exchange, inter-node links 50 GB/s per GPU."""
+    """Per-GPU rates the cost model divides by (defaults: H100 SXM data-sheet bandwidths, not measured here):
+    random 512-byte row gathers are assumed to run at ~0.8 of the 3.35 TB/s HBM3 bandwidth, the read-modify-write
+    sparse update at ~0.55, one NVLink direction carries 450 GB/s, inter-node links 50 GB/s per GPU; 70 of the
+    80 GB are given to embedding tables."""
 
-    def __init__(self, hbm_gbps: float = 6500.0, gather_eff: float = 0.8, update_eff: float = 0.55,
-                 nvlink_gbps: float = 770.0, internode_gbps: float = 50.0, hbm_capacity_gb: float = 150.0):
+    def __init__(self, hbm_gbps: float = 3350.0, gather_eff: float = 0.8, update_eff: float = 0.55,
+                 nvlink_gbps: float = 450.0, internode_gbps: float = 50.0, hbm_capacity_gb: float = 70.0):
         self.hbm, self.gather_eff, self.update_eff = hbm_gbps * 1e9, gather_eff, update_eff
         self.nvlink, self.internode, self.capacity = nvlink_gbps * 1e9, internode_gbps * 1e9, hbm_capacity_gb * 1e9
 

@@ -81,7 +81,7 @@ def kernel_summary(pattern: str = "", log: bool = False):
     (registers / shared memory / occupancy from cudaFuncGetAttributes, cuda_debugging.hpp:44-70),
     read from the cubin with ``cuobjdump -res-usage`` so that it also works without a GPU.
     Returns {demangled kernel name: {"regs", "smem", "stack", "local", "max_blocks_per_sm"}}; the
-    occupancy bound is the register / static-shared-memory limit of sm_100 (64 K registers, 227 KB
+    occupancy bound is the register / static-shared-memory limit of sm_90 (64 K registers, 227 KB
     shared memory, 2048 threads per SM) for a 256-thread block."""
     import re
     import shutil

@@ -3,7 +3,7 @@
 #
 # Generate a Criteo-shaped synthetic Parquet data set, train a DCN through the HugeCTR API (`import hugectr`), evaluate,
 # checkpoint, reload the checkpoint into an inference session and export the model to ONNX.
-# The notebook was executed on CPU (the same script runs unchanged on a B200: one process per GPU under `torchrun`).
+# The notebook was executed on CPU (the same script runs unchanged on an H100: one process per GPU under `torchrun`).
 
 # %%
 import os

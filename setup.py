@@ -1,10 +1,10 @@
-"""In-tree build: `python setup.py build_ext --inplace` compiles the sm_100a kernel library and the
+"""In-tree build: `python setup.py build_ext --inplace` compiles the sm_90a kernel library and the
 host runtime into hugectr_b200/lib (same as `python __graft_entry__.py`)."""
 from setuptools import Command, find_packages, setup
 
 
 class BuildNative(Command):
-    description = "compile libhctr_cuda.so (nvcc, sm_100a) and libhctr_host.so (g++)"
+    description = "compile libhctr_cuda.so (nvcc, sm_90a) and libhctr_host.so (g++)"
     user_options = [("inplace", "i", "kept for setuptools compatibility"), ("force", "f", "rebuild")]
 
     def initialize_options(self):

@@ -243,7 +243,7 @@ def test_native_parameter_server_index(tmp_path):
 
 
 def test_native_library_abi_matches_python_mirrors():
-    """the sm_100a library loads without a GPU; its struct sizes must equal the ctypes mirrors"""
+    """the sm_90a library loads without a GPU; its struct sizes must equal the ctypes mirrors"""
     from hugectr_b200.embedding import ops as E
     from hugectr_b200.ops import dense as D
     E.lib()

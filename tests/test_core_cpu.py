@@ -13,7 +13,7 @@ def test_single_process_backend():
     assert (r.get_global_gpu_id(), r.get_global_gpu_count(), r.get_local_gpu_id(), r.get_local_gpu_count()) == (0, 1, 0, 1)
     assert r.get_device_id() == -1 and r.get_comm() is c
     kp = r.get_kernel_param()
-    assert kp.num_sms == 148 and kp.warp_size == 32
+    assert kp.num_sms == 132 and kp.warp_size == 32
     g = r.get_local_gpu()
     assert g.get_current_stream_name() == "default"
     g.set_stream("emb")

@@ -1,4 +1,4 @@
-"""tcgen05 dot-interaction vs the fp32 oracle (shapes of test/utest/core23_layer_test/interaction_layer_test.cpp:291-320)."""
+"""wgmma dot-interaction vs the fp32 oracle (shapes of test/utest/core23_layer_test/interaction_layer_test.cpp:291-320)."""
 import pytest
 import torch
 

@@ -49,7 +49,7 @@ def test_ebc_fwd_bwd_matches_cpu(opt, ev):
 
 
 def test_dcnv2_step_matches_cpu_reference():
-    """bf16 tcgen05 path vs fp32 CPU path: same init, same batch -> close loss and weights."""
+    """bf16 wgmma path vs fp32 CPU path: same init, same batch -> close loss and weights."""
     from hugectr_b200.models.dlrm import build_dlrm_dcnv2
     from hugectr_b200.parallel.comm import Comm
     kw = dict(batchsize=256, num_gpus=1, table_sizes=[5000, 300, 20000, 40], multi_hot=[3, 1, 10, 2],

@@ -1,5 +1,5 @@
 """Block-scaled fp8 (MX) GEMM: quantiser against the PyTorch reference (bit exact), tensor-core GEMM
-(tcgen05.mma.kind::mxf8f6f4.block_scale, scales in TMEM) against the fp32 product of the de-quantised operands."""
+(fp8 wgmma per 32-wide scale slice, scaled promotion) against the fp32 product of the de-quantised operands."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""Static evidence that needs no GPU: the built library's SASS carries the Blackwell tensor-core / TMEM / TMA
+"""Static evidence that needs no GPU: the built library's SASS carries the Hopper tensor-core (wgmma) / TMA
 instructions in the kernels that are supposed to use them, and no hot kernel spills beyond a small stack."""
 import os
 import shutil
@@ -14,7 +14,7 @@ need = pytest.mark.skipif(not (os.path.exists(LIB) and shutil.which("cuobjdump")
 
 
 @need
-def test_sass_gate_tcgen05_tma_present():
+def test_sass_gate_wgmma_tma_present():
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tools_dev", "sass_evidence.py"), "--check"],
                        capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout + r.stderr
@@ -27,5 +27,5 @@ def test_kernel_resource_report_and_spill_gate():
                        capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr
     names = r.stdout
-    for k in ("gemm_tc2_kernel", "gemm_mxfp8_kernel", "emb_fwd_kernel", "emb_dispatch_kernel", "allreduce_twoshot_kernel"):
+    for k in ("gemm_tc_kernel", "gemm_mxfp8_kernel", "emb_fwd_kernel", "emb_dispatch_kernel", "allreduce_twoshot_kernel"):
         assert k in names, k

@@ -1,4 +1,4 @@
-"""Device-timed microbenchmark of the tcgen05 GEMM vs torch.matmul (cuBLAS) on DLRM shapes."""
+"""Device-timed microbenchmark of the wgmma GEMM vs torch.matmul (cuBLAS) on DLRM shapes."""
 import json, sys, torch
 sys.path.insert(0, ".")
 from hugectr_b200.ops import gemm as G
@@ -24,7 +24,7 @@ def main():
                            (8192,8192,8192,"sq8k")]:
         a = torch.randn(M, K, device="cuda").bfloat16(); w = torch.randn(K, N, device="cuda").bfloat16() * 0.05
         out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
-        for bn in (128, 256, 2128, 2256):
+        for bn in (128, 256, 1128, 1256):
             t = timeit(lambda: G.gemm_bf16(a, w, out, b_mn=True, block_n=bn))
             res.append(dict(tag=tag, M=M, N=N, K=K, bn=bn, ms=t, tflops=2*M*N*K/t/1e9))
         t = timeit(lambda: torch.matmul(a, w, out=out))
@@ -33,7 +33,7 @@ def main():
         dy = torch.randn(M, N, device="cuda").bfloat16()
         dw = torch.zeros(K, N, device="cuda")
         for sp in (1, 2, 4):
-            for bn in (128, 2128, 2256):
+            for bn in (128, 1128, 1256):
                 t = timeit(lambda: G.gemm_bf16(a, dy, dw, a_mn=True, b_mn=True, flags=G.EPI_ATOMIC, splits=sp, block_n=bn))
                 res.append(dict(tag=tag+"_wgrad", M=K, N=N, K=M, bn=f"split{sp}_bn{bn}", ms=t, tflops=2*M*N*K/t/1e9))
         t = timeit(lambda: torch.matmul(a.t(), dy))

@@ -12,12 +12,12 @@ dH = bf(b, pd)
 def rep(tag, ms, flops):
     print(json.dumps(dict(tag=tag, us=round(ms * 1e3, 1), tflops=round(flops / ms / 1e9))), flush=True)
 fl = 2 * b * w * pd
-for bn in (2128, 2256, 128):
+for bn in (1128, 1256, 128):
     rep(f"crossV plain bn{bn}", timeit(lambda: G.gemm_bf16(H, V, out, b_mn=True, block_n=bn)), fl)
     rep(f"crossV EPI_CROSS bn{bn}", timeit(lambda: G.gemm_bf16(H, V, out, b_mn=True, bias=bias, x0=x0, xl=xl, aux=T, flags=G.EPI_CROSS, block_n=bn)), fl)
     rep(f"dgrad EPI_ADD bn{bn}", timeit(lambda: G.gemm_bf16(dH, U, out, xl=xl, flags=G.EPI_ADD, block_n=bn)), fl)
     rep(f"dgrad plain bn{bn}", timeit(lambda: G.gemm_bf16(dH, U, out, block_n=bn)), fl)
 a = bf(b, 1024); wt = bf(1024, 3456); dy = bf(b, 3456); mask = bf(b, 1024); dx = bf(b, 1024)
-for bn in (2128, 2256):
+for bn in (1128, 1256):
     rep(f"top0 dgrad MASK bn{bn}", timeit(lambda: G.gemm_bf16(dy, wt, dx, mask=mask, flags=G.EPI_MASK, block_n=bn)), 2 * b * 1024 * 3456)
     rep(f"top0 dgrad plain bn{bn}", timeit(lambda: G.gemm_bf16(dy, wt, dx, block_n=bn)), 2 * b * 1024 * 3456)

@@ -1,6 +1,6 @@
-"""MX fp8 GEMM (csrc/gemm_mxfp8.cu) vs the bf16 tcgen05 GEMM, cuBLAS bf16 (torch.mm) and torch._scaled_mm (cuBLASLt
+"""MX fp8 GEMM (csrc/gemm_mxfp8.cu) vs the bf16 wgmma GEMM, cuBLAS bf16 (torch.mm) and torch._scaled_mm (cuBLASLt
 fp8, per-tensor scales) on the DLRM-DCNv2 MLP shapes.  CUDA events, L2 flushed between timings.
-    python tools_dev/bench_mxfp8.py > profiles/gemm_mxfp8_microbench.jsonl"""
+    python tools_dev/bench_mxfp8.py > gemm_mxfp8_microbench.jsonl"""
 import json
 import os
 import sys
@@ -43,7 +43,7 @@ for name, M, N, K in SHAPES:
     r["mxfp8_gemm_us"] = timeit(lambda: MX.gemm_mxfp8(aq, sfa, bq, sfb, M, N, K, out=out))
     r["mx_quant_act_us"] = timeit(lambda: MX.mx_quantize(a, aq, sfa))
     r["mx_quant_wT_us"] = timeit(lambda: MX.mx_quantize(w, bq, sfb, transposed=True))
-    r["bf16_tcgen05_us"] = timeit(lambda: G.gemm_bf16(a, w, out, b_mn=True))
+    r["bf16_wgmma_us"] = timeit(lambda: G.gemm_bf16(a, w, out, b_mn=True))
     r["cublas_bf16_us"] = timeit(lambda: torch.mm(a, w, out=out))
     try:
         a8, w8 = a.to(torch.float8_e4m3fn), w.t().contiguous().to(torch.float8_e4m3fn)
@@ -53,7 +53,7 @@ for name, M, N, K in SHAPES:
         r["cublaslt_fp8_scaled_mm_us"] = f"n/a: {str(e)[:80]}"
     fl = 2.0 * M * N * K
     r["mxfp8_tflops"] = fl / r["mxfp8_gemm_us"] / 1e6
-    r["bf16_tcgen05_tflops"] = fl / r["bf16_tcgen05_us"] / 1e6
+    r["bf16_wgmma_tflops"] = fl / r["bf16_wgmma_us"] / 1e6
     ref = MX.mx_dequantize(aq, sfa, M, K).cuda() @ MX.mx_dequantize(bq, sfb, N, K).cuda().t() if M * N <= 1 << 24 else None
     if ref is not None:
         r["max_err_vs_dequant"] = float((out.float() - ref).abs().max())

@@ -7,5 +7,5 @@ a = torch.randn(M, K, device="cuda").bfloat16(); w = (torch.randn(K, N, device="
 out = torch.empty(M, N, device="cuda", dtype=torch.bfloat16)
 bias = torch.zeros(N, device="cuda")
 for _ in range(6):
-    G.gemm_bf16(a, w, out, b_mn=True, bias=bias, flags=G.EPI_RELU, block_n=2128)
+    G.gemm_bf16(a, w, out, b_mn=True, bias=bias, flags=G.EPI_RELU, block_n=1128)
 torch.cuda.synchronize()

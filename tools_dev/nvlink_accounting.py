@@ -1,6 +1,6 @@
 """NVLink byte accounting of the fused embedding paths for the benchmark's sharding plan (no GPU needed: the routes
 are pure metadata).  Per rank and step: key-dispatch stores, pooled-vector stores (owner -> requester), gradient
-push stores; max over ranks.  python tools_dev/nvlink_accounting.py > profiles/r2/nvlink_bytes.txt"""
+push stores; max over ranks.  python tools_dev/nvlink_accounting.py > nvlink_bytes.txt"""
 import os
 import sys
 

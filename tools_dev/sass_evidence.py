@@ -1,7 +1,7 @@
-"""Tensor-core / TMEM / TMA mnemonic counts per kernel of the built library.
+"""Tensor-core / TMA / mbarrier mnemonic counts per kernel of the built library.
 
-  python tools_dev/sass_evidence.py                 # table on stdout (what profiles/*/sass_evidence*.txt hold)
-  python tools_dev/sass_evidence.py --check         # CI gate: the kernels that must use tcgen05 / TMA do
+  python tools_dev/sass_evidence.py                 # table on stdout
+  python tools_dev/sass_evidence.py --check         # CI gate: the kernels that must use wgmma / TMA do
   cuobjdump -sass lib.so | python tools_dev/sass_evidence.py -     # read a listing from stdin
 """
 import collections
@@ -12,13 +12,12 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "hugectr_b200", "lib", "libhctr_cuda.so")
-PAT = re.compile(r'\b(UTCQMMA|UTCHMMA|UTCCP|UTCBAR|LDTM|UTMALDG|UTMASTG|UBLKCP|SYNCS|UTMAPF)[A-Z0-9_.]*')
+PAT = re.compile(r'\b(HGMMA|QGMMA|WARPGROUP|UTMALDG|UTMASTG|UBLKCP|SYNCS|UTMAPF)[A-Z0-9_.]*')
 # kernel-name fragment -> mnemonics it must contain
 REQUIRED = {
-    "gemm_tc2_kernel": ("UTCHMMA", "LDTM", "UTMALDG", "UTCBAR"),
-    "gemm_tc_kernel": ("UTCHMMA", "LDTM", "UTMALDG"),
-    "gemm_mxfp8_kernel": ("UTCQMMA", "UTCCP", "LDTM", "UTMALDG"),
-    "interaction": ("UTCHMMA", "LDTM"),
+    "gemm_tc_kernel": ("HGMMA", "UTMALDG", "SYNCS"),
+    "gemm_mxfp8_kernel": ("QGMMA", "UTMALDG", "UBLKCP"),
+    "interaction": ("HGMMA",),
 }
 
 
@@ -51,11 +50,10 @@ def main(argv):
                 missing = [m for m in need if not cnt[k].get(m)]
                 if missing:
                     bad.append(f"{k[:100]}: missing {missing}")
-        print("\n".join(bad) if bad else f"ok: {sum(1 for k in cnt if cnt[k])} kernels carry tcgen05 / TMA / bulk-copy SASS")
+        print("\n".join(bad) if bad else f"ok: {sum(1 for k in cnt if cnt[k])} kernels carry wgmma / TMA / bulk-copy SASS")
         return 1 if bad else 0
-    print("cuobjdump -sass hugectr_b200/lib/libhctr_cuda.so : tensor-core / TMEM / TMA / bulk-copy mnemonic counts per kernel")
-    print("UTCQMMA = tcgen05.mma block-scaled (kind::mxf8f6f4.block_scale)   UTCHMMA = tcgen05.mma kind::f16")
-    print("UTCCP = tcgen05.cp smem->TMEM   LDTM = tcgen05.ld   UTCBAR = tcgen05.commit   UTMALDG / UTMASTG = TMA tensor load / store")
+    print("cuobjdump -sass hugectr_b200/lib/libhctr_cuda.so : tensor-core / TMA / bulk-copy mnemonic counts per kernel")
+    print("HGMMA / QGMMA = wgmma.mma_async bf16 / fp8   WARPGROUP = wgmma fence / wait   UTMALDG / UTMASTG = TMA tensor load / store")
     print("UBLKCP = cp.async.bulk (1-D)   SYNCS = mbarrier ops\n")
     for k, v in sorted(cnt.items()):
         if v:
