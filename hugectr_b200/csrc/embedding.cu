@@ -25,10 +25,11 @@ namespace hctr {
 
 // ------------------------------------------------------------------ forward
 // One group of G lanes per (src rank, lookup, sample) bucket; each lane owns VEC consecutive
-// floats per 32*VEC-wide column chunk.  G*VEC >= ev for ev <= 128 (VEC=4), wider rows loop.
+// floats per 32*VEC-wide column chunk.  G*VEC >= ev for ev <= 128 (VEC=4), wider rows loop over
+// up to MAXC chunks per lane: one launch covers columns [col_base, col_base + MAXC * G * VEC).
 template <typename KeyT, typename OutT, int VEC, int U>
 __global__ void __launch_bounds__(256, 3)
-    emb_fwd_kernel(const EmbParams p, const int G, const long long total_items) {
+    emb_fwd_kernel(const EmbParams p, const int G, const int col_base) {
   // grid.y = (src rank, lookup): uniform per block, no per-thread integer division
   const int lane = threadIdx.x & 31;
   const int groups_per_warp = 32 / G;
@@ -39,7 +40,6 @@ __global__ void __launch_bounds__(256, 3)
   const int s = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * groups_per_warp + gi;
   const bool active = s < p.batch;
   const unsigned gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (gi * G));
-  (void)total_items;
   const EmbLookup lk = p.lookups[l];
   const int ev = lk.ev_size;
   int nnz = lk.hotness;
@@ -48,20 +48,20 @@ __global__ void __launch_bounds__(256, 3)
   if (active && lk.nnz_off >= 0) nnz = min(lk.hotness, p.nnz[src][lk.nnz_off + s]);
   if (!active) nnz = 0;
 
-  constexpr int MAXC = (U >= 8) ? 8 : 4;  // chunks per lane: ev <= MAXC * G * VEC
+  constexpr int MAXC = (U >= 8) ? 8 : 4;  // chunks per lane
   float acc[MAXC][VEC];
 #pragma unroll
   for (int c = 0; c < MAXC; ++c)
 #pragma unroll
     for (int v = 0; v < VEC; ++v) acc[c][v] = 0.f;
-  const int nchunk = (ev + G * VEC - 1) / (G * VEC);
+  const int nchunk = (ev - col_base + G * VEC - 1) / (G * VEC);
 
   // gathers U rows (rp[u] == nullptr: skip) into the accumulators
   auto gather = [&](const float* const (&rp)[U]) {
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {
       if (c < nchunk) {
-        const int col = (c * G + gl) * VEC;
+        const int col = col_base + (c * G + gl) * VEC;
         if (col < ev) {
           if constexpr (VEC == 4) {
             float4 v[U];
@@ -165,7 +165,7 @@ __global__ void __launch_bounds__(256, 3)
 #pragma unroll
   for (int c = 0; c < MAXC; ++c) {
     if (c < nchunk) {
-      const int col = (c * G + gl) * VEC;
+      const int col = col_base + (c * G + gl) * VEC;
       if (col < ev) {
         if constexpr (VEC == 4) {
           store_vec4<OutT>(o + col, acc[c][0] * scale, acc[c][1] * scale, acc[c][2] * scale,
@@ -208,7 +208,7 @@ __global__ void __launch_bounds__(256)
   if (active && lk.nnz_off >= 0) nnz = min(lk.hotness, p.nnz[src][lk.nnz_off + s]);
   if (!active) nnz = 0;
 
-  constexpr int MAXC = 8;
+  constexpr int MAXC = 32 / VEC;   // ev <= MAXC * G * VEC = kMaxEmbWidth at G = 32
   float g[MAXC][VEC];
   const int nchunk = (ev + G * VEC - 1) / (G * VEC);
   float scale = grad_scale;
@@ -406,10 +406,13 @@ static inline int pick_group(int ev, int vec) {
 }
 
 // key_bytes: 4 or 8 ; out_bf16 / grad_bf16 : element type of activations
+// aligned4: every lookup's ev_size, out_off and out_stride, the table pitch and the base pointers are
+// multiples of 4 elements (16-byte table rows, whole-vector output stores); 0 selects scalar accesses
 extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, int out_bf16,
-                                void* stream_) {
+                                int aligned4, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
-  const int vec = (max_ev % 4 == 0) ? 4 : 1;
+  if (max_ev > kMaxEmbWidth) return -4;
+  const int vec = (aligned4 && max_ev % 4 == 0) ? 4 : 1;
   int G = pick_group(max_ev, vec);
   // wide rows: 8 lanes per bucket, every lane owns up to 4 float4 chunks of the row -> 4 buckets
   // per warp and 16 independent 16-byte loads in flight per lane (latency-bound -> bandwidth-bound)
@@ -421,8 +424,12 @@ extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, i
   const int buckets_per_block = (threads / 32) * (32 / G);
   const dim3 blocks((p->batch + buckets_per_block - 1) / buckets_per_block,
                     p->num_ranks * p->num_lookups);
+  // one pass covers every column, except scalar rows wider than 8 chunks x 32 lanes: those take
+  // passes of 256 columns (keeps the accumulators of the scalar kernel in registers)
+  const int pass = (vec == 4) ? max_ev : 8 * G;
+  for (int c0 = 0; c0 < max_ev; c0 += pass) {
 #define LAUNCH(K, O, V, UU) \
-  emb_fwd_kernel<K, O, V, UU><<<blocks, threads, 0, st>>>(*p, G, items)
+  emb_fwd_kernel<K, O, V, UU><<<blocks, threads, 0, st>>>(*p, G, c0)
 #define LAUNCH_U(K, O, V)            \
   if (narrow) { LAUNCH(K, O, V, 4); } \
   else { LAUNCH(K, O, V, 8); }
@@ -432,6 +439,7 @@ extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, i
   } else {
     if (key_bytes == 8) { if (out_bf16) { LAUNCH(long long, __nv_bfloat16, 1, 8); } else { LAUNCH(long long, float, 1, 8); } }
     else { if (out_bf16) { LAUNCH(int, __nv_bfloat16, 1, 8); } else { LAUNCH(int, float, 1, 8); } }
+  }
   }
 #undef LAUNCH_U
 #undef LAUNCH
@@ -484,9 +492,10 @@ extern "C" int hctr_emb_shard_split(const void* keys, void* out, int* nnz, int b
 extern "C" int hctr_emb_backward_accum(const EmbParams* p, const UniqueTable* ut,
                                        float* wgrad_unique, float grad_scale, int max_ev,
                                        int key_bytes, int grad_bf16, int dp_ev4, void* stream_) {
-  // dp_ev4: every lookup's ev_size is a multiple of 4 and its gradient rows are 16-byte aligned
+  // dp_ev4: every lookup's ev_size, grad_off and grad_stride, the pitch and the base pointers are
+  // multiples of 4 elements (whole-vector gradient loads); 0 selects scalar accesses
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
-  const int vec = (max_ev % 4 == 0) ? 4 : 1;
+  const int vec = (dp_ev4 && max_ev % 4 == 0) ? 4 : 1;
   const int G = pick_group(max_ev, vec);
   const long long items = static_cast<long long>(p->num_ranks) * p->num_lookups * p->batch;
   if (items == 0) return 0;
@@ -513,6 +522,7 @@ extern "C" int hctr_emb_backward_accum(const EmbParams* p, const UniqueTable* ut
 #undef LAUNCH_DP
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
   }
+  if (max_ev > kMaxEmbWidth) return -4;
   const long long warps = (items + (32 / G) - 1) / (32 / G);
   const int threads = 256;
   const long long blocks = (warps * 32 + threads - 1) / threads;

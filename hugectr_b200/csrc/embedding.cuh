@@ -11,6 +11,9 @@ namespace hctr {
 constexpr int kMaxRanks = 16;
 constexpr unsigned long long kEmptyKey = 0xFFFFFFFFFFFFFFFFull;
 constexpr unsigned int kInvalidVal = 0xFFFFFFFFu;
+// widest row the lookup / accumulate / fused-update kernels cover (32 lanes x 32 columns per lane);
+// the entry points reject wider tables instead of truncating them
+constexpr int kMaxEmbWidth = 1024;
 
 struct EmbLookup {
   long long table_row_off;  // first row of this table shard inside the local arena

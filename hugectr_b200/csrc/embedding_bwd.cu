@@ -398,6 +398,7 @@ HCTR_DEVICE const GradT* locate_grad(const EmbParams& p, unsigned int e) {
 // sharing a warp would otherwise wait for the longest of them (2.6x measured slowdown).
 // List positions are reserved with one atomicAdd per block and class.
 constexpr unsigned int kLightMax = 4;
+constexpr unsigned int kMaxHeavyChunks = 4096;   // heavy item = (uid, scratch slot << 12 | chunk)
 __global__ void __launch_bounds__(1024)
     emb_bwd_classify_kernel(const UniqueTable ut, const BwdIndex ix) {
   __shared__ unsigned int s_cnt[2][32];
@@ -412,7 +413,28 @@ __global__ void __launch_bounds__(1024)
       cnt = ix.offsets[uid + 1] - o0;
     }
     const bool is_light = cnt >= 1 && cnt <= kLightMax;
-    const bool is_medium = cnt > kLightMax && cnt <= kHeavy;
+    bool is_medium = cnt > kLightMax && cnt <= kHeavy;
+    if (cnt > kHeavy) {
+      // a heavy row gets a scratch row and its chunks' work items only if all of them fit (and the
+      // chunk index fits its 12 bits); otherwise it falls back to the warp-per-row medium list, which
+      // handles any count, so every row is updated exactly once whatever the caps
+      const unsigned int nch = (cnt + kChunk - 1) / kChunk;
+      bool placed = false;
+      if (nch <= kMaxHeavyChunks) {
+        const unsigned int slot = atomicAdd(ix.heavy_slot, 1u);
+        if (slot < ix.max_heavy_rows) {
+          const unsigned int hb = atomicAdd(ix.heavy_count, nch);
+          placed = hb + nch <= ix.max_heavy_items;
+          // items reserved past the cap by a row that does not fit are marked invalid, so the
+          // heavy kernel never picks up a stale item of an earlier step
+          for (unsigned int c = 0; c < nch && hb + c < ix.max_heavy_items; ++c) {
+            ix.heavy_items[2 * (hb + c)] = placed ? uid : kInvalidVal;
+            ix.heavy_items[2 * (hb + c) + 1] = (slot << 12) | c;
+          }
+        }
+      }
+      is_medium = !placed;
+    }
     const unsigned int bl = __ballot_sync(0xffffffffu, is_light);
     const unsigned int bm = __ballot_sync(0xffffffffu, is_medium);
     if (lane == 0) {
@@ -438,16 +460,6 @@ __global__ void __launch_bounds__(1024)
     } else if (is_medium) {
       const unsigned int pos = s_base[1] + s_cnt[1][warp] + __popc(bm & below);
       ix.medium_list[pos] = make_uint2(uid, o0);
-    } else if (cnt > kHeavy) {
-      const unsigned int nch = (cnt + kChunk - 1) / kChunk;
-      const unsigned int slot = atomicAdd(ix.heavy_slot, 1u);
-      const unsigned int hb = atomicAdd(ix.heavy_count, nch);
-      for (unsigned int c = 0; c < nch; ++c) {
-        if (hb + c < ix.max_heavy_items && slot < ix.max_heavy_rows) {
-          ix.heavy_items[2 * (hb + c)] = uid;
-          ix.heavy_items[2 * (hb + c) + 1] = (slot << 12) | c;   // <= 4096 chunks per row
-        }
-      }
     }
     __syncthreads();
   }
@@ -645,6 +657,7 @@ __global__ void __launch_bounds__(256)
   const float inv_scaler = grad_scale / hp.scaler;
   for (unsigned int it = blockIdx.x; it < nitems; it += gridDim.x) {
     const unsigned int uid = ix.heavy_items[2 * it];
+    if (uid == kInvalidVal) continue;   // reserved by a row that fell back to the medium list
     const unsigned int sc_ = ix.heavy_items[2 * it + 1];
     const unsigned int slot = sc_ >> 12, chunk = sc_ & 0xFFFu;
     const unsigned int o0 = ix.offsets[uid] + chunk * kChunk;
@@ -711,11 +724,11 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// (heavy rows past the caps take the medium path, see emb_bwd_classify_kernel: only the unique-row
+// capacity can overflow)
 __global__ void emb_bwd_finish_kernel(unsigned int* counter, unsigned int* overflow_flag,
-                                      unsigned int max_unique, const unsigned int* heavy_count,
-                                      unsigned int max_heavy_items) {
+                                      unsigned int max_unique) {
   if (*counter > max_unique) atomicMax(overflow_flag, *counter);
-  if (*heavy_count > max_heavy_items) atomicMax(overflow_flag, 0x80000000u | *heavy_count);
   *counter = 0;
 }
 
@@ -739,6 +752,7 @@ extern "C" int hctr_emb_bwd_index(const EmbParams* p, const UniqueTable* ut, con
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (total_pairs == 0) return 0;
   if (p->num_lookups > kMaxSmemLookups) return -5;
+  if (ix->max_heavy_rows > (1u << 20)) return -6;   // 20-bit scratch slot field of a heavy item
   const unsigned int blocks = static_cast<unsigned int>((total_pairs + kPairsPerBlock - 1) / kPairsPerBlock);
   if (key_bytes == 8)
     emb_bwd_index_kernel<long long><<<blocks, kIdxThreads, 0, st>>>(*p, *ut, *ix, total_pairs);
@@ -822,7 +836,8 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
                                           void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (p->ev_size % 4) return -3;
-#define LAUNCH(O)                                                                               \
+  if (p->ev_size > kMaxEmbWidth) return -4;
+#define LAUNCH(O)                                                                             \
   if (state_bf16)                                                                               \
     launch_reduce<O, __nv_bfloat16>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st); \
   else                                                                                          \
@@ -838,7 +853,6 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
     default: return -2;
   }
 #undef LAUNCH
-  emb_bwd_finish_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique,
-                                         ix->heavy_count, ix->max_heavy_items);
+  emb_bwd_finish_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -175,6 +175,15 @@ class _Group:
         self.opt: Optional[OptParamsPy] = None
 
 
+def fused_backward_ok(grp: _Group) -> bool:
+    """Whether a model-parallel group may use the fused index + reduce/update backward: it locates
+    gradient rows in 4-element units, so every lookup's gradient columns must be 4-aligned (a top
+    that concatenates an ev-6 table in front of another table, or that follows a width-6 top at an
+    odd batch, is not); other groups take the accumulate + update path."""
+    return E.vec4_aligned(grp.lookups, grp.pitch) and \
+        os.environ.get("HCTR_EMB_BWD", "indexed") == "indexed"
+
+
 class EmbeddingCollection:
     def __init__(self, cfg: EmbeddingCollectionConfig, batch_per_gpu: int, hotness: Dict[str, int],
                  device, act_dtype, comm, default_opt: OptParamsPy, key_dtype=torch.int32,
@@ -344,6 +353,8 @@ class EmbeddingCollection:
             cf = pl.col_factor
             ev_part = t.ev_size // cf
             assert ev_part * cf == t.ev_size, "ev_size must be divisible by the column factor"
+            if self.device.type == "cuda":
+                E.check_ev_size(ev_part, f"table {t.name}: embedding vector")
             if pl.kind == "dp":
                 parts = [(0, 1, 0)]
             else:
@@ -435,9 +446,7 @@ class EmbeddingCollection:
             pairs = po
             if self.is_train:
                 if grp.kind == "mp":
-                    import os
-                    grp.indexed = (dev.type == "cuda" and grp.pitch % 4 == 0
-                                   and os.environ.get("HCTR_EMB_BWD", "indexed") == "indexed")
+                    grp.indexed = dev.type == "cuda" and fused_backward_ok(grp)
                     grp.ws = E.UniqueWorkspace(max(pairs, 1), grp.pitch, dev, indexed=grp.indexed,
                                                need_scale=any(l.combiner == 1 for l in grp.lookups))
                 else:
@@ -769,6 +778,8 @@ class EmbeddingCollection:
             if ht.overflowed():
                 raise RuntimeError(f"dynamic embedding table {name}: more than init_capacity="
                                    f"{ht.max_rows} distinct keys on one shard (shard {s_})")
+        for grp in self.groups:
+            E.check_workspace_overflow(getattr(grp, "ws", None), f"{grp.kind} group ev={grp.pitch}")
 
     def grow_dynamic(self, factor: float = 2.0):
         """DynamicEmbeddingTable semantics (embedding_storage/dynamic_embedding.cu: the vocabulary is not bounded):

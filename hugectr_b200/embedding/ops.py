@@ -70,7 +70,7 @@ def lib():
     if _lib is None:
         l = _native.cuda_lib()
         vp, i, f, ll = C.c_void_p, C.c_int, C.c_float, C.c_longlong
-        l.hctr_emb_forward.argtypes = [C.POINTER(CEmbParams), i, i, i, vp]
+        l.hctr_emb_forward.argtypes = [C.POINTER(CEmbParams), i, i, i, i, vp]
         l.hctr_emb_backward_accum.argtypes = [C.POINTER(CEmbParams), C.POINTER(CUniqueTable), vp, f,
                                               i, i, i, i, vp]
         l.hctr_emb_update.argtypes = [vp, vp, vp, vp, C.POINTER(CUniqueTable), i, i, i,
@@ -134,6 +134,35 @@ def lookups_to_device(lookups: List[LookupDesc], device) -> torch.Tensor:
 
 def _st(dev):
     return torch.cuda.current_stream(dev).cuda_stream
+
+
+# widest embedding row the CUDA lookup / accumulate / fused-update kernels cover (kMaxEmbWidth in
+# csrc/embedding.cuh); wider tables are rejected rather than truncated
+MAX_EV_SIZE = 1024
+
+
+def check_ev_size(ev_size: int, what: str = "embedding vector"):
+    if ev_size > MAX_EV_SIZE:
+        raise ValueError(f"{what} size {ev_size} exceeds the widest row the embedding kernels support "
+                         f"({MAX_EV_SIZE}); split the table's columns (column-wise sharding) or use a "
+                         f"narrower ev_size")
+
+
+def vec4_aligned(lookups, ev_pitch, bufs=(), grad: bool = True) -> bool:
+    """True when the kernels may move 4 consecutive elements as one vector for every lookup: ev_size,
+    pitch and the gradient (``grad``) or output offsets and strides are multiples of 4 elements and
+    every base pointer in ``bufs`` (tensors or int device pointers) is 16-byte aligned.  Collections
+    that concatenate a narrow table in front of another one (column 6 of a 134-wide top), or odd
+    batches behind a width-6 top, break this; the kernels then take their scalar paths."""
+    def ptr(b):
+        return b if isinstance(b, int) else b.data_ptr()
+    if ev_pitch % 4:
+        return False
+    for l in lookups:
+        off, stride = (l.grad_off, l.grad_stride) if grad else (l.out_off, l.out_stride)
+        if l.ev_size % 4 or off % 4 or stride % 4:
+            return False
+    return all(ptr(b) % 16 == 0 for b in bufs if b is not None)
 
 
 # ----------------------------------------------------------------------------- shard split
@@ -274,9 +303,11 @@ def forward(lookups, lookups_dev, table, ev_pitch, key_bufs, out_bufs, batch, my
         p.table = table.data_ptr()
         p.ev_size = ev_pitch
         max_ev = max((l.ev_size for l in lookups), default=ev_pitch)
-        rc = lib().hctr_emb_forward(C.byref(p), max_ev, kb, out_bf16, _st(table.device))
+        check_ev_size(max_ev)
+        al4 = int(vec4_aligned(lookups, ev_pitch, [table, *out_bufs], grad=False))
+        rc = lib().hctr_emb_forward(C.byref(p), max_ev, kb, out_bf16, al4, _st(table.device))
         if rc:
-            raise RuntimeError("hctr_emb_forward failed")
+            raise RuntimeError(f"hctr_emb_forward failed rc={rc}")
         D._count()
         return
     forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs)
@@ -314,11 +345,21 @@ def forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_b
 
 
 # ----------------------------------------------------------------------------- backward
+HEAVY_MIN_COUNT = 65   # occurrences in one step from which a row is reduced block-per-chunk (kHeavy + 1)
+
+
 class UniqueWorkspace:
     """Transient hash + fp32 per-unique-row gradient accumulator (device)."""
 
     def __init__(self, max_pairs: int, ev_pitch: int, device, unique_ratio: float = 1.0,
-                 indexed: bool = False, need_scale: bool = False):
+                 indexed: bool = False, need_scale: bool = False, max_heavy_rows: int = None,
+                 max_heavy_items: int = None):
+        """``max_heavy_rows`` / ``max_heavy_items`` (indexed path) size the scratch rows and the
+        512-entry chunk work items of the block-per-chunk kernel for rows with more than 64
+        occurrences in a step; heavy rows beyond them, and rows of more than 4096 chunks, are
+        reduced by the warp-per-row kernel (correct, but one warp per row).  By default they are
+        sized from ``max_pairs`` so that every heavy row fits -- at most max_pairs / 65 rows and
+        max_pairs / 512 + rows chunks -- with the scratch rows capped at 64 MiB (and >= 8192)."""
         self.device = device
         self.ev = ev_pitch
         self.max_unique = max(16, int(max_pairs * unique_ratio))
@@ -351,8 +392,15 @@ class UniqueWorkspace:
                 self.pair_uid = torch.full((mp,), -1, **i32)
                 self.bucket_list = torch.zeros(mp, **i32)
                 self.bucket_scale = torch.ones(mp, dtype=torch.float32, device=device) if need_scale else None
-                self.max_heavy_rows = 8192
-                self.max_heavy_items = 65536
+                if max_heavy_rows is None:
+                    max_heavy_rows = min(max(mp // HEAVY_MIN_COUNT, 1),
+                                         max(8192, (1 << 24) // max(ev_pitch, 1)), 1 << 20)
+                if max_heavy_items is None:
+                    max_heavy_items = mp // 512 + max_heavy_rows
+                if not 1 <= max_heavy_rows <= (1 << 20) or max_heavy_items < 1:
+                    raise ValueError("max_heavy_rows must be in [1, 2^20] and max_heavy_items >= 1")
+                self.max_heavy_rows = int(max_heavy_rows)
+                self.max_heavy_items = int(max_heavy_items)
                 self.heavy_items = torch.zeros(2 * self.max_heavy_items, **i32)
                 self.heavy_count = torch.zeros(1, **i32)
                 self.heavy_slot = torch.zeros(1, **i32)
@@ -375,6 +423,16 @@ class UniqueWorkspace:
         else:
             self.ref_rows = None
             self.ref_grads = None
+
+
+def check_workspace_overflow(ws, what: str):
+    """Raise if a backward step found more distinct rows than ``ws`` holds (their updates were
+    dropped).  Reads the workspace's sticky device flag: a host sync."""
+    flag = getattr(ws, "overflow", None)
+    if flag is not None and int(flag.item()) != 0:
+        raise RuntimeError(f"embedding backward workspace of {what} overflowed: "
+                           f"{int(flag.item()) & 0xFFFFFFFF} distinct rows in one step, room for "
+                           f"{ws.max_unique}")
 
 
 def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch, ws, grad_scale=1.0,
@@ -405,13 +463,13 @@ def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, b
             dst = dense_wgrad.data_ptr()
         else:
             ut, dst = ws.c, ws.wgrad.data_ptr()
-        esz = 2 if gbf else 4
-        ev4 = int(all(l.ev_size % 4 == 0 and (l.grad_off * esz) % 16 == 0 and
-                      (l.grad_stride * esz) % 16 == 0 for l in lookups))
+        if dense_wgrad is None:
+            check_ev_size(max_ev)
+        ev4 = int(vec4_aligned(lookups, ev_pitch, [dst, *grad_bufs], grad=True))
         rc = lib().hctr_emb_backward_accum(C.byref(p), C.byref(ut), dst, float(grad_scale), max_ev,
                                            kb, gbf, ev4, _st(table.device))
         if rc:
-            raise RuntimeError("hctr_emb_backward_accum failed")
+            raise RuntimeError(f"hctr_emb_backward_accum failed rc={rc}")
         D._count()
         return
     rows_all, grads_all = [], []
@@ -569,6 +627,10 @@ def _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, bat
 def bwd_index(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, ws, my_rank=0, nnz_bufs=None,
               key_bytes=4):
     """Gradient-independent part of the backward: unique rows + per-row bucket lists."""
+    check_ev_size(ev_pitch)
+    if not vec4_aligned(lookups, ev_pitch, [table], grad=True):
+        raise ValueError("the fused backward needs 4-element aligned gradient rows and pitch "
+                         "(see vec4_aligned); use backward_accum + update")
     p, kb, _ = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, None, batch, my_rank,
                             nnz_bufs, key_bytes)
     total_pairs = len(key_bufs) * batch * sum(l.hotness for l in lookups)
@@ -583,6 +645,10 @@ def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_
                       grad_bufs, batch, ws, hp: dict, lr_t, step_t, grad_scale=1.0, my_rank=0,
                       nnz_bufs=None, num_sms: int = 132, key_bytes=4, act_bf16=True):
     """Fused gradient gather (local / peer loads) + duplicate reduction + optimizer."""
+    check_ev_size(ev_pitch)
+    if not vec4_aligned(lookups, ev_pitch, [table, *grad_bufs], grad=True):
+        raise ValueError("the fused backward needs 4-element aligned gradient rows and pitch "
+                         "(see vec4_aligned); use backward_accum + update")
     p, kb, gbf = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch,
                               my_rank, nnz_bufs, key_bytes, act_bf16)
     h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),

@@ -131,7 +131,7 @@ class SparseEmbeddingRuntime:
             po += W * b * H
         self.lookups_dev = E.lookups_to_device(self.lookups, device)
         if self.is_train:
-            self.indexed = device.type == "cuda" and vec % 4 == 0 and \
+            self.indexed = device.type == "cuda" and E.vec4_aligned(self.lookups, vec) and \
                 os.environ.get("HCTR_EMB_BWD", "indexed") == "indexed"
             self.ws = E.UniqueWorkspace(max(po, 1), vec, device, indexed=self.indexed)
         self.slot_offsets = None
@@ -173,6 +173,7 @@ class SparseEmbeddingRuntime:
             n = self.hash.size()
             raise RuntimeError(f"Runtime vocabulary size (>= {n}) exceeds max_vocabulary_size_per_gpu "
                                f"({self.max_rows}) of {self.name}, new feature insertion failed.")
+        E.check_workspace_overflow(getattr(self, "ws", None), self.name)
 
     # ------------------------------------------------------------------ forward / backward
     def _translate(self, is_train: bool):
