@@ -27,7 +27,8 @@ namespace hctr {
 // One group of G lanes per (src rank, lookup, sample) bucket; each lane owns VEC consecutive
 // floats per 32*VEC-wide column chunk.  G*VEC >= ev for ev <= 128 (VEC=4), wider rows loop over
 // up to MAXC chunks per lane: one launch covers columns [col_base, col_base + MAXC * G * VEC).
-template <typename KeyT, typename OutT, int VEC, int U>
+// WT: weight type of the arena (fp32, or bf16 loaded 8 bytes per 4 columns); pooling is in fp32.
+template <typename KeyT, typename OutT, int VEC, int U, typename WT>
 __global__ void __launch_bounds__(256, 3)
     emb_fwd_kernel(const EmbParams p, const int G, const int col_base) {
   // grid.y = (src rank, lookup): uniform per block, no per-thread integer division
@@ -47,6 +48,7 @@ __global__ void __launch_bounds__(256, 3)
                       static_cast<long long>(s) * lk.key_stride;
   if (active && lk.nnz_off >= 0) nnz = min(lk.hotness, p.nnz[src][lk.nnz_off + s]);
   if (!active) nnz = 0;
+  const WT* table = static_cast<const WT*>(p.table);
 
   constexpr int MAXC = (U >= 8) ? 8 : 4;  // chunks per lane
   float acc[MAXC][VEC];
@@ -57,7 +59,7 @@ __global__ void __launch_bounds__(256, 3)
   const int nchunk = (ev - col_base + G * VEC - 1) / (G * VEC);
 
   // gathers U rows (rp[u] == nullptr: skip) into the accumulators
-  auto gather = [&](const float* const (&rp)[U]) {
+  auto gather = [&](const WT* const (&rp)[U]) {
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {
       if (c < nchunk) {
@@ -67,8 +69,7 @@ __global__ void __launch_bounds__(256, 3)
             float4 v[U];
 #pragma unroll
             for (int u = 0; u < U; ++u)
-              v[u] = rp[u] ? __ldg(reinterpret_cast<const float4*>(rp[u] + col))
-                           : make_float4(0.f, 0.f, 0.f, 0.f);
+              v[u] = rp[u] ? ldg_row4(rp[u] + col) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int u = 0; u < U; ++u) {
               acc[c][0] += v[u].x; acc[c][1] += v[u].y; acc[c][2] += v[u].z; acc[c][3] += v[u].w;
@@ -76,7 +77,7 @@ __global__ void __launch_bounds__(256, 3)
           } else {
             float v[U];
 #pragma unroll
-            for (int u = 0; u < U; ++u) v[u] = rp[u] ? __ldg(rp[u] + col) : 0.f;
+            for (int u = 0; u < U; ++u) v[u] = rp[u] ? ldg_row1(rp[u] + col) : 0.f;
 #pragma unroll
             for (int u = 0; u < U; ++u) acc[c][0] += v[u];
           }
@@ -123,7 +124,7 @@ __global__ void __launch_bounds__(256, 3)
         }
       }
       while (m) {               // group-uniform
-        const float* rp[U];
+        const WT* rp[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           rp[u] = nullptr;
@@ -133,7 +134,7 @@ __global__ void __launch_bounds__(256, 3)
           const int i = b / G, sl = b - i * G;
           const unsigned int cand = i == 0 ? rowv[0] : (i == 1 ? rowv[1] : (i == 2 ? rowv[2] : rowv[3]));
           const unsigned int r = __shfl_sync(gmask, cand, gi * G + sl);
-          if (take) rp[u] = p.table + (lk.table_row_off + r) * static_cast<long long>(p.ev_size);
+          if (take) rp[u] = table + (lk.table_row_off + r) * static_cast<long long>(p.ev_size);
         }
         gather(rp);
       }
@@ -145,13 +146,13 @@ __global__ void __launch_bounds__(256, 3)
       if (h0 + gl < nnz) mykey = static_cast<long long>(kbase[h0 + gl]);
       const int cnt = min(G, nnz - h0);
       for (int j0 = 0; j0 < cnt; j0 += U) {
-        const float* rp[U];
+        const WT* rp[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int j = j0 + u;
           const long long key = __shfl_sync(gmask, mykey, gi * G + (j < cnt ? j : 0));
           const bool ok = (j < cnt) && key >= 0 && key < lk.rows;
-          rp[u] = ok ? p.table + (lk.table_row_off + key) * static_cast<long long>(p.ev_size) : nullptr;
+          rp[u] = ok ? table + (lk.table_row_off + key) * static_cast<long long>(p.ev_size) : nullptr;
         }
         gather(rp);
       }
@@ -331,9 +332,9 @@ __global__ void __launch_bounds__(256)
 
 // One warp per unique row: reads the accumulated fp32 gradient (and zeroes it for the next step),
 // updates weight + optimizer state in place and releases the row's hash slot.
-template <int OPT, typename StateT>
+template <int OPT, typename StateT, typename WT>
 __global__ void __launch_bounds__(256)
-    emb_update_kernel(float* __restrict__ table, StateT* __restrict__ s0, StateT* __restrict__ s1,
+    emb_update_kernel(WT* __restrict__ table, StateT* __restrict__ s0, StateT* __restrict__ s1,
                       float* __restrict__ wgrad_unique, const UniqueTable ut, const int ev,
                       const OptHyper hp) {
   const unsigned int n = min(*ut.counter, ut.max_unique);
@@ -345,6 +346,7 @@ __global__ void __launch_bounds__(256)
     bc2 = 1.f - powf(hp.beta2, t);
   }
   const float inv_scaler = 1.f / hp.scaler;
+  const unsigned long long srk = sr_key<WT>(hp.sr_seed, hp.step_ptr);
   const int lane = threadIdx.x & 31;
   const unsigned int warps = (gridDim.x * blockDim.x) >> 5;
   for (unsigned int uid = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; uid < n; uid += warps) {
@@ -355,17 +357,17 @@ __global__ void __launch_bounds__(256)
       for (int col = lane * 4; col < ev; col += 128) {
         float4 g = *reinterpret_cast<float4*>(gsrc + col);
         *reinterpret_cast<float4*>(gsrc + col) = make_float4(0.f, 0.f, 0.f, 0.f);
-        float4 w = *reinterpret_cast<float4*>(table + base + col);
+        float4 w = load_vec4<WT>(table + base + col);
         apply_opt4<OPT, StateT>(w, make_float4(g.x * inv_scaler, g.y * inv_scaler, g.z * inv_scaler, g.w * inv_scaler), s0, s1, base + col, hp, lr, bc1, bc2);
-        *reinterpret_cast<float4*>(table + base + col) = w;
+        store_w4<WT>(table + base + col, w, srk, base + col);
       }
     } else {
       for (int col = lane; col < ev; col += 32) {
         const float g = gsrc[col];
         gsrc[col] = 0.f;
-        float w = table[base + col];
+        float w = to_f<WT>(table[base + col]);
         apply_opt<OPT, StateT>(w, g * inv_scaler, s0, s1, base + col, hp, lr, bc1, bc2);
-        table[base + col] = w;
+        store_w<WT>(table + base + col, w, srk, base + col);
       }
     }
     if (lane == 0) {
@@ -383,15 +385,15 @@ __global__ void emb_reset_counter_kernel(unsigned int* counter, unsigned int* ov
 }
 
 // plain gather (no pooling): out[i] = table[rows[i]]  (concat combiner / dense lookups / SOK)
-template <typename OutT>
-__global__ void emb_gather_rows_kernel(const float* __restrict__ table, const long long* rows,
+template <typename OutT, typename WT>
+__global__ void emb_gather_rows_kernel(const WT* __restrict__ table, const long long* rows,
                                        OutT* out, long long n, int ev) {
   const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= n) return;
   const long long r = rows[w];
   for (int c = lane; c < ev; c += 32)
-    out[w * ev + c] = from_f<OutT>(r < 0 ? 0.f : table[r * ev + c]);
+    out[w * ev + c] = from_f<OutT>(r < 0 ? 0.f : to_f<WT>(table[r * ev + c]));
 }
 
 }  // namespace hctr
@@ -405,11 +407,11 @@ static inline int pick_group(int ev, int vec) {
   return p;
 }
 
-// key_bytes: 4 or 8 ; out_bf16 / grad_bf16 : element type of activations
+// key_bytes: 4 or 8 ; out_bf16 / grad_bf16 : element type of activations ; table_bf16 : of the arena
 // aligned4: every lookup's ev_size, out_off and out_stride, the table pitch and the base pointers are
-// multiples of 4 elements (16-byte table rows, whole-vector output stores); 0 selects scalar accesses
+// multiples of 4 elements (whole-vector table rows and output stores); 0 selects scalar accesses
 extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, int out_bf16,
-                                int aligned4, void* stream_) {
+                                int aligned4, int table_bf16, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (max_ev > kMaxEmbWidth) return -4;
   const int vec = (aligned4 && max_ev % 4 == 0) ? 4 : 1;
@@ -428,8 +430,9 @@ extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, i
   // passes of 256 columns (keeps the accumulators of the scalar kernel in registers)
   const int pass = (vec == 4) ? max_ev : 8 * G;
   for (int c0 = 0; c0 < max_ev; c0 += pass) {
-#define LAUNCH(K, O, V, UU) \
-  emb_fwd_kernel<K, O, V, UU><<<blocks, threads, 0, st>>>(*p, G, c0)
+#define LAUNCH(K, O, V, UU)                                                                       \
+  if (table_bf16) emb_fwd_kernel<K, O, V, UU, __nv_bfloat16><<<blocks, threads, 0, st>>>(*p, G, c0); \
+  else emb_fwd_kernel<K, O, V, UU, float><<<blocks, threads, 0, st>>>(*p, G, c0)
 #define LAUNCH_U(K, O, V)            \
   if (narrow) { LAUNCH(K, O, V, 4); } \
   else { LAUNCH(K, O, V, 8); }
@@ -539,20 +542,22 @@ extern "C" int hctr_emb_backward_accum(const EmbParams* p, const UniqueTable* ut
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
-extern "C" int hctr_emb_update(float* table, void* s0, void* s1, float* wgrad_unique,
+extern "C" int hctr_emb_update(void* table, void* s0, void* s1, float* wgrad_unique,
                                const UniqueTable* ut, int ev, int opt, int state_bf16,
                                const OptHyper* hp, unsigned int* overflow_flag, int num_sms,
-                               void* stream_) {
+                               int table_bf16, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   const int threads = 256;
   const int blocks = num_sms * 8;
-#define LAUNCH(O)                                                                             \
+#define LAUNCH_W(O, W)                                                                        \
   if (state_bf16)                                                                             \
-    emb_update_kernel<O, __nv_bfloat16><<<blocks, threads, 0, st>>>(                         \
-        table, (__nv_bfloat16*)s0, (__nv_bfloat16*)s1, wgrad_unique, *ut, ev, *hp);          \
+    emb_update_kernel<O, __nv_bfloat16, W><<<blocks, threads, 0, st>>>(                      \
+        (W*)table, (__nv_bfloat16*)s0, (__nv_bfloat16*)s1, wgrad_unique, *ut, ev, *hp);      \
   else                                                                                        \
-    emb_update_kernel<O, float><<<blocks, threads, 0, st>>>(table, (float*)s0, (float*)s1,   \
-                                                            wgrad_unique, *ut, ev, *hp);
+    emb_update_kernel<O, float, W><<<blocks, threads, 0, st>>>((W*)table, (float*)s0,         \
+                                                               (float*)s1, wgrad_unique, *ut, ev, *hp);
+#define LAUNCH(O) \
+  if (table_bf16) { LAUNCH_W(O, __nv_bfloat16) } else { LAUNCH_W(O, float) }
   switch (opt) {
     case OPT_SGD: LAUNCH(OPT_SGD); break;
     case OPT_ADAGRAD: LAUNCH(OPT_ADAGRAD); break;
@@ -564,18 +569,23 @@ extern "C" int hctr_emb_update(float* table, void* s0, void* s1, float* wgrad_un
     default: return -2;
   }
 #undef LAUNCH
+#undef LAUNCH_W
   emb_reset_counter_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
-extern "C" int hctr_emb_gather_rows(const float* table, const long long* rows, void* out,
-                                    long long n, int ev, int out_bf16, void* stream_) {
+extern "C" int hctr_emb_gather_rows(const void* table, const long long* rows, void* out,
+                                    long long n, int ev, int out_bf16, int table_bf16, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (n == 0) return 0;
-  const long long blocks = (n * 32 + 255) / 256;
-  if (out_bf16)
-    emb_gather_rows_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, st>>>(table, rows, (__nv_bfloat16*)out, n, ev);
-  else
-    emb_gather_rows_kernel<float><<<(unsigned)blocks, 256, 0, st>>>(table, rows, (float*)out, n, ev);
+  const unsigned blocks = static_cast<unsigned>((n * 32 + 255) / 256);
+#define LAUNCH(O, W) \
+  emb_gather_rows_kernel<O, W><<<blocks, 256, 0, st>>>((const W*)table, rows, (O*)out, n, ev)
+  if (table_bf16) {
+    if (out_bf16) LAUNCH(__nv_bfloat16, __nv_bfloat16); else LAUNCH(float, __nv_bfloat16);
+  } else {
+    if (out_bf16) LAUNCH(__nv_bfloat16, float); else LAUNCH(float, float);
+  }
+#undef LAUNCH
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -41,7 +41,7 @@ struct EmbParams {
   void* out[kMaxRanks];          // per source rank: output activation base
   const void* grad[kMaxRanks];   // per source rank: top-grad base
   const EmbLookup* lookups;      // device array [num_lookups]
-  float* table;                  // [rows, ev] fp32 arena
+  void* table;                   // [rows, ev] arena of fp32 or bf16 weights (the launcher's table_bf16)
   int ev_size;                   // row pitch of the arena (all tables of a group share it)
 };
 
@@ -59,14 +59,17 @@ struct UniqueTable {
   unsigned int max_unique;
 };
 
-HCTR_DEVICE unsigned int hash64(unsigned long long k) {
+// MurmurHash3 64-bit finaliser (a bijection of 64-bit words)
+HCTR_DEVICE unsigned long long fmix64(unsigned long long k) {
   k ^= k >> 33;
   k *= 0xff51afd7ed558ccdull;
   k ^= k >> 33;
   k *= 0xc4ceb9fe1a85ec53ull;
   k ^= k >> 33;
-  return static_cast<unsigned int>(k);
+  return k;
 }
+
+HCTR_DEVICE unsigned int hash64(unsigned long long k) { return static_cast<unsigned int>(fmix64(k)); }
 
 template <typename T>
 HCTR_DEVICE void store_vec4(T* p, float a, float b, float c, float d);
@@ -101,6 +104,86 @@ template <>
 HCTR_DEVICE float from_f<float>(float v) { return v; }
 template <>
 HCTR_DEVICE __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return __float2bfloat16(v); }
+
+// ------------------------------------------------------------------ bf16 weights: stochastic rounding
+// Every optimizer store of a bf16 weight rounds stochastically: the stored value is the upper 16 bits
+// of (fp32 bits + r), r = 16 pseudo-random bits, so it rounds away from zero with probability equal to
+// the dropped fraction of an ulp and the expected stored value is the fp32 result (updates far below
+// one bf16 ulp still move the weights on average).  Inf / NaN are stored as round-to-nearest does.
+// r is a stateless hash of (seed, device step counter, arena index i = row * pitch + col): no host
+// input, capturable in a CUDA graph, independent across steps and kernels, and reproduced by a resumed
+// run.  One 64-bit hash serves four consecutive elements: r(i) = 16-bit lane i % 4 of
+// fmix64(step key ^ i / 4), so a 4-wide store hashes once.
+// Mirrored bit for bit by embedding/ops.py (sr_step_key, sr_bits, sr_round_bf16).
+HCTR_DEVICE unsigned long long sr_step_key(unsigned int seed, unsigned int step) {
+  return fmix64((static_cast<unsigned long long>(seed) << 32) | step);
+}
+HCTR_DEVICE unsigned long long sr_hash4(unsigned long long key, long long idx) {
+  return fmix64(key ^ (static_cast<unsigned long long>(idx) >> 2));
+}
+HCTR_DEVICE unsigned short sr_round(float v, unsigned int r) {
+  const unsigned int b = __float_as_uint(v);
+  if ((b & 0x7f800000u) == 0x7f800000u) return __bfloat16_as_ushort(__float2bfloat16_rn(v));
+  return static_cast<unsigned short>((b + r) >> 16);
+}
+
+// Weight rows of the arena: WT = float or __nv_bfloat16.  Loads widen to fp32 (load_vec4 / to_f);
+// the optimizer stores go through store_w / store_w4 with the launch's key (sr_key), which the fp32
+// instantiations never compute.
+template <typename WT>
+HCTR_DEVICE unsigned long long sr_key(unsigned int seed, const unsigned int* step_ptr) {
+  if constexpr (sizeof(WT) == 2) return sr_step_key(seed, step_ptr ? *step_ptr : 1u);
+  return 0ull;
+}
+template <typename WT>
+HCTR_DEVICE void store_w(WT* p, float w, unsigned long long key, long long idx);
+template <>
+HCTR_DEVICE void store_w<float>(float* p, float w, unsigned long long, long long) { *p = w; }
+template <>
+HCTR_DEVICE void store_w<__nv_bfloat16>(__nv_bfloat16* p, float w, unsigned long long key, long long idx) {
+  const unsigned int r = static_cast<unsigned int>(sr_hash4(key, idx) >> (16 * (idx & 3))) & 0xFFFFu;
+  *reinterpret_cast<unsigned short*>(p) = sr_round(w, r);
+}
+template <typename WT>
+HCTR_DEVICE void store_w4(WT* p, float4 w, unsigned long long key, long long idx);
+template <>
+HCTR_DEVICE void store_w4<float>(float* p, float4 w, unsigned long long, long long) {
+  *reinterpret_cast<float4*>(p) = w;
+}
+template <>
+HCTR_DEVICE void store_w4<__nv_bfloat16>(__nv_bfloat16* p, float4 w, unsigned long long key, long long idx) {
+  // idx % 4 == 0 (4-aligned rows and columns): the four lanes of one hash
+  const unsigned long long h = sr_hash4(key, idx);
+  const unsigned int lo = static_cast<unsigned int>(h), hi = static_cast<unsigned int>(h >> 32);
+  const unsigned int a = sr_round(w.x, lo & 0xFFFFu), b = sr_round(w.y, lo >> 16);
+  const unsigned int c = sr_round(w.z, hi & 0xFFFFu), d = sr_round(w.w, hi >> 16);
+  *reinterpret_cast<uint2*>(p) = make_uint2(a | (b << 16), c | (d << 16));
+}
+// A 4-column slice of a weight row as loaded: float4 (fp32) or the packed bf16 pairs (uint2), widened
+// to fp32 where the optimizer needs it, so a bf16 row held across the gradient gather takes half the
+// registers.
+template <typename WT>
+struct Row4 {
+  using type = float4;
+};
+template <>
+struct Row4<__nv_bfloat16> {
+  using type = uint2;
+};
+template <typename WT>
+HCTR_DEVICE typename Row4<WT>::type load_row4(const WT* p) {
+  return *reinterpret_cast<const typename Row4<WT>::type*>(p);
+}
+HCTR_DEVICE float4 widen4(float4 v) { return v; }
+HCTR_DEVICE float4 widen4(uint2 v) { return make_float4(bf16_lo(v.x), bf16_hi(v.x), bf16_lo(v.y), bf16_hi(v.y)); }
+// read-only (non-coherent cache) row loads of the lookup
+HCTR_DEVICE float4 ldg_row4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+HCTR_DEVICE float4 ldg_row4(const __nv_bfloat16* p) {
+  const uint2 v = __ldg(reinterpret_cast<const uint2*>(p));
+  return make_float4(bf16_lo(v.x), bf16_hi(v.x), bf16_lo(v.y), bf16_hi(v.y));
+}
+HCTR_DEVICE float ldg_row1(const float* p) { return __ldg(p); }
+HCTR_DEVICE float ldg_row1(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
 
 // ------------------------------------------------------------------ unique (transient hash)
 HCTR_DEVICE unsigned int unique_get_insert(const UniqueTable& t, unsigned long long row) {
@@ -142,6 +225,8 @@ struct OptHyper {
   float momentum;
   float initial_accu;
   const unsigned int* step_ptr;  // device step counter (Adam bias correction), 1-based
+  unsigned int sr_seed;          // seed of the stochastic rounding of bf16 weights (sr_step_key)
+  unsigned int pad_;
 };
 
 template <int OPT, typename StateT>

@@ -472,7 +472,9 @@ __global__ void __launch_bounds__(1024)
 // and the row id / entries of i+1 are in flight while row i is reduced, and the weight / state
 // vectors are requested together with the gradients, so ONE DRAM latency is exposed per row.
 // Medium part: one warp per row, 8 gradient rows in flight per round.
-template <int OPT, typename StateT, typename GradT, int G>
+// WT: weight type of the arena (fp32, or bf16 moved 8 bytes per 4 columns and stored with stochastic
+// rounding); the reduction and the optimizer run in fp32 either way.
+template <int OPT, typename StateT, typename GradT, int G, typename WT>
 __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
     emb_bwd_reduce_update_kernel(const EmbParams p, const UniqueTable ut, const BwdIndex ix,
                                  StateT* __restrict__ s0, StateT* __restrict__ s1, const OptHyper hp,
@@ -486,6 +488,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
     bc2 = 1.f - powf(hp.beta2, t);
   }
   const float inv_scaler = grad_scale / hp.scaler;
+  const unsigned long long srk = sr_key<WT>(hp.sr_seed, hp.step_ptr);
   const int lane = threadIdx.x & 31;
   const int ev = p.ev_size;
   const bool has_scale = ix.bucket_scale != nullptr;
@@ -540,13 +543,15 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       // 128 registers of two resident blocks per SM for G == 32 (8 chunks per lane)
 #pragma unroll
       for (int c0 = 0; c0 < NC; c0 += 4) {
-      float4 wv[4], sv[4], acc[4];
+      typename Row4<WT>::type wv[4];
+      float4 sv[4], acc[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         const int col = ((c0 + c) * G + gl) * 4;
-        wv[c] = sv[c] = acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+        wv[c] = {};
+        sv[c] = acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (col < ev) {
-          wv[c] = *reinterpret_cast<const float4*>(p.table + base + col);
+          wv[c] = load_row4<WT>(static_cast<const WT*>(p.table) + base + col);
           if constexpr (kHasS0) sv[c] = load_vec4<StateT>(s0 + base + col);
         }
       }
@@ -570,11 +575,11 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       for (int c = 0; c < 4; ++c) {
         const int col = ((c0 + c) * G + gl) * 4;
         if (col < ev) {
-          float4 w = wv[c];
+          float4 w = widen4(wv[c]);
           apply_opt4_pre<OPT, StateT>(w, make_float4(acc[c].x * inv_scaler, acc[c].y * inv_scaler,
                                                      acc[c].z * inv_scaler, acc[c].w * inv_scaler),
                                       sv[c], s0, s1, base + col, hp, lr, bc1, bc2);
-          *reinterpret_cast<float4*>(p.table + base + col) = w;
+          store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
         }
       }
       }
@@ -601,7 +606,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
     const unsigned int o1 = ix.offsets[uid + 1];
     const long long base = static_cast<long long>(ut.rows[uid]) * ev;
     for (int col = lane * 4; col < ev; col += 128) {
-      float4 w = *reinterpret_cast<const float4*>(p.table + base + col);
+      float4 w = load_vec4<WT>(static_cast<const WT*>(p.table) + base + col);
       float4 sv = make_float4(0.f, 0.f, 0.f, 0.f);
       if constexpr (kHasS0) sv = load_vec4<StateT>(s0 + base + col);
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -626,7 +631,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       apply_opt4_pre<OPT, StateT>(w, make_float4(acc.x * inv_scaler, acc.y * inv_scaler,
                                                  acc.z * inv_scaler, acc.w * inv_scaler),
                                   sv, s0, s1, base + col, hp, lr, bc1, bc2);
-      *reinterpret_cast<float4*>(p.table + base + col) = w;
+      store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
     }
     if (lane == 0) {
       const unsigned int slot = ut.slots[uid];
@@ -637,7 +642,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
 }
 
 // heavy rows: one block per (uid, chunk)
-template <int OPT, typename StateT, typename GradT>
+template <int OPT, typename StateT, typename GradT, typename WT>
 __global__ void __launch_bounds__(256)
     emb_bwd_heavy_kernel(const EmbParams p, const UniqueTable ut, const BwdIndex ix,
                          StateT* __restrict__ s0, StateT* __restrict__ s1, const OptHyper hp,
@@ -706,12 +711,13 @@ __global__ void __launch_bounds__(256)
       __threadfence();
       const unsigned long long row = ut.rows[uid];
       const long long base = static_cast<long long>(row) * ev;
+      const unsigned long long srk = sr_key<WT>(hp.sr_seed, hp.step_ptr);
       for (int c = threadIdx.x; c < ev; c += blockDim.x) {
         const float g = __ldcg(scratch + c);
         scratch[c] = 0.f;
-        float w = p.table[base + c];
+        float w = to_f<WT>(static_cast<const WT*>(p.table)[base + c]);
         apply_opt<OPT, StateT>(w, g * inv_scaler, s0, s1, base + c, hp, lr, bc1, bc2);
-        p.table[base + c] = w;
+        store_w<WT>(static_cast<WT*>(p.table) + base + c, w, srk, base + c);
       }
       if (threadIdx.x == 0) {
         ix.heavy_ticket[slot] = 0;
@@ -788,7 +794,7 @@ struct SideStream {
 };
 static SideStream g_heavy_side;
 
-template <int OPT, typename StateT>
+template <int OPT, typename StateT, typename WT>
 static int launch_reduce(const EmbParams* p, const UniqueTable* ut, const BwdIndex* ix, void* s0,
                          void* s1, const OptHyper* hp, float grad_scale, int grad_bf16, int num_sms,
                          cudaStream_t st) {
@@ -804,25 +810,25 @@ static int launch_reduce(const EmbParams* p, const UniqueTable* ut, const BwdInd
     cudaStreamWaitEvent(hs, g_heavy_side.fork, 0);
   }
   if (grad_bf16)
-    emb_bwd_heavy_kernel<OPT, StateT, __nv_bfloat16><<<num_sms * 4, 256, smem, hs>>>(
+    emb_bwd_heavy_kernel<OPT, StateT, __nv_bfloat16, WT><<<num_sms * 4, 256, smem, hs>>>(
         *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
   else
-    emb_bwd_heavy_kernel<OPT, StateT, float><<<num_sms * 4, 256, smem, hs>>>(
+    emb_bwd_heavy_kernel<OPT, StateT, float, WT><<<num_sms * 4, 256, smem, hs>>>(
         *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
   if (fork) cudaEventRecord(g_heavy_side.join, hs);
   if (grad_bf16) {
     if (g8)
-      emb_bwd_reduce_update_kernel<OPT, StateT, __nv_bfloat16, 8><<<blocks, 256, 0, st>>>(
+      emb_bwd_reduce_update_kernel<OPT, StateT, __nv_bfloat16, 8, WT><<<blocks, 256, 0, st>>>(
           *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
     else
-      emb_bwd_reduce_update_kernel<OPT, StateT, __nv_bfloat16, 32><<<blocks, 256, 0, st>>>(
+      emb_bwd_reduce_update_kernel<OPT, StateT, __nv_bfloat16, 32, WT><<<blocks, 256, 0, st>>>(
           *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
   } else {
     if (g8)
-      emb_bwd_reduce_update_kernel<OPT, StateT, float, 8><<<blocks, 256, 0, st>>>(
+      emb_bwd_reduce_update_kernel<OPT, StateT, float, 8, WT><<<blocks, 256, 0, st>>>(
           *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
     else
-      emb_bwd_reduce_update_kernel<OPT, StateT, float, 32><<<blocks, 256, 0, st>>>(
+      emb_bwd_reduce_update_kernel<OPT, StateT, float, 32, WT><<<blocks, 256, 0, st>>>(
           *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
   }
   if (fork) cudaStreamWaitEvent(st, g_heavy_side.join, 0);
@@ -833,15 +839,17 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
                                           const BwdIndex* ix, void* s0, void* s1, int opt,
                                           int state_bf16, const OptHyper* hp, float grad_scale,
                                           int grad_bf16, unsigned int* overflow_flag, int num_sms,
-                                          void* stream_) {
+                                          int table_bf16, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (p->ev_size % 4) return -3;
   if (p->ev_size > kMaxEmbWidth) return -4;
-#define LAUNCH(O)                                                                             \
-  if (state_bf16)                                                                               \
-    launch_reduce<O, __nv_bfloat16>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st); \
-  else                                                                                          \
-    launch_reduce<O, float>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st);
+#define LAUNCH_W(O, W)                                                                             \
+  if (state_bf16)                                                                                  \
+    launch_reduce<O, __nv_bfloat16, W>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st); \
+  else                                                                                             \
+    launch_reduce<O, float, W>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st);
+#define LAUNCH(O) \
+  if (table_bf16) { LAUNCH_W(O, __nv_bfloat16) } else { LAUNCH_W(O, float) }
   switch (opt) {
     case OPT_SGD: LAUNCH(OPT_SGD); break;
     case OPT_ADAGRAD: LAUNCH(OPT_ADAGRAD); break;
@@ -853,6 +861,7 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
     default: return -2;
   }
 #undef LAUNCH
+#undef LAUNCH_W
   emb_bwd_finish_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -34,6 +34,9 @@ def _stable_seed(*parts) -> int:
 
 
 # ------------------------------------------------------------------------- configs
+WEIGHT_DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16}
+
+
 @dataclass
 class InitParams:
     """embedding_storage/common.hpp:43-77: Uniform(up_bound) or Sinusoidal(max_sequence_len, ev)."""
@@ -59,6 +62,12 @@ class EmbeddingTableConfig:
         self.init_capacity = int(kw.get("init_capacity", 1 << 20))
         # rows per shard a dynamic table may grow to (0 = no limit but memory): see EmbeddingCollection.grow_dynamic
         self.max_capacity = int(kw.get("max_capacity", 0))
+        # storage of the weights of a model-parallel table: "fp32" or "bf16" (half the bytes; every
+        # optimizer store rounds stochastically, see csrc/embedding.cuh).  Data-parallel tables stay fp32.
+        self.weight_dtype = str(kw.get("weight_dtype", "fp32"))
+        if self.weight_dtype not in WEIGHT_DTYPES:
+            raise ValueError(f"table {self.name}: weight_dtype must be one of {sorted(WEIGHT_DTYPES)}, "
+                             f"not {self.weight_dtype!r}")
 
 
 class EmbeddingCollectionConfig:
@@ -158,6 +167,14 @@ def resolve_placement(cfg: EmbeddingCollectionConfig, num_gpus: int) -> Dict[str
     return place
 
 
+def _uniform_fill(view, bound, gen):
+    """U(-bound, bound) into ``view``: drawn in fp32, a bf16 arena gets them rounded to nearest"""
+    if view.dtype == torch.float32:
+        view.uniform_(-bound, bound, generator=gen)
+    else:
+        view.copy_(torch.empty(view.shape, dtype=torch.float32, device=view.device).uniform_(-bound, bound, generator=gen))
+
+
 def shard_rows(vocab: int, k: int, s: int) -> int:
     """number of keys in [0, vocab) with key % k == s"""
     return (vocab - s + k - 1) // k if vocab > s else 0
@@ -165,10 +182,10 @@ def shard_rows(vocab: int, k: int, s: int) -> int:
 
 # ------------------------------------------------------------------------- runtime
 class _Group:
-    """Local tables of one (kind, ev pitch) group: one fp32 arena + optimizer state."""
+    """Local tables of one (kind, ev pitch, weight dtype) group: one arena + optimizer state."""
 
-    def __init__(self, kind, pitch):
-        self.kind, self.pitch = kind, pitch
+    def __init__(self, kind, pitch, wdtype="fp32"):
+        self.kind, self.pitch, self.wdtype = kind, pitch, wdtype
         self.rows = 0
         self.table_slices = []   # (table name, col part, row_off, rows, num_shards, shard_idx, col0)
         self.lookups: List[E.LookupDesc] = []
@@ -221,6 +238,9 @@ class EmbeddingCollection:
         self.is_train = is_train
         self.hotness = dict(hotness)
         self.seed = seed
+        # seed of the stochastic rounding of bf16 weights (with the device step counter and the arena
+        # index: a run is reproducible for a fixed sharding plan)
+        self.sr_seed = int(seed) & 0xFFFFFFFF
         self._unique_tables = self._resolve_unique_tables()
         self._kb = 8 if key_dtype == torch.int64 else 4
         self._abf = act_dtype == torch.bfloat16
@@ -346,8 +366,14 @@ class EmbeddingCollection:
 
     # ---- local storage + owner-side lookup descriptors
     def _build_storage(self, seed, share_from=None):
-        groups: Dict[Tuple[str, int], _Group] = {}
+        groups: Dict[Tuple[str, int, str], _Group] = {}
         b = self.b
+        wdtype = {t.name: getattr(t, "weight_dtype", "fp32") for t in self.tables}
+        dp_bf16 = [n for n, w in wdtype.items() if w != "fp32" and self.placement[n].kind == "dp"]
+        if dp_bf16 and share_from is None:
+            from ..utils import logger
+            logger.info(f"weight_dtype: data-parallel tables {sorted(dp_bf16)} keep fp32 weights (their gradients "
+                        "take the dense all-reduce and the dense optimizer)")
         for t in self.tables:
             pl = self.placement[t.name]
             cf = pl.col_factor
@@ -364,8 +390,9 @@ class EmbeddingCollection:
                     if g == self.rank:
                         parts.append((idx // kk, kk, idx % kk))   # (col part, num row shards, shard)
             for (cpart, k, s) in parts:
-                key = (pl.kind, ev_part)
-                grp = groups.setdefault(key, _Group(pl.kind, ev_part))
+                wdt = wdtype[t.name] if pl.kind == "mp" else "fp32"
+                key = (pl.kind, ev_part, wdt)
+                grp = groups.setdefault(key, _Group(pl.kind, ev_part, wdt))
                 rows = t.init_capacity if t.dynamic else shard_rows(t.max_vocabulary_size, k, s)
                 grp.table_slices.append({"table": t.name, "cpart": cpart, "row_off": grp.rows,
                                          "rows": rows, "k": k, "s": s, "col0": cpart * ev_part,
@@ -378,7 +405,7 @@ class EmbeddingCollection:
         for gi, gl in enumerate(self.glookups):
             t = self.tmap[gl["table"]]
             pl = self.placement[t.name]
-            for (kind, pitch), grp in groups.items():
+            for grp in groups.values():
                 for sl in grp.table_slices:
                     if sl["table"] != t.name:
                         continue
@@ -419,14 +446,15 @@ class EmbeddingCollection:
         gen = torch.Generator(device="cpu")
         if share_from is not None:
             for grp, src in zip(self.groups, share_from.groups):
-                assert (grp.kind, grp.pitch, len(grp.table_slices)) == (src.kind, src.pitch, len(src.table_slices))
+                assert (grp.kind, grp.pitch, grp.wdtype, len(grp.table_slices)) == \
+                    (src.kind, src.pitch, src.wdtype, len(src.table_slices))
                 grp.opt = src.opt
                 grp.ws = None
             self._resync_storage(share_from)     # arrays + row windows (dynamic shards may have grown since)
             return
         for grp in self.groups:
             n = max(grp.rows, 1) * grp.pitch
-            grp.table = torch.empty(n, dtype=torch.float32, device=dev)
+            grp.table = torch.empty(n, dtype=WEIGHT_DTYPES[grp.wdtype], device=dev)
             self._init_group(grp, gen, seed)
             ns = grp.opt.num_states if grp.opt is not None else 0
             if grp.opt.optimizer_type == Optimizer_t.Adam:
@@ -478,11 +506,11 @@ class EmbeddingCollection:
                 full_rows = t.max_vocabulary_size
                 if not t.dynamic and full_rows * grp.pitch <= (1 << 26):
                     full = (torch.rand(full_rows, grp.pitch, generator=gen) * 2 - 1) * bound
-                    view.copy_(full[sl["s"]::sl["k"]].reshape(-1).to(view.device))
+                    view.copy_(full[sl["s"]::sl["k"]].reshape(-1).to(view.device))   # bf16: to nearest
                     continue
             g2 = torch.Generator(device=self.device)
             g2.manual_seed(_stable_seed(seed, sl["table"], sl["cpart"], sl["s"]))
-            view.uniform_(-bound, bound, generator=g2)
+            _uniform_fill(view, bound, g2)
 
     def _alloc_buffers(self):
         dev, b, W = self.device, self.b, self.world
@@ -841,7 +869,7 @@ class EmbeddingCollection:
             bound = t.init_param.up_bound
         gen = torch.Generator(device=dev)
         gen.manual_seed(_stable_seed(self.seed, sl["table"], sl["cpart"], sl["s"], new_rows))
-        table = relayout(grp.table, lambda v: v.uniform_(-bound, bound, generator=gen))
+        table = relayout(grp.table, lambda v: _uniform_fill(v, bound, gen))
         accu = grp.opt.initial_accu_value if (grp.opt is not None and grp.opt.optimizer_type == Optimizer_t.AdaGrad) \
             else 0.0
         s0 = relayout(grp.s0, lambda v: v.fill_(accu))
@@ -1033,7 +1061,8 @@ class EmbeddingCollection:
     def _hp(self, o: OptParamsPy):
         return {"scaler": self.scaler, "beta1": o.beta1, "beta2": o.beta2, "epsilon": o.epsilon,
                 "lambda1": o.lambda1, "lambda2": o.lambda2, "ftrl_beta": o.beta,
-                "momentum": o.momentum_factor, "initial_accu_value": o.initial_accu_value}
+                "momentum": o.momentum_factor, "initial_accu_value": o.initial_accu_value,
+                "sr_seed": self.sr_seed}
 
     def _accum_update(self, grp, key_bufs, grad_bufs, lr_t, step_t):
         o = grp.opt
@@ -1068,18 +1097,20 @@ class EmbeddingCollection:
 
     # ------------------------------------------------------------------ checkpoint helpers
     def local_table_items(self):
-        """yield (table name, column part, global keys tensor, weight view [rows, ev], group, slice)"""
+        """yield (table name, column part, global keys tensor, weights [rows, ev], group, slice); the
+        weights are fp32 (a view of an fp32 arena, an exact fp32 copy of a bf16 one)"""
         for grp in self.groups:
             for sl in grp.table_slices:
                 w = grp.table[sl["row_off"] * grp.pitch:(sl["row_off"] + sl["rows"]) * grp.pitch] \
-                    .view(sl["rows"], grp.pitch)
+                    .view(sl["rows"], grp.pitch).float()
                 keys = torch.arange(sl["rows"], dtype=torch.int64) * sl["k"] + sl["s"]
                 yield sl["table"], sl, keys, w, grp
 
     def load_table_rows(self, name: str, keys: torch.Tensor, values: torch.Tensor, state=None):
         """Scatter (key, row-vector) pairs of table ``name`` into the local shards (re-sharding on
         load: only keys with key % num_shards == shard_id are kept, parameter_IO.cpp:262-350).
-        ``state``: optional list of per-state [n, ev] tensors (optimizer states)."""
+        ``state``: optional list of per-state [n, ev] tensors (optimizer states).  A bf16 arena stores
+        the values rounded to nearest."""
         keys = keys.to(torch.int64).cpu()
         for grp in self.groups:
             for sl in grp.table_slices:
@@ -1106,7 +1137,7 @@ class EmbeddingCollection:
                     rows = (sl["row_off"] + keys[m] // sl["k"]).to(grp.table.device)
                 c0, ev = sl["col0"], sl["ev"]
                 grp.table.view(-1, grp.pitch)[rows] = values[m][:, c0:c0 + ev].to(grp.table.device,
-                                                                                 torch.float32)
+                                                                                 torch.float32).to(grp.table.dtype)
                 if state is not None:
                     for st, dst in zip(state, (grp.s0, grp.s1)):
                         if dst is not None and st is not None:
@@ -1129,7 +1160,8 @@ class EmbeddingCollection:
         return res
 
     def dump_table_local(self, name: str, only=None):
-        """-> list of (keys int64 [n], values fp32 [n, ev_part], col0, states list) local shards.
+        """-> list of (keys int64 [n], values fp32 [n, ev_part], col0, states list) local shards (a bf16
+        arena's values widen to fp32 exactly).
         ``only``: optional set of part indices to materialise (others are returned as None)."""
         res = []
         for grp in self.groups:
@@ -1140,7 +1172,7 @@ class EmbeddingCollection:
                     res.append(None)
                     continue
                 lo, hi = sl["row_off"], sl["row_off"] + sl["rows"]
-                w = grp.table.view(-1, grp.pitch)[lo:hi].detach().cpu()
+                w = grp.table.view(-1, grp.pitch)[lo:hi].detach().float().cpu()
                 keys = torch.arange(sl["rows"], dtype=torch.int64) * sl["k"] + sl["s"]
                 sts = [None if t is None else t.view(-1, grp.pitch)[lo:hi].detach().float().cpu()
                        for t in (grp.s0, grp.s1)]

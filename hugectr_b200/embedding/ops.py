@@ -59,7 +59,8 @@ class COptHyper(C.Structure):
     _fields_ = [("lr_ptr", C.c_void_p), ("lr_scale", C.c_float), ("scaler", C.c_float),
                 ("beta1", C.c_float), ("beta2", C.c_float), ("epsilon", C.c_float),
                 ("lambda1", C.c_float), ("lambda2", C.c_float), ("ftrl_beta", C.c_float),
-                ("momentum", C.c_float), ("initial_accu", C.c_float), ("step_ptr", C.c_void_p)]
+                ("momentum", C.c_float), ("initial_accu", C.c_float), ("step_ptr", C.c_void_p),
+                ("sr_seed", C.c_uint), ("pad_", C.c_uint)]
 
 
 _lib = None
@@ -70,17 +71,17 @@ def lib():
     if _lib is None:
         l = _native.cuda_lib()
         vp, i, f, ll = C.c_void_p, C.c_int, C.c_float, C.c_longlong
-        l.hctr_emb_forward.argtypes = [C.POINTER(CEmbParams), i, i, i, i, vp]
+        l.hctr_emb_forward.argtypes = [C.POINTER(CEmbParams), i, i, i, i, i, vp]
         l.hctr_emb_backward_accum.argtypes = [C.POINTER(CEmbParams), C.POINTER(CUniqueTable), vp, f,
                                               i, i, i, i, vp]
         l.hctr_emb_update.argtypes = [vp, vp, vp, vp, C.POINTER(CUniqueTable), i, i, i,
-                                      C.POINTER(COptHyper), vp, i, vp]
-        l.hctr_emb_gather_rows.argtypes = [vp, vp, vp, ll, i, i, vp]
+                                      C.POINTER(COptHyper), vp, i, i, vp]
+        l.hctr_emb_gather_rows.argtypes = [vp, vp, vp, ll, i, i, i, vp]
         l.hctr_emb_bwd_index.argtypes = [C.POINTER(CEmbParams), C.POINTER(CUniqueTable),
                                          C.POINTER(CBwdIndex), ll, i, vp]
         l.hctr_emb_bwd_reduce_update.argtypes = [C.POINTER(CEmbParams), C.POINTER(CUniqueTable),
                                                  C.POINTER(CBwdIndex), vp, vp, i, i,
-                                                 C.POINTER(COptHyper), f, i, vp, i, vp]
+                                                 C.POINTER(COptHyper), f, i, vp, i, i, vp]
         for n in ("hctr_emb_forward", "hctr_emb_backward_accum", "hctr_emb_update",
                   "hctr_emb_gather_rows", "hctr_emb_bwd_index", "hctr_emb_bwd_reduce_update"):
             getattr(l, n).restype = i
@@ -305,7 +306,8 @@ def forward(lookups, lookups_dev, table, ev_pitch, key_bufs, out_bufs, batch, my
         max_ev = max((l.ev_size for l in lookups), default=ev_pitch)
         check_ev_size(max_ev)
         al4 = int(vec4_aligned(lookups, ev_pitch, [table, *out_bufs], grad=False))
-        rc = lib().hctr_emb_forward(C.byref(p), max_ev, kb, out_bf16, al4, _st(table.device))
+        rc = lib().hctr_emb_forward(C.byref(p), max_ev, kb, out_bf16, al4, table_bf16(table),
+                                    _st(table.device))
         if rc:
             raise RuntimeError(f"hctr_emb_forward failed rc={rc}")
         D._count()
@@ -504,6 +506,62 @@ def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, b
     ws.ref_rows, ws.ref_grads = rows, grads
 
 
+# ----------------------------------------------------------------------------- bf16 weights
+def table_bf16(table) -> int:
+    """1 when the arena stores bf16 weights (the kernels' WT = __nv_bfloat16), 0 for fp32"""
+    if table.dtype not in (torch.float32, torch.bfloat16):
+        raise TypeError(f"embedding tables are fp32 or bf16, not {table.dtype}")
+    return int(table.dtype == torch.bfloat16)
+
+
+_M64 = (1 << 64) - 1
+
+
+def _fmix64(k):
+    """MurmurHash3 64-bit finaliser on uint64 numpy arrays (fmix64 in csrc/embedding.cuh)"""
+    import numpy as np
+    with np.errstate(over="ignore"):
+        k = k ^ (k >> np.uint64(33))
+        k = k * np.uint64(0xff51afd7ed558ccd)
+        k = k ^ (k >> np.uint64(33))
+        k = k * np.uint64(0xc4ceb9fe1a85ec53)
+        return k ^ (k >> np.uint64(33))
+
+
+def sr_step_key(seed: int, step: int) -> int:
+    """per-(seed, step) key of the stochastic rounding (sr_step_key in csrc/embedding.cuh)"""
+    import numpy as np
+    k = np.array([((int(seed) & 0xFFFFFFFF) << 32) | (int(step) & 0xFFFFFFFF)], dtype=np.uint64)
+    return int(_fmix64(k)[0])
+
+
+def sr_bits(key: int, idx):
+    """the 16 random bits r of the elements at arena indices ``idx`` (int tensor / array of
+    row * pitch + col) under the step key ``key``: 16-bit lane idx % 4 of fmix64(key ^ idx // 4)
+    (one hash per four consecutive elements); uint32 numpy array in [0, 65536)"""
+    import numpy as np
+    i = np.asarray(idx.cpu().numpy() if torch.is_tensor(idx) else idx, dtype=np.int64).astype(np.uint64)
+    h = _fmix64(np.uint64(key & _M64) ^ (i >> np.uint64(2)))
+    return ((h >> (np.uint64(16) * (i & np.uint64(3)))) & np.uint64(0xFFFF)).astype(np.uint32)
+
+
+def sr_round_bf16(x, seed: int, step: int, idx):
+    """bf16 values of the fp32 tensor ``x`` stored with stochastic rounding, bit for bit as the
+    kernels store a bf16 weight: the upper 16 bits of (fp32 bits + r), r = sr_bits of (seed, step,
+    arena index ``idx``, same shape as ``x``); inf / NaN round to nearest.  Unbiased: the expected
+    stored value is ``x``."""
+    import numpy as np
+    xf = x.detach().float().contiguous()
+    b = xf.cpu().numpy().view(np.uint32).reshape(-1)
+    r = sr_bits(sr_step_key(seed, step), torch.as_tensor(idx).reshape(-1))
+    out = ((b.astype(np.uint64) + r) >> np.uint64(16)).astype(np.uint16)
+    res = torch.from_numpy(out.view(np.int16).copy()).view(torch.bfloat16).view(xf.shape)
+    special = torch.from_numpy((b & 0x7f800000) == 0x7f800000).view(xf.shape)
+    if bool(special.any()):
+        res = torch.where(special, xf.cpu().to(torch.bfloat16), res)
+    return res.to(x.device)
+
+
 def sparse_opt_reference(opt: Optimizer_t, w, s0, s1, g, hp, lr, step):
     """Row-block update (w, s0, s1, g all [n, ev] fp32). Returns nothing, updates in place."""
     g = g / hp.get("scaler", 1.0)
@@ -541,6 +599,11 @@ def sparse_opt_reference(opt: Optimizer_t, w, s0, s1, g, hp, lr, step):
         w -= lr * g / (s0.sqrt() + eps)
 
 
+def sr_seed(hp: dict) -> int:
+    """32-bit seed of the stochastic rounding of bf16 weights (``hp["sr_seed"]``, default 0)"""
+    return int(hp.get("sr_seed", 0)) & 0xFFFFFFFF
+
+
 def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: dict, lr_t, step_t,
            num_sms: int = 132):
     """Fused per-unique-row optimizer; consumes and clears the workspace."""
@@ -548,12 +611,13 @@ def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: d
         h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),
                       hp.get("beta2", 0.999), hp.get("epsilon", 1e-7), hp.get("lambda1", 0.0),
                       hp.get("lambda2", 0.0), hp.get("ftrl_beta", 0.0), hp.get("momentum", 0.0),
-                      hp.get("initial_accu_value", 0.0), step_t.data_ptr())
+                      hp.get("initial_accu_value", 0.0), step_t.data_ptr(), sr_seed(hp), 0)
         sbf = int(s0 is not None and s0.dtype == torch.bfloat16)
         rc = lib().hctr_emb_update(table.data_ptr(), 0 if s0 is None else s0.data_ptr(),
                                    0 if s1 is None else s1.data_ptr(), ws.wgrad.data_ptr(),
                                    C.byref(ws.c), ev_pitch, OPT_CODE[opt], sbf, C.byref(h),
-                                   ws.overflow.data_ptr(), num_sms, _st(table.device))
+                                   ws.overflow.data_ptr(), num_sms, table_bf16(table),
+                                   _st(table.device))
         if rc:
             raise RuntimeError("hctr_emb_update failed")
         D._count(2)
@@ -568,16 +632,21 @@ def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: d
 def update_rows(opt: Optimizer_t, table, s0, s1, ev_pitch, rows, grads, hp: dict, lr_t, step_t):
     """One optimizer application per DISTINCT row (``rows`` [n] may repeat, ``grads`` [n, pitch] fp32 are
     summed per row first).  Plain tensor ops on the tables' device: the CPU path of ``update`` and the
-    owner side of the Unique-compression exchange (embedding/unique_exchange.py)."""
+    owner side of the Unique-compression exchange (embedding/unique_exchange.py).  A bf16 table is
+    updated in fp32 and stored with the kernels' stochastic rounding (sr_round_bf16)."""
     if rows.numel() == 0:
         return
     uniq, inv = torch.unique(rows, return_inverse=True)
     g = torch.zeros(uniq.numel(), ev_pitch, dtype=torch.float32, device=grads.device).index_add_(0, inv, grads.float())
     tab = table.view(-1, ev_pitch)
-    w = tab[uniq].clone()
+    w = tab[uniq].float().clone()
     a = None if s0 is None else s0.view(-1, ev_pitch)[uniq].float().clone()
     b = None if s1 is None else s1.view(-1, ev_pitch)[uniq].float().clone()
-    sparse_opt_reference(opt, w, a, b, g, hp, float(lr_t.item()), int(step_t.item()))
+    step = int(step_t.item())
+    sparse_opt_reference(opt, w, a, b, g, hp, float(lr_t.item()), step)
+    if table_bf16(table):
+        idx = uniq.view(-1, 1) * ev_pitch + torch.arange(ev_pitch, device=uniq.device).view(1, -1)
+        w = sr_round_bf16(w, sr_seed(hp), step, idx)
     tab[uniq] = w
     if a is not None:
         s0.view(-1, ev_pitch)[uniq] = a.to(s0.dtype)
@@ -590,7 +659,7 @@ def gather_rows(table, ev_pitch, rows, out):
     if table.is_cuda and rows.dtype == torch.int64:
         rc = lib().hctr_emb_gather_rows(table.data_ptr(), rows.data_ptr(), out.data_ptr(),
                                         rows.numel(), ev_pitch, int(out.dtype == torch.bfloat16),
-                                        _st(table.device))
+                                        table_bf16(table), _st(table.device))
         if rc:
             raise RuntimeError("hctr_emb_gather_rows failed")
         D._count()
@@ -654,13 +723,13 @@ def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_
     h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),
                   hp.get("beta2", 0.999), hp.get("epsilon", 1e-7), hp.get("lambda1", 0.0),
                   hp.get("lambda2", 0.0), hp.get("ftrl_beta", 0.0), hp.get("momentum", 0.0),
-                  hp.get("initial_accu_value", 0.0), step_t.data_ptr())
+                  hp.get("initial_accu_value", 0.0), step_t.data_ptr(), sr_seed(hp), 0)
     sbf = int(s0 is not None and s0.dtype == torch.bfloat16)
     rc = lib().hctr_emb_bwd_reduce_update(C.byref(p), C.byref(ws.c), C.byref(ws.ix),
                                           0 if s0 is None else s0.data_ptr(),
                                           0 if s1 is None else s1.data_ptr(), OPT_CODE[opt], sbf,
                                           C.byref(h), float(grad_scale), gbf, ws.overflow.data_ptr(),
-                                          num_sms, _st(table.device))
+                                          num_sms, table_bf16(table), _st(table.device))
     if rc:
         raise RuntimeError(f"hctr_emb_bwd_reduce_update failed rc={rc}")
     D._count(3)
