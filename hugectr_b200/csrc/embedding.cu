@@ -330,6 +330,54 @@ __global__ void __launch_bounds__(256)
   }
 }
 
+// Row-wise AdaGrad on one row by one warp (accumulate path and data-parallel tables): a warp-reduced
+// pass over the row's fp32 gradient gives sum g^2, lane 0 updates the row's accumulator *s, then the
+// update pass applies the factor to every column and zeroes the gradient.
+template <typename WT>
+HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, float* gsrc, long long base, int ev,
+                                      float inv_scaler, const OptHyper& hp, float lr,
+                                      unsigned long long srk, int lane) {
+  const bool v4 = (ev & 3) == 0;
+  float sq = 0.f;
+  if (v4) {
+    for (int col = lane * 4; col < ev; col += 128) {
+      const float4 g = *reinterpret_cast<const float4*>(gsrc + col);
+      sq += sumsq4(make_float4(g.x * inv_scaler, g.y * inv_scaler, g.z * inv_scaler, g.w * inv_scaler));
+    }
+  } else {
+    for (int col = lane; col < ev; col += 32) {
+      const float g = gsrc[col] * inv_scaler;
+      sq += g * g;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+  float f = 0.f;
+  if (lane == 0) {
+    const float s_new = rowwise_accumulate(*s, sq, ev);
+    *s = s_new;
+    f = rowwise_factor(s_new, hp, lr);
+  }
+  f = __shfl_sync(0xffffffffu, f, 0);
+  if (v4) {
+    for (int col = lane * 4; col < ev; col += 128) {
+      const float4 g = *reinterpret_cast<float4*>(gsrc + col);
+      *reinterpret_cast<float4*>(gsrc + col) = make_float4(0.f, 0.f, 0.f, 0.f);
+      float4 w = load_vec4<WT>(table + base + col);
+      apply_rowwise4(w, make_float4(g.x * inv_scaler, g.y * inv_scaler, g.z * inv_scaler, g.w * inv_scaler), f);
+      store_w4<WT>(table + base + col, w, srk, base + col);
+    }
+  } else {
+    for (int col = lane; col < ev; col += 32) {
+      const float g = gsrc[col] * inv_scaler;
+      gsrc[col] = 0.f;
+      float w = to_f<WT>(table[base + col]);
+      w -= f * g;
+      store_w<WT>(table + base + col, w, srk, base + col);
+    }
+  }
+}
+
 // One warp per unique row: reads the accumulated fp32 gradient (and zeroes it for the next step),
 // updates weight + optimizer state in place and releases the row's hash slot.
 template <int OPT, typename StateT, typename WT>
@@ -353,7 +401,9 @@ __global__ void __launch_bounds__(256)
     const unsigned long long row = ut.rows[uid];
     float* gsrc = wgrad_unique + static_cast<long long>(uid) * ev;
     const long long base = static_cast<long long>(row) * ev;
-    if ((ev & 3) == 0) {
+    if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
+      rowwise_update_warp<WT>(table, s0 + row, gsrc, base, ev, inv_scaler, hp, lr, srk, lane);
+    } else if ((ev & 3) == 0) {
       for (int col = lane * 4; col < ev; col += 128) {
         float4 g = *reinterpret_cast<float4*>(gsrc + col);
         *reinterpret_cast<float4*>(gsrc + col) = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -376,6 +426,23 @@ __global__ void __launch_bounds__(256)
       ut.vals[slot] = kInvalidVal;
     }
   }
+}
+
+// Data-parallel tables with row-wise AdaGrad: every row of the all-reduced dense wgrad [rows, pitch]
+// takes the row rule (one warp per row) and is zeroed.  An all-zero row leaves s and w as they are,
+// as the element-wise AdaGrad of the dense optimizer does.
+__global__ void __launch_bounds__(256)
+    emb_dp_rowwise_update_kernel(float* __restrict__ table, float* __restrict__ s,
+                                 float* __restrict__ wgrad, const long long rows, const int pitch,
+                                 const OptHyper hp) {
+  const float lr = (hp.lr_ptr ? *hp.lr_ptr : 1.f) * hp.lr_scale;
+  const float inv_scaler = 1.f / hp.scaler;
+  const int lane = threadIdx.x & 31;
+  const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  for (long long r = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; r < rows;
+       r += warps)
+    rowwise_update_warp<float>(table, s + r, wgrad + r * pitch, r * pitch, pitch, inv_scaler, hp, lr,
+                               0ull, lane);
 }
 
 __global__ void emb_reset_counter_kernel(unsigned int* counter, unsigned int* overflow_flag,
@@ -549,7 +616,9 @@ extern "C" int hctr_emb_update(void* table, void* s0, void* s1, float* wgrad_uni
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   const int threads = 256;
   const int blocks = num_sms * 8;
-#define LAUNCH_W(O, W)                                                                        \
+  // row-wise AdaGrad: s0 is a [rows] fp32 accumulator indexed by arena row (never bf16)
+  if (opt == OPT_ROWWISE_ADAGRAD && state_bf16) return -7;
+#define LAUNCH_W(O, W)                                                                      \
   if (state_bf16)                                                                             \
     emb_update_kernel<O, __nv_bfloat16, W><<<blocks, threads, 0, st>>>(                      \
         (W*)table, (__nv_bfloat16*)s0, (__nv_bfloat16*)s1, wgrad_unique, *ut, ev, *hp);      \
@@ -566,11 +635,32 @@ extern "C" int hctr_emb_update(void* table, void* s0, void* s1, float* wgrad_uni
     case OPT_MOMENTUM: LAUNCH(OPT_MOMENTUM); break;
     case OPT_NESTEROV: LAUNCH(OPT_NESTEROV); break;
     case OPT_RMSPROP: LAUNCH(OPT_RMSPROP); break;
+    case OPT_ROWWISE_ADAGRAD:
+      if (table_bf16)
+        emb_update_kernel<OPT_ROWWISE_ADAGRAD, float, __nv_bfloat16><<<blocks, threads, 0, st>>>(
+            (__nv_bfloat16*)table, (float*)s0, nullptr, wgrad_unique, *ut, ev, *hp);
+      else
+        emb_update_kernel<OPT_ROWWISE_ADAGRAD, float, float><<<blocks, threads, 0, st>>>(
+            (float*)table, (float*)s0, nullptr, wgrad_unique, *ut, ev, *hp);
+      break;
     default: return -2;
   }
 #undef LAUNCH
 #undef LAUNCH_W
   emb_reset_counter_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
+  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+// Row-wise AdaGrad of a data-parallel table: table [rows, pitch] fp32, s [rows] fp32, wgrad the
+// all-reduced dense gradient [rows, pitch] (zeroed on return)
+extern "C" int hctr_emb_dp_rowwise_update(float* table, float* s, float* wgrad, long long rows,
+                                          int pitch, const OptHyper* hp, int num_sms, void* stream_) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+  if (rows <= 0) return 0;
+  long long blocks = (rows * 32 + 255) / 256;
+  if (blocks > num_sms * 8ll) blocks = num_sms * 8ll;
+  emb_dp_rowwise_update_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(table, s, wgrad, rows,
+                                                                              pitch, *hp);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

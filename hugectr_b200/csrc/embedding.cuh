@@ -214,7 +214,7 @@ HCTR_DEVICE unsigned int unique_get_insert(const UniqueTable& t, unsigned long l
 
 // ------------------------------------------------------------------ fused sparse optimizers
 enum SparseOpt : int { OPT_SGD = 0, OPT_ADAGRAD, OPT_ADAM, OPT_FTRL, OPT_MOMENTUM, OPT_NESTEROV,
-                       OPT_RMSPROP };
+                       OPT_RMSPROP, OPT_ROWWISE_ADAGRAD };
 
 struct OptHyper {
   const float* lr_ptr;    // device learning rate (graph friendly)
@@ -327,5 +327,22 @@ HCTR_DEVICE void apply_opt4_pre(float4& w, const float4 g, const float4 s0v, Sta
   if constexpr (kHasS0) store_vec4<StateT>(s0 + idx, a[0], a[1], a[2], a[3]);
   if constexpr (kHasS1) store_vec4<StateT>(s1 + idx, b[0], b[1], b[2], b[3]);
 }
+
+// Row-wise AdaGrad (OPT_ROWWISE_ADAGRAD): ONE fp32 accumulator per row, s[row] (never bf16).
+//   s += (1/ev) * sum_c g[c]^2 ;  w[c] -= lr * g[c] / (sqrt(s) + eps)  for every column of the row
+// The caller reduces sum_c g[c]^2 over the whole row first (its lanes / warps / block), then calls
+// rowwise_factor once per row, and applies the returned factor f = lr / (sqrt(s) + eps) to every
+// column.  Square root and divisions round to nearest even whatever the fast-math flags, so a row
+// whose update is exact in fp32 is reproduced bit for bit by the CPU path (embedding/ops.py).
+HCTR_DEVICE float rowwise_accumulate(float s, float sumsq, int ev) {
+  return s + __fdiv_rn(sumsq, static_cast<float>(ev));
+}
+HCTR_DEVICE float rowwise_factor(float s_new, const OptHyper& hp, float lr) {
+  return __fdiv_rn(lr, __fsqrt_rn(s_new) + hp.epsilon);
+}
+HCTR_DEVICE void apply_rowwise4(float4& w, const float4 g, float f) {
+  w.x -= f * g.x; w.y -= f * g.y; w.z -= f * g.z; w.w -= f * g.w;
+}
+HCTR_DEVICE float sumsq4(const float4 g) { return g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w; }
 
 }  // namespace hctr

@@ -539,6 +539,65 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       load_a(i + groups, 1, 1);
       const unsigned int uid = rec[0].x;
       const long long base = static_cast<long long>(row[0]) * ev;
+      if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
+        // Row-wise AdaGrad needs the whole row's sum of g^2 before any of its weights is stored.
+        // The gradient sums of all NC chunks stay in registers (they take the place of the
+        // per-element state vectors of the other optimizers), so a row is gathered exactly once
+        // even when it spans two passes (G == 32, ev > 512).  The weights of the first four
+        // chunks and the row's accumulator (one 4-byte load by the group's first lane) are
+        // requested with the gradients; a second pass loads its weights once the factor is known.
+        const unsigned int gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (gi * G));
+        typename Row4<WT>::type wv[4];
+        float4 acc[NC];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const int col = (c * G + gl) * 4;
+          wv[c] = {};
+          if (col < ev) wv[c] = load_row4<WT>(static_cast<const WT*>(p.table) + base + col);
+        }
+        const float s_old = gl == 0 ? s0[row[0]] : 0.f;
+        float sq = 0.f;
+#pragma unroll
+        for (int c = 0; c < NC; ++c) {
+          const int col = (c * G + gl) * 4;
+          acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (col < ev) {
+            float4 g[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+              g[u] = ent[0][u] != 0xFFFFFFFFu ? load_vec4<GradT>(locate_grad<GradT>(p, ent[0][u]) + col)
+                                              : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+              acc[c].x += g[u].x * esc[0][u]; acc[c].y += g[u].y * esc[0][u];
+              acc[c].z += g[u].z * esc[0][u]; acc[c].w += g[u].w * esc[0][u];
+            }
+            acc[c] = make_float4(acc[c].x * inv_scaler, acc[c].y * inv_scaler, acc[c].z * inv_scaler,
+                                 acc[c].w * inv_scaler);
+            sq += sumsq4(acc[c]);
+          }
+        }
+#pragma unroll
+        for (int o = G / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(gmask, sq, o);
+        float f = 0.f;
+        if (gl == 0) {
+          const float s_new = rowwise_accumulate(s_old, sq, ev);
+          s0[row[0]] = s_new;
+          f = rowwise_factor(s_new, hp, lr);
+        }
+        f = __shfl_sync(gmask, f, gi * G);
+#pragma unroll
+        for (int c = 0; c < NC; ++c) {
+          const int col = (c * G + gl) * 4;
+          if (col < ev) {
+            float4 w;
+            if (c < 4) w = widen4(wv[c & 3]);
+            else w = load_vec4<WT>(static_cast<const WT*>(p.table) + base + col);
+            apply_rowwise4(w, acc[c], f);
+            store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
+          }
+        }
+      } else {
       // the row in passes of at most 4 chunks: weights, state and sums of one pass stay within the
       // 128 registers of two resident blocks per SM for G == 32 (8 chunks per lane)
 #pragma unroll
@@ -583,6 +642,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
         }
       }
       }
+      }
       if (gl == 0) {
         const unsigned int slot = ut.slots[uid];
         ut.keys[slot] = kEmptyKey;
@@ -605,6 +665,61 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
     const unsigned int uid = r.x, o0 = r.y;
     const unsigned int o1 = ix.offsets[uid + 1];
     const long long base = static_cast<long long>(ut.rows[uid]) * ev;
+    if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
+      // as the light rows: the sums of all (up to 8) column iterations stay in registers until the
+      // row's sum of g^2 is known, then every column takes the row's factor
+      const unsigned long long arow = ut.rows[uid];
+      const float s_old = lane == 0 ? s0[arow] : 0.f;
+      constexpr int kIters = (G == 8) ? 1 : kMaxEmbWidth / 128;   // G == 8 launches have ev <= 128
+      float4 acc[kIters];
+      float sq = 0.f;
+#pragma unroll
+      for (int c = 0; c < kIters; ++c) {
+        const int col = lane * 4 + c * 128;
+        acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (col < ev) {
+          for (unsigned int j = o0; j < o1; j += 8) {
+            float4 g[8];
+            float sc[8];
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+              g[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+              sc[u] = 0.f;
+              if (j + u < o1) {
+                g[u] = load_vec4<GradT>(locate_grad<GradT>(p, ix.bucket_list[j + u]) + col);
+                sc[u] = has_scale ? ix.bucket_scale[j + u] : 1.f;
+              }
+            }
+#pragma unroll
+            for (int u = 0; u < 8; ++u) {
+              acc[c].x += g[u].x * sc[u]; acc[c].y += g[u].y * sc[u];
+              acc[c].z += g[u].z * sc[u]; acc[c].w += g[u].w * sc[u];
+            }
+          }
+          acc[c] = make_float4(acc[c].x * inv_scaler, acc[c].y * inv_scaler, acc[c].z * inv_scaler,
+                               acc[c].w * inv_scaler);
+          sq += sumsq4(acc[c]);
+        }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+      float f = 0.f;
+      if (lane == 0) {
+        const float s_new = rowwise_accumulate(s_old, sq, ev);
+        s0[arow] = s_new;
+        f = rowwise_factor(s_new, hp, lr);
+      }
+      f = __shfl_sync(0xffffffffu, f, 0);
+#pragma unroll
+      for (int c = 0; c < kIters; ++c) {
+        const int col = lane * 4 + c * 128;
+        if (col < ev) {
+          float4 w = load_vec4<WT>(static_cast<const WT*>(p.table) + base + col);
+          apply_rowwise4(w, acc[c], f);
+          store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
+        }
+      }
+    } else
     for (int col = lane * 4; col < ev; col += 128) {
       float4 w = load_vec4<WT>(static_cast<const WT*>(p.table) + base + col);
       float4 sv = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -712,6 +827,38 @@ __global__ void __launch_bounds__(256)
       const unsigned long long row = ut.rows[uid];
       const long long base = static_cast<long long>(row) * ev;
       const unsigned long long srk = sr_key<WT>(hp.sr_seed, hp.step_ptr);
+      if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
+        // the block reduces the row's sum of g^2 over the scratch row, thread 0 updates the
+        // accumulator once, then every column is applied; scratch is zeroed only by this second read
+        __shared__ float sq_s[8];
+        __shared__ float f_s;
+        float sq = 0.f;
+        for (int c = threadIdx.x; c < ev; c += blockDim.x) {
+          const float g = __ldcg(scratch + c) * inv_scaler;
+          sq += g * g;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+        if (lane == 0) sq_s[warp] = sq;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+          float t = 0.f;
+#pragma unroll
+          for (int w = 0; w < 8; ++w) t += sq_s[w];
+          const float s_new = rowwise_accumulate(s0[row], t, ev);
+          s0[row] = s_new;
+          f_s = rowwise_factor(s_new, hp, lr);
+        }
+        __syncthreads();
+        const float f = f_s;
+        for (int c = threadIdx.x; c < ev; c += blockDim.x) {
+          const float g = __ldcg(scratch + c) * inv_scaler;
+          scratch[c] = 0.f;
+          float w = to_f<WT>(static_cast<const WT*>(p.table)[base + c]);
+          w -= f * g;
+          store_w<WT>(static_cast<WT*>(p.table) + base + c, w, srk, base + c);
+        }
+      } else
       for (int c = threadIdx.x; c < ev; c += blockDim.x) {
         const float g = __ldcg(scratch + c);
         scratch[c] = 0.f;
@@ -843,6 +990,9 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (p->ev_size % 4) return -3;
   if (p->ev_size > kMaxEmbWidth) return -4;
+  // row-wise AdaGrad: s0 is a [rows] fp32 accumulator indexed by arena row (never bf16: a value
+  // that only grows would drop small increments)
+  if (opt == OPT_ROWWISE_ADAGRAD && state_bf16) return -7;
 #define LAUNCH_W(O, W)                                                                             \
   if (state_bf16)                                                                                  \
     launch_reduce<O, __nv_bfloat16, W>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st); \
@@ -858,6 +1008,14 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
     case OPT_MOMENTUM: LAUNCH(OPT_MOMENTUM); break;
     case OPT_NESTEROV: LAUNCH(OPT_NESTEROV); break;
     case OPT_RMSPROP: LAUNCH(OPT_RMSPROP); break;
+    case OPT_ROWWISE_ADAGRAD:
+      if (table_bf16)
+        launch_reduce<OPT_ROWWISE_ADAGRAD, float, __nv_bfloat16>(p, ut, ix, s0, s1, hp, grad_scale,
+                                                                 grad_bf16, num_sms, st);
+      else
+        launch_reduce<OPT_ROWWISE_ADAGRAD, float, float>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16,
+                                                         num_sms, st);
+      break;
     default: return -2;
   }
 #undef LAUNCH

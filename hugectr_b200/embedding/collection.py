@@ -182,14 +182,22 @@ def shard_rows(vocab: int, k: int, s: int) -> int:
 
 # ------------------------------------------------------------------------- runtime
 class _Group:
-    """Local tables of one (kind, ev pitch, weight dtype) group: one arena + optimizer state."""
+    """Local tables of one (kind, ev pitch, weight dtype) group: one arena + optimizer state.
+    Row-wise AdaGrad tables form groups of their own, keyed also by their epsilon and initial value,
+    whose state ``s0`` holds one fp32 accumulator per arena row."""
 
-    def __init__(self, kind, pitch, wdtype="fp32"):
+    def __init__(self, kind, pitch, wdtype="fp32", rowwise=False):
         self.kind, self.pitch, self.wdtype = kind, pitch, wdtype
+        self.rowwise = rowwise
         self.rows = 0
         self.table_slices = []   # (table name, col part, row_off, rows, num_shards, shard_idx, col0)
         self.lookups: List[E.LookupDesc] = []
         self.opt: Optional[OptParamsPy] = None
+
+    @property
+    def state_pitch(self) -> int:
+        """state values per arena row: the pitch, or 1 for row-wise AdaGrad"""
+        return 1 if self.rowwise else self.pitch
 
 
 def fused_backward_ok(grp: _Group) -> bool:
@@ -389,16 +397,20 @@ class EmbeddingCollection:
                 for idx, g in enumerate(pl.shard_gpus):
                     if g == self.rank:
                         parts.append((idx // kk, kk, idx % kk))   # (col part, num row shards, shard)
+            o = t.opt_params or self.default_opt
+            rowwise = o is not None and o.optimizer_type == Optimizer_t.RowWiseAdaGrad
             for (cpart, k, s) in parts:
                 wdt = wdtype[t.name] if pl.kind == "mp" else "fp32"
                 key = (pl.kind, ev_part, wdt)
-                grp = groups.setdefault(key, _Group(pl.kind, ev_part, wdt))
+                if rowwise:
+                    # never shares an arena (and its first table's optimizer) with another optimizer
+                    key += ("rowwise", float(o.epsilon), float(o.initial_accu_value))
+                grp = groups.setdefault(key, _Group(pl.kind, ev_part, wdt, rowwise))
                 rows = t.init_capacity if t.dynamic else shard_rows(t.max_vocabulary_size, k, s)
                 grp.table_slices.append({"table": t.name, "cpart": cpart, "row_off": grp.rows,
                                          "rows": rows, "k": k, "s": s, "col0": cpart * ev_part,
                                          "ev": ev_part, "dynamic": t.dynamic})
                 grp.rows += rows
-                o = t.opt_params or self.default_opt
                 if grp.opt is None:
                     grp.opt = o
         # lookups per group
@@ -446,8 +458,8 @@ class EmbeddingCollection:
         gen = torch.Generator(device="cpu")
         if share_from is not None:
             for grp, src in zip(self.groups, share_from.groups):
-                assert (grp.kind, grp.pitch, grp.wdtype, len(grp.table_slices)) == \
-                    (src.kind, src.pitch, src.wdtype, len(src.table_slices))
+                assert (grp.kind, grp.pitch, grp.wdtype, grp.rowwise, len(grp.table_slices)) == \
+                    (src.kind, src.pitch, src.wdtype, src.rowwise, len(src.table_slices))
                 grp.opt = src.opt
                 grp.ws = None
             self._resync_storage(share_from)     # arrays + row windows (dynamic shards may have grown since)
@@ -465,6 +477,11 @@ class EmbeddingCollection:
             if grp.s0 is not None and grp.opt.optimizer_type == Optimizer_t.AdaGrad \
                     and grp.opt.initial_accu_value != 0.0:
                 grp.s0.fill_(grp.opt.initial_accu_value)
+            if grp.rowwise and self.is_train:
+                # one fp32 accumulator per row, whatever the state dtype (an only-growing bf16 value
+                # would drop small increments)
+                grp.s0 = torch.full((max(grp.rows, 1),), float(grp.opt.initial_accu_value),
+                                    dtype=torch.float32, device=dev)
             R = self.world if grp.kind == "mp" else 1
             po = 0
             for l in grp.lookups:
@@ -851,13 +868,13 @@ class EmbeddingCollection:
 
     def _grow_slice(self, grp, sl, new_rows: int):
         """re-layout ``grp``'s flat arrays with ``sl`` enlarged to ``new_rows`` (slices behind it shift)"""
-        pitch, dev = grp.pitch, self.device
+        dev = self.device
         delta = new_rows - sl["rows"]
-        cut = (sl["row_off"] + sl["rows"]) * pitch           # first element behind the slice
 
-        def relayout(a, fill):
+        def relayout(a, fill, pitch=grp.pitch):
             if a is None:
                 return None
+            cut = (sl["row_off"] + sl["rows"]) * pitch           # first element behind the slice
             out = torch.empty(a.numel() + delta * pitch, dtype=a.dtype, device=dev)
             out[:cut].copy_(a[:cut])
             out[cut + delta * pitch:].copy_(a[cut:])
@@ -870,9 +887,9 @@ class EmbeddingCollection:
         gen = torch.Generator(device=dev)
         gen.manual_seed(_stable_seed(self.seed, sl["table"], sl["cpart"], sl["s"], new_rows))
         table = relayout(grp.table, lambda v: _uniform_fill(v, bound, gen))
-        accu = grp.opt.initial_accu_value if (grp.opt is not None and grp.opt.optimizer_type == Optimizer_t.AdaGrad) \
-            else 0.0
-        s0 = relayout(grp.s0, lambda v: v.fill_(accu))
+        accu = grp.opt.initial_accu_value if (grp.opt is not None and grp.opt.optimizer_type in
+                                              (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad)) else 0.0
+        s0 = relayout(grp.s0, lambda v: v.fill_(accu), grp.state_pitch)
         s1 = relayout(grp.s1, lambda v: v.zero_())
         grp.table, grp.s0, grp.s1 = table, s0, s1
         old_end = sl["row_off"] + sl["rows"]
@@ -1088,6 +1105,9 @@ class EmbeddingCollection:
                     grp.p2p_ar.run()
                 else:
                     self.comm.all_reduce(grp.dense_wgrad)
+            if grp.rowwise:
+                E.dp_rowwise_update(grp.table, grp.s0, grp.dense_wgrad, grp.pitch, self._hp(o), lr_t)
+                return
             dcode = {Optimizer_t.SGD: D.D_SGD, Optimizer_t.AdaGrad: D.D_ADAGRAD,
                      Optimizer_t.Adam: D.D_ADAM, Optimizer_t.Ftrl: D.D_FTRL,
                      Optimizer_t.MomentumSGD: D.D_MOMENTUM, Optimizer_t.Nesterov: D.D_NESTEROV,
@@ -1141,7 +1161,12 @@ class EmbeddingCollection:
                 if state is not None:
                     for st, dst in zip(state, (grp.s0, grp.s1)):
                         if dst is not None and st is not None:
-                            dst.view(-1, grp.pitch)[rows] = st[m][:, c0:c0 + ev].to(dst.device, dst.dtype)
+                            v = st[m][:, c0:c0 + ev]
+                            if grp.rowwise:
+                                # a row's accumulator: the mean of the state over the slice's columns
+                                # (exact for a row-wise file, the natural conversion of an AdaGrad one)
+                                v = v.double().mean(1, keepdim=True).float()
+                            dst.view(-1, grp.state_pitch)[rows] = v.to(dst.device, dst.dtype)
 
     def table_parts(self, name: str):
         """Metadata of the local shards of table ``name`` in ``dump_table_local`` order (no data is
@@ -1174,8 +1199,8 @@ class EmbeddingCollection:
                 lo, hi = sl["row_off"], sl["row_off"] + sl["rows"]
                 w = grp.table.view(-1, grp.pitch)[lo:hi].detach().float().cpu()
                 keys = torch.arange(sl["rows"], dtype=torch.int64) * sl["k"] + sl["s"]
-                sts = [None if t is None else t.view(-1, grp.pitch)[lo:hi].detach().float().cpu()
-                       for t in (grp.s0, grp.s1)]
+                sts = [None if t is None else t.view(-1, grp.state_pitch)[lo:hi].detach().float().cpu()
+                       .expand(hi - lo, grp.pitch).contiguous() for t in (grp.s0, grp.s1)]
                 if sl.get("dynamic"):
                     dk, dr = self._dyn_hash(name, dict(sl, cpart=0)).dump()
                     order = torch.argsort(dk)

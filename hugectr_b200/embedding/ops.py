@@ -19,7 +19,8 @@ from ..ops import dense as D
 
 MAX_RANKS = 16
 OPT_CODE = {Optimizer_t.SGD: 0, Optimizer_t.AdaGrad: 1, Optimizer_t.Adam: 2, Optimizer_t.Ftrl: 3,
-            Optimizer_t.MomentumSGD: 4, Optimizer_t.Nesterov: 5, Optimizer_t.RMSProp: 6}
+            Optimizer_t.MomentumSGD: 4, Optimizer_t.Nesterov: 5, Optimizer_t.RMSProp: 6,
+            Optimizer_t.RowWiseAdaGrad: 7}
 
 
 class CEmbLookup(C.Structure):
@@ -82,8 +83,10 @@ def lib():
         l.hctr_emb_bwd_reduce_update.argtypes = [C.POINTER(CEmbParams), C.POINTER(CUniqueTable),
                                                  C.POINTER(CBwdIndex), vp, vp, i, i,
                                                  C.POINTER(COptHyper), f, i, vp, i, i, vp]
+        l.hctr_emb_dp_rowwise_update.argtypes = [vp, vp, vp, ll, i, C.POINTER(COptHyper), i, vp]
         for n in ("hctr_emb_forward", "hctr_emb_backward_accum", "hctr_emb_update",
-                  "hctr_emb_gather_rows", "hctr_emb_bwd_index", "hctr_emb_bwd_reduce_update"):
+                  "hctr_emb_gather_rows", "hctr_emb_bwd_index", "hctr_emb_bwd_reduce_update",
+                  "hctr_emb_dp_rowwise_update"):
             getattr(l, n).restype = i
         # ABI self-check: ctypes mirrors vs the structs the kernels were compiled with
         if hasattr(l, "hctr_abi_sizes_emb"):
@@ -563,10 +566,15 @@ def sr_round_bf16(x, seed: int, step: int, idx):
 
 
 def sparse_opt_reference(opt: Optimizer_t, w, s0, s1, g, hp, lr, step):
-    """Row-block update (w, s0, s1, g all [n, ev] fp32). Returns nothing, updates in place."""
+    """Row-block update (w, s0, s1, g all [n, ev] fp32; RowWiseAdaGrad: s0 [n], one accumulator per
+    row). Returns nothing, updates in place."""
     g = g / hp.get("scaler", 1.0)
     eps = hp.get("epsilon", 1e-7)
-    if opt == Optimizer_t.SGD:
+    if opt == Optimizer_t.RowWiseAdaGrad:
+        # s += mean_c g^2 ; w -= (lr / (sqrt(s) + eps)) g  -- the factor first, as the kernels do
+        s0 += (g * g).sum(1) / g.shape[1]
+        w -= (lr / (s0.sqrt() + eps)).unsqueeze(1) * g
+    elif opt == Optimizer_t.SGD:
         w -= lr * g
     elif opt == Optimizer_t.AdaGrad:
         s0 += g * g
@@ -640,8 +648,13 @@ def update_rows(opt: Optimizer_t, table, s0, s1, ev_pitch, rows, grads, hp: dict
     g = torch.zeros(uniq.numel(), ev_pitch, dtype=torch.float32, device=grads.device).index_add_(0, inv, grads.float())
     tab = table.view(-1, ev_pitch)
     w = tab[uniq].float().clone()
-    a = None if s0 is None else s0.view(-1, ev_pitch)[uniq].float().clone()
+    # row-wise state: s0 [rows], one accumulator per row
+    rowwise = opt == Optimizer_t.RowWiseAdaGrad
+    spitch = 1 if rowwise else ev_pitch
+    a = None if s0 is None else s0.view(-1, spitch)[uniq].float().clone()
     b = None if s1 is None else s1.view(-1, ev_pitch)[uniq].float().clone()
+    if rowwise and a is not None:
+        a = a.view(-1)
     step = int(step_t.item())
     sparse_opt_reference(opt, w, a, b, g, hp, float(lr_t.item()), step)
     if table_bf16(table):
@@ -649,9 +662,32 @@ def update_rows(opt: Optimizer_t, table, s0, s1, ev_pitch, rows, grads, hp: dict
         w = sr_round_bf16(w, sr_seed(hp), step, idx)
     tab[uniq] = w
     if a is not None:
-        s0.view(-1, ev_pitch)[uniq] = a.to(s0.dtype)
+        s0.view(-1, spitch)[uniq] = a.view(-1, spitch).to(s0.dtype)
     if b is not None:
         s1.view(-1, ev_pitch)[uniq] = b.to(s1.dtype)
+
+
+def dp_rowwise_update(table, s0, wgrad, pitch, hp: dict, lr_t, num_sms: int = 132):
+    """Row-wise AdaGrad of a data-parallel table from its all-reduced dense gradient ``wgrad``
+    ([rows * pitch] fp32, zeroed on return): every row takes the row rule; an all-zero row keeps its
+    weights and accumulator (``s0`` [rows] fp32)."""
+    rows = table.numel() // pitch
+    if table.is_cuda:
+        h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), 0.9, 0.999, hp.get("epsilon", 1e-7),
+                      0.0, 0.0, 0.0, 0.0, hp.get("initial_accu_value", 0.0), None, 0, 0)
+        rc = lib().hctr_emb_dp_rowwise_update(table.data_ptr(), s0.data_ptr(), wgrad.data_ptr(), rows,
+                                              pitch, C.byref(h), num_sms, _st(table.device))
+        if rc:
+            raise RuntimeError(f"hctr_emb_dp_rowwise_update failed rc={rc}")
+        D._count()
+        return
+    g = wgrad[:rows * pitch].view(rows, pitch)
+    w = table.view(rows, pitch).clone()
+    a = s0.clone()
+    sparse_opt_reference(Optimizer_t.RowWiseAdaGrad, w, a, None, g.clone(), hp, float(lr_t.item()), 1)
+    table.view(rows, pitch).copy_(w)
+    s0.copy_(a)
+    wgrad.zero_()
 
 
 def gather_rows(table, ev_pitch, rows, out):

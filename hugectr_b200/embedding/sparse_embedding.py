@@ -41,6 +41,8 @@ from .hashtable import HashTable
 class SparseEmbeddingRuntime:
     def __init__(self, cfg, param, layout, batch_per_gpu, device, act_dtype, comm, opt, key_dtype,
                  scaler=1.0, seed=0, share_from=None):
+        from ..solver import check_not_rowwise
+        check_not_rowwise(opt, "a legacy sparse embedding (also with CreateETC / offloaded tables)")
         self.cfg, self.param, self.layout = cfg, param, layout
         self.name = cfg.sparse_embedding_name
         self.top_name = cfg.sparse_embedding_name

@@ -136,6 +136,8 @@ class Optimizer_t(Enum):
     MomentumSGD = 4
     Nesterov = 5
     SGD = 6
+    # embedding-collection tables only: one fp32 accumulator per row (docs/embedding.md)
+    RowWiseAdaGrad = 7
 
 
 class Update_t(Enum):
@@ -230,4 +232,5 @@ OPT_STATES_PER_WEIGHT = {
     Optimizer_t.MomentumSGD: 1,
     Optimizer_t.Nesterov: 1,
     Optimizer_t.SGD: 0,
+    Optimizer_t.RowWiseAdaGrad: 0,   # one value per row, not per weight
 }

@@ -26,7 +26,8 @@ from .lr_scheduler import LearningRateScheduler
 from .network import Network, insert_fanout_slices
 from .ops import dense as D
 from .parallel.comm import Comm
-from .solver import (DataReaderParams, DenseLayer, Input, OptParamsPy, Solver, SparseEmbedding)
+from .solver import (DataReaderParams, DenseLayer, Input, OptParamsPy, Solver, SparseEmbedding,
+                     check_not_rowwise)
 from .utils import logger
 
 DENSE_OPT_CODE = {Optimizer_t.SGD: D.D_SGD, Optimizer_t.AdaGrad: D.D_ADAGRAD,
@@ -50,6 +51,7 @@ class Model:
         self.solver = solver
         self.etc = etc                 # hugectr.CreateETC(...): host parameter server + gpu_cache per embedding
         self.reader_params = reader_params
+        check_not_rowwise(opt_params, "the model optimizer (dense layers have no embedding rows)")
         self.opt_params = opt_params or OptParamsPy()
         self.comm = comm or Comm.init_from_env()
         self.device = self.comm.device

@@ -44,7 +44,15 @@ def build_dlrm_dcnv2(batchsize: int = 55296, num_gpus: int = 8, table_sizes: Opt
                      mixed: bool = True, scaler: float = 1.0, source=None, shard_plan=None,
                      optimizer: str = "adagrad", bottom=(512, 256, 128),
                      top=(1024, 1024, 512, 256, 1), cross_layers: int = 3, projection_dim: int = 512,
-                     comm=None, comm_strategy=None, compression_strategy=None, **solver_kw) -> "hugectr.Model":
+                     comm=None, comm_strategy=None, compression_strategy=None,
+                     embedding_optimizer: str = "adagrad", weight_dtype: str = "fp32",
+                     **solver_kw) -> "hugectr.Model":
+    """``embedding_optimizer``: "adagrad" (the model optimizer for every table) or "rowwise_adagrad"
+    (every table gets row-wise AdaGrad with the model optimizer's epsilon and initial value, one fp32
+    accumulator per row; the dense layers keep the model optimizer).  ``weight_dtype``: "fp32" or
+    "bf16" storage of the tables' weights."""
+    if embedding_optimizer not in ("adagrad", "rowwise_adagrad"):
+        raise ValueError(f"embedding_optimizer must be 'adagrad' or 'rowwise_adagrad', not {embedding_optimizer!r}")
     table_sizes = list(table_sizes or CRITEO_TB_TABLE_SIZES)
     multi_hot = list(multi_hot or CRITEO_TB_MULTI_HOT)
     n = len(table_sizes)
@@ -67,8 +75,13 @@ def build_dlrm_dcnv2(batchsize: int = 55296, num_gpus: int = 8, table_sizes: Opt
         data_reader_sparse_param_array=[
             hugectr.DataReaderSparseParam(f"data{i}", multi_hot[i], True, 1) for i in range(n)]))
     evs = [int(ev_size)] * n if isinstance(ev_size, int) else [int(e) for e in ev_size]   # per-table widths
+    table_opt = None
+    if embedding_optimizer == "rowwise_adagrad":
+        table_opt = hugectr.CreateOptimizer(hugectr.Optimizer_t.RowWiseAdaGrad, hugectr.Update_t.Global,
+                                            initial_accu_value=opt.initial_accu_value, epsilon=opt.epsilon)
     tables = [hugectr.EmbeddingTableConfig(name=str(i), max_vocabulary_size=table_sizes[i],
-                                           ev_size=evs[i]) for i in range(n)]
+                                           ev_size=evs[i], opt_params=table_opt, weight_dtype=weight_dtype)
+              for i in range(n)]
     ebc = hugectr.EmbeddingCollectionConfig(
         use_exclusive_keys=True, comm_strategy=comm_strategy or hugectr.CommunicationStrategy.Uniform)
     ebc.embedding_lookup(table_config=tables, bottom_name=[f"data{i}" for i in range(n)],

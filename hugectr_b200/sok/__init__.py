@@ -478,6 +478,8 @@ class OptimizerWrapper:
     per-variable slot tensors, consumes ``var.sparse_grad``."""
 
     def __init__(self, optimizer: Optimizer_t = Optimizer_t.SGD, lr: float = 0.01, **hp):
+        from ..solver import check_not_rowwise
+        check_not_rowwise(optimizer, "sok.OptimizerWrapper")
         self.opt, self.lr, self.hp = optimizer, lr, hp
         self.step = 0
 

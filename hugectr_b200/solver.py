@@ -123,8 +123,8 @@ class OptParamsPy:
     lambda2: float = 0.0        # ftrl
     beta1: float = 0.9          # adam
     beta2: float = 0.999        # adam
-    epsilon: float = 1e-7       # adam / adagrad
-    initial_accu_value: float = 0.0  # adagrad
+    epsilon: float = 1e-7       # adam / adagrad / row-wise adagrad
+    initial_accu_value: float = 0.0  # adagrad / row-wise adagrad
     momentum_factor: float = 0.0     # momentum sgd / nesterov
     atomic_update: bool = True       # sgd
     initialized: bool = True
@@ -141,7 +141,7 @@ class OptParamsPy:
         d = {"type": t.name, "update_type": self.update_type.name}
         if t == Optimizer_t.Adam:
             d["adam_hparam"] = {"beta1": self.beta1, "beta2": self.beta2, "epsilon": self.epsilon}
-        elif t == Optimizer_t.AdaGrad:
+        elif t in (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad):
             d["adagrad_hparam"] = {"initial_accu_value": self.initial_accu_value,
                                    "epsilon": self.epsilon}
         elif t == Optimizer_t.Ftrl:
@@ -166,6 +166,16 @@ class OptParamsPy:
                 if hasattr(o, k):
                     setattr(o, k, v)
         return o
+
+
+def check_not_rowwise(opt: Optional[OptParamsPy], where: str) -> None:
+    """Row-wise AdaGrad keeps one accumulator per embedding row: only embedding-collection tables
+    have it.  Raises ValueError for any other user of an optimizer (``where``)."""
+    t = getattr(opt, "optimizer_type", opt)
+    if t == Optimizer_t.RowWiseAdaGrad:
+        raise ValueError(f"Optimizer_t.RowWiseAdaGrad is not supported for {where}; it applies to "
+                         "embedding-collection tables only: pass it per table with "
+                         "EmbeddingTableConfig(opt_params=...)")
 
 
 def CreateOptimizer(optimizer_type=Optimizer_t.Adam, update_type=Update_t.Global, beta: float = 0.0,
@@ -285,6 +295,7 @@ class SparseEmbedding:
                  max_vocabulary_size_per_gpu: int = 0):
         if combiner not in ("sum", "mean"):
             raise ValueError("combiner must be 'sum' or 'mean'")
+        check_not_rowwise(optimizer, "a legacy SparseEmbedding")
         self.embedding_type = embedding_type
         self.workspace_size_per_gpu_in_mb = int(workspace_size_per_gpu_in_mb)
         self.embedding_vec_size = int(embedding_vec_size)

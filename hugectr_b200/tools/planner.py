@@ -86,7 +86,8 @@ def plan_tables(table_sizes: Sequence[int], hotness: Sequence[int], ev_sizes, nu
                 global_batch: int = 65536, combiners: Sequence[str] = None, num_nodes: int = 1,
                 hw: HardwareModel = None, weight_bytes: int = 4, state_bytes: int = 4,
                 act_bytes: int = 2, dp_threshold_bytes: float = 4e6, min_rows_per_shard: int = 1024,
-                min_cols_per_shard: int = 32, balance_tol: float = 1.10, per_key_bytes: float = 96.0):
+                min_cols_per_shard: int = 32, balance_tol: float = 1.10, per_key_bytes: float = 96.0,
+                state_row_bytes: int = 0):
     """Plan for tables of different widths and combiners (the role of the reference's larger planner,
     benchmarks/embedding_collection/hugectr/sharding/planner.py:38-620: cost model with per-table
     ev sizes, hot-shard / out-of-memory splits that may be column-wise, hierarchical mode).
@@ -106,6 +107,9 @@ def plan_tables(table_sizes: Sequence[int], hotness: Sequence[int], ev_sizes, nu
     longest-first on the least-loaded GPU that does not hold the table yet (same node for the shards
     of one table when ``num_nodes`` > 1) and that has memory left.
 
+    ``state_bytes`` is optimizer state per weight, ``state_row_bytes`` per row and column slice (row-wise
+    AdaGrad: 4, with ``state_bytes=0``); both enter the memory and update terms.
+
     Returns (shard_matrix, shard_strategy, report); strategy entries are ``name`` or
     ``(name, column_wise_factor)``."""
     hw = hw or HardwareModel()
@@ -117,7 +121,7 @@ def plan_tables(table_sizes: Sequence[int], hotness: Sequence[int], ev_sizes, nu
     link = hw.nvlink if num_nodes == 1 else (hw.nvlink * (gpn - 1) + hw.internode * (num_gpus - gpn)) / max(1, num_gpus - 1)
 
     def mem(t, k=1, c=1):
-        return table_sizes[t] * evs[t] * (weight_bytes + state_bytes) / (k * c)
+        return table_sizes[t] * (evs[t] * (weight_bytes + state_bytes) / c + state_row_bytes) / k
 
     def vec_per_sample(t):
         return hotness[t] if comb[t] == "concat" else 1
@@ -126,7 +130,8 @@ def plan_tables(table_sizes: Sequence[int], hotness: Sequence[int], ev_sizes, nu
         keys = global_batch * hotness[t] / k
         row = evs[t] / c
         lookup = keys * row * weight_bytes / (hw.hbm * hw.gather_eff)
-        update = 2.0 * min(keys, table_sizes[t] / k) * row * (weight_bytes + state_bytes) / (hw.hbm * hw.update_eff) \
+        update = 2.0 * min(keys, table_sizes[t] / k) * (row * (weight_bytes + state_bytes) + state_row_bytes) \
+            / (hw.hbm * hw.update_eff) \
             + keys * row * act_bytes / hw.hbm
         exch = 2.0 * global_batch * vec_per_sample(t) * row * act_bytes * (num_gpus - 1) / num_gpus / link
         return lookup + update + exch + keys * per_key_bytes / hw.hbm
@@ -135,7 +140,7 @@ def plan_tables(table_sizes: Sequence[int], hotness: Sequence[int], ev_sizes, nu
         keys = global_batch / num_gpus * hotness[t]
         lookup = keys * evs[t] * weight_bytes / (hw.hbm * hw.gather_eff)
         allreduce = 2.0 * table_sizes[t] * evs[t] * 4 / link
-        dense_update = 3.0 * table_sizes[t] * evs[t] * (weight_bytes + state_bytes) / hw.hbm
+        dense_update = 3.0 * table_sizes[t] * (evs[t] * (weight_bytes + state_bytes) + state_row_bytes) / hw.hbm
         return lookup + allreduce + dense_update + keys * per_key_bytes / hw.hbm
 
     if num_gpus == 1:
