@@ -445,8 +445,8 @@ __global__ void __launch_bounds__(256)
                                0ull, lane);
 }
 
-__global__ void emb_reset_counter_kernel(unsigned int* counter, unsigned int* overflow_flag,
-                                         unsigned int max_unique) {
+__global__ void emb_finish_kernel(unsigned int* counter, unsigned int* overflow_flag,
+                                  unsigned int max_unique) {
   if (*counter > max_unique) atomicMax(overflow_flag, *counter);
   *counter = 0;
 }
@@ -616,38 +616,14 @@ extern "C" int hctr_emb_update(void* table, void* s0, void* s1, float* wgrad_uni
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   const int threads = 256;
   const int blocks = num_sms * 8;
-  // row-wise AdaGrad: s0 is a [rows] fp32 accumulator indexed by arena row (never bf16)
-  if (opt == OPT_ROWWISE_ADAGRAD && state_bf16) return -7;
-#define LAUNCH_W(O, W)                                                                      \
-  if (state_bf16)                                                                             \
-    emb_update_kernel<O, __nv_bfloat16, W><<<blocks, threads, 0, st>>>(                      \
-        (W*)table, (__nv_bfloat16*)s0, (__nv_bfloat16*)s1, wgrad_unique, *ut, ev, *hp);      \
-  else                                                                                        \
-    emb_update_kernel<O, float, W><<<blocks, threads, 0, st>>>((W*)table, (float*)s0,         \
-                                                               (float*)s1, wgrad_unique, *ut, ev, *hp);
-#define LAUNCH(O) \
-  if (table_bf16) { LAUNCH_W(O, __nv_bfloat16) } else { LAUNCH_W(O, float) }
-  switch (opt) {
-    case OPT_SGD: LAUNCH(OPT_SGD); break;
-    case OPT_ADAGRAD: LAUNCH(OPT_ADAGRAD); break;
-    case OPT_ADAM: LAUNCH(OPT_ADAM); break;
-    case OPT_FTRL: LAUNCH(OPT_FTRL); break;
-    case OPT_MOMENTUM: LAUNCH(OPT_MOMENTUM); break;
-    case OPT_NESTEROV: LAUNCH(OPT_NESTEROV); break;
-    case OPT_RMSPROP: LAUNCH(OPT_RMSPROP); break;
-    case OPT_ROWWISE_ADAGRAD:
-      if (table_bf16)
-        emb_update_kernel<OPT_ROWWISE_ADAGRAD, float, __nv_bfloat16><<<blocks, threads, 0, st>>>(
-            (__nv_bfloat16*)table, (float*)s0, nullptr, wgrad_unique, *ut, ev, *hp);
-      else
-        emb_update_kernel<OPT_ROWWISE_ADAGRAD, float, float><<<blocks, threads, 0, st>>>(
-            (float*)table, (float*)s0, nullptr, wgrad_unique, *ut, ev, *hp);
-      break;
-    default: return -2;
-  }
-#undef LAUNCH
-#undef LAUNCH_W
-  emb_reset_counter_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
+  const int rc = dispatch_opt(opt, state_bf16, table_bf16, [&](auto o, auto s, auto w) {
+    using StateT = typename decltype(s)::type;
+    using WT = typename decltype(w)::type;
+    emb_update_kernel<decltype(o)::value, StateT, WT><<<blocks, threads, 0, st>>>(
+        (WT*)table, (StateT*)s0, (StateT*)s1, wgrad_unique, *ut, ev, *hp);
+  });
+  if (rc) return rc;
+  emb_finish_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "ptx.cuh"
 
 namespace hctr {
@@ -344,5 +346,46 @@ HCTR_DEVICE void apply_rowwise4(float4& w, const float4 g, float f) {
   w.x -= f * g.x; w.y -= f * g.y; w.z -= f * g.z; w.w -= f * g.w;
 }
 HCTR_DEVICE float sumsq4(const float4 g) { return g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w; }
+
+// Clears the counter of unique rows after an update and records an overflow of it (the update kernels
+// release their rows' hash slots, so the table is empty again)
+__global__ void emb_finish_kernel(unsigned int* counter, unsigned int* overflow_flag, unsigned int max_unique);
+
+// Host dispatch of the sparse optimizers: calls fn(std::integral_constant<int, OPT>, Tag<StateT>,
+// Tag<WT>) with the kernels' template arguments for optimizer `opt`, state type (bf16 when state_bf16)
+// and weight type (bf16 when table_bf16).  SGD (no state) and row-wise AdaGrad (a [rows] fp32
+// accumulator, never bf16: a value that only grows would drop small increments) run with the fp32 state
+// type.  Returns 0, -2 for an unknown optimizer, or -7 for row-wise AdaGrad with bf16 state.
+template <typename T>
+struct Tag {
+  using type = T;
+};
+template <typename Fn>
+inline int dispatch_opt(int opt, int state_bf16, int table_bf16, Fn&& fn) {
+  auto run = [&](auto o) {
+    constexpr int O = decltype(o)::value;
+    auto with_w = [&](auto s) {
+      if (table_bf16) fn(o, s, Tag<__nv_bfloat16>{});
+      else fn(o, s, Tag<float>{});
+    };
+    if constexpr (O != OPT_SGD && O != OPT_ROWWISE_ADAGRAD) {
+      if (state_bf16) return with_w(Tag<__nv_bfloat16>{});
+    }
+    with_w(Tag<float>{});
+  };
+  if (opt == OPT_ROWWISE_ADAGRAD && state_bf16) return -7;
+  switch (opt) {
+    case OPT_SGD: run(std::integral_constant<int, OPT_SGD>{}); break;
+    case OPT_ADAGRAD: run(std::integral_constant<int, OPT_ADAGRAD>{}); break;
+    case OPT_ADAM: run(std::integral_constant<int, OPT_ADAM>{}); break;
+    case OPT_FTRL: run(std::integral_constant<int, OPT_FTRL>{}); break;
+    case OPT_MOMENTUM: run(std::integral_constant<int, OPT_MOMENTUM>{}); break;
+    case OPT_NESTEROV: run(std::integral_constant<int, OPT_NESTEROV>{}); break;
+    case OPT_RMSPROP: run(std::integral_constant<int, OPT_RMSPROP>{}); break;
+    case OPT_ROWWISE_ADAGRAD: run(std::integral_constant<int, OPT_ROWWISE_ADAGRAD>{}); break;
+    default: return -2;
+  }
+  return 0;
+}
 
 }  // namespace hctr

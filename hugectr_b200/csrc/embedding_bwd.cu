@@ -877,14 +877,6 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// (heavy rows past the caps take the medium path, see emb_bwd_classify_kernel: only the unique-row
-// capacity can overflow)
-__global__ void emb_bwd_finish_kernel(unsigned int* counter, unsigned int* overflow_flag,
-                                      unsigned int max_unique) {
-  if (*counter > max_unique) atomicMax(overflow_flag, *counter);
-  *counter = 0;
-}
-
 }  // namespace hctr
 
 using namespace hctr;
@@ -942,7 +934,7 @@ struct SideStream {
 static SideStream g_heavy_side;
 
 template <int OPT, typename StateT, typename WT>
-static int launch_reduce(const EmbParams* p, const UniqueTable* ut, const BwdIndex* ix, void* s0,
+static void launch_reduce(const EmbParams* p, const UniqueTable* ut, const BwdIndex* ix, void* s0,
                          void* s1, const OptHyper* hp, float grad_scale, int grad_bf16, int num_sms,
                          cudaStream_t st) {
   const size_t smem = 8 * static_cast<size_t>(p->ev_size) * sizeof(float);
@@ -979,7 +971,6 @@ static int launch_reduce(const EmbParams* p, const UniqueTable* ut, const BwdInd
           *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
   }
   if (fork) cudaStreamWaitEvent(st, g_heavy_side.join, 0);
-  return 0;
 }
 
 extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable* ut,
@@ -990,36 +981,13 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (p->ev_size % 4) return -3;
   if (p->ev_size > kMaxEmbWidth) return -4;
-  // row-wise AdaGrad: s0 is a [rows] fp32 accumulator indexed by arena row (never bf16: a value
-  // that only grows would drop small increments)
-  if (opt == OPT_ROWWISE_ADAGRAD && state_bf16) return -7;
-#define LAUNCH_W(O, W)                                                                             \
-  if (state_bf16)                                                                                  \
-    launch_reduce<O, __nv_bfloat16, W>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st); \
-  else                                                                                             \
-    launch_reduce<O, float, W>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st);
-#define LAUNCH(O) \
-  if (table_bf16) { LAUNCH_W(O, __nv_bfloat16) } else { LAUNCH_W(O, float) }
-  switch (opt) {
-    case OPT_SGD: LAUNCH(OPT_SGD); break;
-    case OPT_ADAGRAD: LAUNCH(OPT_ADAGRAD); break;
-    case OPT_ADAM: LAUNCH(OPT_ADAM); break;
-    case OPT_FTRL: LAUNCH(OPT_FTRL); break;
-    case OPT_MOMENTUM: LAUNCH(OPT_MOMENTUM); break;
-    case OPT_NESTEROV: LAUNCH(OPT_NESTEROV); break;
-    case OPT_RMSPROP: LAUNCH(OPT_RMSPROP); break;
-    case OPT_ROWWISE_ADAGRAD:
-      if (table_bf16)
-        launch_reduce<OPT_ROWWISE_ADAGRAD, float, __nv_bfloat16>(p, ut, ix, s0, s1, hp, grad_scale,
-                                                                 grad_bf16, num_sms, st);
-      else
-        launch_reduce<OPT_ROWWISE_ADAGRAD, float, float>(p, ut, ix, s0, s1, hp, grad_scale, grad_bf16,
-                                                         num_sms, st);
-      break;
-    default: return -2;
-  }
-#undef LAUNCH
-#undef LAUNCH_W
-  emb_bwd_finish_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
+  const int rc = dispatch_opt(opt, state_bf16, table_bf16, [&](auto o, auto s, auto w) {
+    launch_reduce<decltype(o)::value, typename decltype(s)::type, typename decltype(w)::type>(
+        p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st);
+  });
+  if (rc) return rc;
+  // heavy rows past the caps take the medium path (emb_bwd_classify_kernel): only the unique-row
+  // capacity can overflow
+  emb_finish_kernel<<<1, 1, 0, st>>>(ut->counter, overflow_flag, ut->max_unique);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

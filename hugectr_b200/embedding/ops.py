@@ -612,14 +612,21 @@ def sr_seed(hp: dict) -> int:
     return int(hp.get("sr_seed", 0)) & 0xFFFFFFFF
 
 
+def _opt_hyper(hp: dict, lr_t, step_t) -> COptHyper:
+    """Kernel hyper-parameters: the device learning rate ``lr_t`` and step counter ``step_t`` (None: the
+    kernels take step 1) with the optimizer's values from ``hp``."""
+    return COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),
+                     hp.get("beta2", 0.999), hp.get("epsilon", 1e-7), hp.get("lambda1", 0.0),
+                     hp.get("lambda2", 0.0), hp.get("ftrl_beta", 0.0), hp.get("momentum", 0.0),
+                     hp.get("initial_accu_value", 0.0), None if step_t is None else step_t.data_ptr(),
+                     sr_seed(hp), 0)
+
+
 def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: dict, lr_t, step_t,
            num_sms: int = 132):
     """Fused per-unique-row optimizer; consumes and clears the workspace."""
     if table.is_cuda:
-        h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),
-                      hp.get("beta2", 0.999), hp.get("epsilon", 1e-7), hp.get("lambda1", 0.0),
-                      hp.get("lambda2", 0.0), hp.get("ftrl_beta", 0.0), hp.get("momentum", 0.0),
-                      hp.get("initial_accu_value", 0.0), step_t.data_ptr(), sr_seed(hp), 0)
+        h = _opt_hyper(hp, lr_t, step_t)
         sbf = int(s0 is not None and s0.dtype == torch.bfloat16)
         rc = lib().hctr_emb_update(table.data_ptr(), 0 if s0 is None else s0.data_ptr(),
                                    0 if s1 is None else s1.data_ptr(), ws.wgrad.data_ptr(),
@@ -673,8 +680,7 @@ def dp_rowwise_update(table, s0, wgrad, pitch, hp: dict, lr_t, num_sms: int = 13
     weights and accumulator (``s0`` [rows] fp32)."""
     rows = table.numel() // pitch
     if table.is_cuda:
-        h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), 0.9, 0.999, hp.get("epsilon", 1e-7),
-                      0.0, 0.0, 0.0, 0.0, hp.get("initial_accu_value", 0.0), None, 0, 0)
+        h = _opt_hyper(hp, lr_t, None)
         rc = lib().hctr_emb_dp_rowwise_update(table.data_ptr(), s0.data_ptr(), wgrad.data_ptr(), rows,
                                               pitch, C.byref(h), num_sms, _st(table.device))
         if rc:
@@ -756,10 +762,7 @@ def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_
                          "(see vec4_aligned); use backward_accum + update")
     p, kb, gbf = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch,
                               my_rank, nnz_bufs, key_bytes, act_bf16)
-    h = COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),
-                  hp.get("beta2", 0.999), hp.get("epsilon", 1e-7), hp.get("lambda1", 0.0),
-                  hp.get("lambda2", 0.0), hp.get("ftrl_beta", 0.0), hp.get("momentum", 0.0),
-                  hp.get("initial_accu_value", 0.0), step_t.data_ptr(), sr_seed(hp), 0)
+    h = _opt_hyper(hp, lr_t, step_t)
     sbf = int(s0 is not None and s0.dtype == torch.bfloat16)
     rc = lib().hctr_emb_bwd_reduce_update(C.byref(p), C.byref(ws.c), C.byref(ws.ix),
                                           0 if s0 is None else s0.data_ptr(),

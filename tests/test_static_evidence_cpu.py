@@ -27,5 +27,6 @@ def test_kernel_resource_report_and_spill_gate():
                        capture_output=True, text=True, timeout=600)
     assert r.returncode == 0, r.stdout[-2000:] + r.stderr
     names = r.stdout
-    for k in ("gemm_tc_kernel", "gemm_mxfp8_kernel", "emb_fwd_kernel", "emb_dispatch_kernel", "allreduce_twoshot_kernel"):
+    for k in ("gemm_tc_kernel", "gemm_mxfp8_kernel", "emb_fwd_kernel", "emb_dispatch_kernel", "allreduce_twoshot_kernel",
+              "emb_bwd_reduce_update_kernel", "emb_bwd_heavy_kernel", "emb_update_kernel"):
         assert k in names, k
