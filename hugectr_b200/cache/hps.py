@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from ..enums import TrainPSType_t
-from ..embedding import ops as E
+from ..ops.optim import opt_hp, opt_reference
 from .gpu_cache import GpuCache
 
 
@@ -311,9 +311,7 @@ class OffloadedEmbedding:
         s0 = self.states[0] if len(self.states) > 0 else None
         s1 = self.states[1] if len(self.states) > 1 else None
         o = self.opt
-        hp = {"beta1": o.beta1, "beta2": o.beta2, "epsilon": o.epsilon, "lambda1": o.lambda1,
-              "lambda2": o.lambda2, "ftrl_beta": o.beta, "momentum": o.momentum_factor}
-        E.sparse_opt_reference(o.optimizer_type, w, s0, s1, gu, hp, self.lr, step)
+        opt_reference(o.optimizer_type, w, s0, s1, gu, opt_hp(o), self.lr, step)
         self.cache.update(self.uniq, w)
         for c, s in zip(self.state_cache, (s0, s1)):
             if s is not None:

@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "optim.cuh"
 #include "ptx.cuh"
 
 namespace hctr {
@@ -15,8 +16,6 @@ namespace hctr {
 using bf16 = __nv_bfloat16;
 
 // ------------------------------------------------------------------ dense optimizers
-enum DenseOpt : int { D_SGD = 0, D_ADAGRAD, D_ADAM, D_FTRL, D_MOMENTUM, D_NESTEROV, D_RMSPROP };
-
 struct DenseOptArgs {
   float* w;            // fp32 master weights (flat)
   float* g;            // fp32 wgrad (flat) ; zeroed after use when zero_grad
@@ -24,20 +23,22 @@ struct DenseOptArgs {
   float* s0;
   float* s1;
   long long n;
-  const float* lr_ptr;
-  const unsigned int* step_ptr;
-  float scaler, beta1, beta2, epsilon, lambda1, lambda2, ftrl_beta, momentum;
+  OptHyper hp;         // the rule's hyper-parameters, device learning rate and step counter
   int zero_grad;
 };
 
 template <int OPT>
 __global__ void __launch_bounds__(256) dense_opt_kernel(const DenseOptArgs a) {
-  const float lr = *a.lr_ptr;
-  const float inv_scaler = 1.f / a.scaler;
-  float alpha = lr;
-  if constexpr (OPT == D_ADAM) {
-    const float t = static_cast<float>(*a.step_ptr);
-    alpha = lr * sqrtf(1.f - powf(a.beta2, t)) / (1.f - powf(a.beta1, t));
+  constexpr bool kHasS0 = OPT != OPT_SGD;
+  constexpr bool kHasS1 = OPT == OPT_ADAM || OPT == OPT_FTRL;
+  const OptHyper& hp = a.hp;
+  const float lr = *hp.lr_ptr * hp.lr_scale;
+  const float inv_scaler = 1.f / hp.scaler;
+  float bc1 = 1.f, bc2 = 1.f;
+  if constexpr (OPT == OPT_ADAM) {
+    const float t = static_cast<float>(*hp.step_ptr);
+    bc1 = 1.f - powf(hp.beta1, t);
+    bc2 = 1.f - powf(hp.beta2, t);
   }
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
   for (long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4; i < a.n;
@@ -49,11 +50,11 @@ __global__ void __launch_bounds__(256) dense_opt_kernel(const DenseOptArgs a) {
       const float4 gv = *reinterpret_cast<const float4*>(a.g + i);
       w[0] = wv.x; w[1] = wv.y; w[2] = wv.z; w[3] = wv.w;
       g[0] = gv.x; g[1] = gv.y; g[2] = gv.z; g[3] = gv.w;
-      if constexpr (OPT != D_SGD) {
+      if constexpr (kHasS0) {
         const float4 sv = *reinterpret_cast<const float4*>(a.s0 + i);
         s0[0] = sv.x; s0[1] = sv.y; s0[2] = sv.z; s0[3] = sv.w;
       }
-      if constexpr (OPT == D_ADAM || OPT == D_FTRL) {
+      if constexpr (kHasS1) {
         const float4 sv = *reinterpret_cast<const float4*>(a.s1 + i);
         s1[0] = sv.x; s1[1] = sv.y; s1[2] = sv.z; s1[3] = sv.w;
       }
@@ -62,47 +63,19 @@ __global__ void __launch_bounds__(256) dense_opt_kernel(const DenseOptArgs a) {
         const bool ok = j < cnt;
         w[j] = ok ? a.w[i + j] : 0.f;
         g[j] = ok ? a.g[i + j] : 0.f;
-        s0[j] = (ok && OPT != D_SGD) ? a.s0[i + j] : 0.f;
-        s1[j] = (ok && (OPT == D_ADAM || OPT == D_FTRL)) ? a.s1[i + j] : 0.f;
+        s0[j] = (ok && kHasS0) ? a.s0[i + j] : 0.f;
+        s1[j] = (ok && kHasS1) ? a.s1[i + j] : 0.f;
       }
     }
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float gg = g[j] * inv_scaler;
-      if constexpr (OPT == D_SGD) {
-        w[j] -= lr * gg;
-      } else if constexpr (OPT == D_ADAGRAD) {
-        s0[j] += gg * gg;
-        w[j] -= lr * gg / (sqrtf(s0[j]) + a.epsilon);
-      } else if constexpr (OPT == D_ADAM) {
-        s0[j] = a.beta1 * s0[j] + (1.f - a.beta1) * gg;
-        s1[j] = a.beta2 * s1[j] + (1.f - a.beta2) * gg * gg;
-        w[j] -= alpha * s0[j] / (sqrtf(s1[j]) + a.epsilon);
-      } else if constexpr (OPT == D_FTRL) {
-        const float n_new = s1[j] + gg * gg;
-        s0[j] += gg + (sqrtf(s1[j] + a.ftrl_beta) - sqrtf(n_new + a.ftrl_beta)) * w[j] / lr;
-        s1[j] = n_new;
-        const float p = (s0[j] > 0.f ? 1.f : -1.f) * a.lambda1 - s0[j];
-        const float q = sqrtf(n_new + a.ftrl_beta) / lr + a.lambda2;
-        w[j] = fabsf(s0[j]) > a.lambda1 ? p / q : 0.f;
-      } else if constexpr (OPT == D_MOMENTUM) {
-        s0[j] = a.momentum * s0[j] - lr * gg;
-        w[j] += s0[j];
-      } else if constexpr (OPT == D_NESTEROV) {
-        const float an = a.momentum * s0[j] - lr * gg;
-        w[j] += -a.momentum * s0[j] + (1.f + a.momentum) * an;
-        s0[j] = an;
-      } else if constexpr (OPT == D_RMSPROP) {
-        s0[j] = a.beta2 * s0[j] + (1.f - a.beta2) * gg * gg;
-        w[j] -= lr * gg / (sqrtf(s0[j]) + a.epsilon);
-      }
-    }
+    for (int j = 0; j < 4; ++j)
+      apply_opt<OPT, float>(w[j], g[j] * inv_scaler, s0 + j, s1 + j, 0, hp, lr, bc1, bc2);
     if (cnt == 4) {
       *reinterpret_cast<float4*>(a.w + i) = make_float4(w[0], w[1], w[2], w[3]);
       if (a.zero_grad) *reinterpret_cast<float4*>(a.g + i) = make_float4(0.f, 0.f, 0.f, 0.f);
-      if constexpr (OPT != D_SGD)
+      if constexpr (kHasS0)
         *reinterpret_cast<float4*>(a.s0 + i) = make_float4(s0[0], s0[1], s0[2], s0[3]);
-      if constexpr (OPT == D_ADAM || OPT == D_FTRL)
+      if constexpr (kHasS1)
         *reinterpret_cast<float4*>(a.s1 + i) = make_float4(s1[0], s1[1], s1[2], s1[3]);
       if (a.w16)
         *reinterpret_cast<uint2*>(a.w16 + i) =
@@ -111,8 +84,8 @@ __global__ void __launch_bounds__(256) dense_opt_kernel(const DenseOptArgs a) {
       for (int j = 0; j < cnt; ++j) {
         a.w[i + j] = w[j];
         if (a.zero_grad) a.g[i + j] = 0.f;
-        if (OPT != D_SGD) a.s0[i + j] = s0[j];
-        if (OPT == D_ADAM || OPT == D_FTRL) a.s1[i + j] = s1[j];
+        if (kHasS0) a.s0[i + j] = s0[j];
+        if (kHasS1) a.s1[i + j] = s1[j];
         if (a.w16) a.w16[i + j] = __float2bfloat16(w[j]);
       }
     }
@@ -499,13 +472,13 @@ extern "C" int hctr_dense_opt(const DenseOptArgs* a, int opt, void* stream) {
   const int threads = 256;
   const int blocks = grid_for((a->n + 3) / 4, threads, num_sms() * 8);
   switch (opt) {
-    case D_SGD: dense_opt_kernel<D_SGD><<<blocks, threads, 0, ST(stream)>>>(*a); break;
-    case D_ADAGRAD: dense_opt_kernel<D_ADAGRAD><<<blocks, threads, 0, ST(stream)>>>(*a); break;
-    case D_ADAM: dense_opt_kernel<D_ADAM><<<blocks, threads, 0, ST(stream)>>>(*a); break;
-    case D_FTRL: dense_opt_kernel<D_FTRL><<<blocks, threads, 0, ST(stream)>>>(*a); break;
-    case D_MOMENTUM: dense_opt_kernel<D_MOMENTUM><<<blocks, threads, 0, ST(stream)>>>(*a); break;
-    case D_NESTEROV: dense_opt_kernel<D_NESTEROV><<<blocks, threads, 0, ST(stream)>>>(*a); break;
-    case D_RMSPROP: dense_opt_kernel<D_RMSPROP><<<blocks, threads, 0, ST(stream)>>>(*a); break;
+    case OPT_SGD: dense_opt_kernel<OPT_SGD><<<blocks, threads, 0, ST(stream)>>>(*a); break;
+    case OPT_ADAGRAD: dense_opt_kernel<OPT_ADAGRAD><<<blocks, threads, 0, ST(stream)>>>(*a); break;
+    case OPT_ADAM: dense_opt_kernel<OPT_ADAM><<<blocks, threads, 0, ST(stream)>>>(*a); break;
+    case OPT_FTRL: dense_opt_kernel<OPT_FTRL><<<blocks, threads, 0, ST(stream)>>>(*a); break;
+    case OPT_MOMENTUM: dense_opt_kernel<OPT_MOMENTUM><<<blocks, threads, 0, ST(stream)>>>(*a); break;
+    case OPT_NESTEROV: dense_opt_kernel<OPT_NESTEROV><<<blocks, threads, 0, ST(stream)>>>(*a); break;
+    case OPT_RMSPROP: dense_opt_kernel<OPT_RMSPROP><<<blocks, threads, 0, ST(stream)>>>(*a); break;
     default: return -2;
   }
   return OK();

@@ -24,6 +24,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 
 from ..enums import CommunicationStrategy, Optimizer_t
+from ..ops.optim import opt_hp, opt_states
 from ..solver import OptParamsPy
 from . import ops as E
 
@@ -468,15 +469,8 @@ class EmbeddingCollection:
             n = max(grp.rows, 1) * grp.pitch
             grp.table = torch.empty(n, dtype=WEIGHT_DTYPES[grp.wdtype], device=dev)
             self._init_group(grp, gen, seed)
-            ns = grp.opt.num_states if grp.opt is not None else 0
-            if grp.opt.optimizer_type == Optimizer_t.Adam:
-                ns = 2
             sdt = self.state_dtype if grp.kind == "mp" else torch.float32
-            grp.s0 = torch.zeros(n, dtype=sdt, device=dev) if ns >= 1 and self.is_train else None
-            grp.s1 = torch.zeros(n, dtype=sdt, device=dev) if ns >= 2 and self.is_train else None
-            if grp.s0 is not None and grp.opt.optimizer_type == Optimizer_t.AdaGrad \
-                    and grp.opt.initial_accu_value != 0.0:
-                grp.s0.fill_(grp.opt.initial_accu_value)
+            grp.s0, grp.s1 = opt_states(grp.opt, n, sdt, dev) if self.is_train else (None, None)
             if grp.rowwise and self.is_train:
                 # one fp32 accumulator per row, whatever the state dtype (an only-growing bf16 value
                 # would drop small increments)
@@ -1076,10 +1070,7 @@ class EmbeddingCollection:
             self.comm.barrier_device()
 
     def _hp(self, o: OptParamsPy):
-        return {"scaler": self.scaler, "beta1": o.beta1, "beta2": o.beta2, "epsilon": o.epsilon,
-                "lambda1": o.lambda1, "lambda2": o.lambda2, "ftrl_beta": o.beta,
-                "momentum": o.momentum_factor, "initial_accu_value": o.initial_accu_value,
-                "sr_seed": self.sr_seed}
+        return opt_hp(o, self.scaler, self.sr_seed)
 
     def _accum_update(self, grp, key_bufs, grad_bufs, lr_t, step_t):
         o = grp.opt
@@ -1108,12 +1099,8 @@ class EmbeddingCollection:
             if grp.rowwise:
                 E.dp_rowwise_update(grp.table, grp.s0, grp.dense_wgrad, grp.pitch, self._hp(o), lr_t)
                 return
-            dcode = {Optimizer_t.SGD: D.D_SGD, Optimizer_t.AdaGrad: D.D_ADAGRAD,
-                     Optimizer_t.Adam: D.D_ADAM, Optimizer_t.Ftrl: D.D_FTRL,
-                     Optimizer_t.MomentumSGD: D.D_MOMENTUM, Optimizer_t.Nesterov: D.D_NESTEROV,
-                     Optimizer_t.RMSProp: D.D_RMSPROP}[o.optimizer_type]
-            D.dense_opt_step(dcode, grp.table, grp.dense_wgrad, None, grp.s0, grp.s1, lr_t, step_t,
-                             self._hp(o), zero_grad=True)
+            D.dense_opt_step(o.optimizer_type, grp.table, grp.dense_wgrad, None, grp.s0, grp.s1, lr_t,
+                             step_t, self._hp(o), zero_grad=True)
 
     # ------------------------------------------------------------------ checkpoint helpers
     def local_table_items(self):

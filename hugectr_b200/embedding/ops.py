@@ -16,11 +16,10 @@ import torch
 from .. import _native
 from ..enums import Optimizer_t
 from ..ops import dense as D
+from ..ops.optim import OPT_CODE, COptHyper, opt_hyper, sr_seed
+from ..ops.optim import opt_reference as sparse_opt_reference
 
 MAX_RANKS = 16
-OPT_CODE = {Optimizer_t.SGD: 0, Optimizer_t.AdaGrad: 1, Optimizer_t.Adam: 2, Optimizer_t.Ftrl: 3,
-            Optimizer_t.MomentumSGD: 4, Optimizer_t.Nesterov: 5, Optimizer_t.RMSProp: 6,
-            Optimizer_t.RowWiseAdaGrad: 7}
 
 
 class CEmbLookup(C.Structure):
@@ -54,14 +53,6 @@ class CBwdIndex(C.Structure):
                 ("heavy_ticket", C.c_void_p), ("heavy_slot", C.c_void_p),
                 ("max_heavy_rows", C.c_uint), ("max_heavy_items", C.c_uint),
                 ("light_list", C.c_void_p), ("medium_list", C.c_void_p), ("class_count", C.c_void_p)]
-
-
-class COptHyper(C.Structure):
-    _fields_ = [("lr_ptr", C.c_void_p), ("lr_scale", C.c_float), ("scaler", C.c_float),
-                ("beta1", C.c_float), ("beta2", C.c_float), ("epsilon", C.c_float),
-                ("lambda1", C.c_float), ("lambda2", C.c_float), ("ftrl_beta", C.c_float),
-                ("momentum", C.c_float), ("initial_accu", C.c_float), ("step_ptr", C.c_void_p),
-                ("sr_seed", C.c_uint), ("pad_", C.c_uint)]
 
 
 _lib = None
@@ -565,68 +556,11 @@ def sr_round_bf16(x, seed: int, step: int, idx):
     return res.to(x.device)
 
 
-def sparse_opt_reference(opt: Optimizer_t, w, s0, s1, g, hp, lr, step):
-    """Row-block update (w, s0, s1, g all [n, ev] fp32; RowWiseAdaGrad: s0 [n], one accumulator per
-    row). Returns nothing, updates in place."""
-    g = g / hp.get("scaler", 1.0)
-    eps = hp.get("epsilon", 1e-7)
-    if opt == Optimizer_t.RowWiseAdaGrad:
-        # s += mean_c g^2 ; w -= (lr / (sqrt(s) + eps)) g  -- the factor first, as the kernels do
-        s0 += (g * g).sum(1) / g.shape[1]
-        w -= (lr / (s0.sqrt() + eps)).unsqueeze(1) * g
-    elif opt == Optimizer_t.SGD:
-        w -= lr * g
-    elif opt == Optimizer_t.AdaGrad:
-        s0 += g * g
-        w -= lr * g / (s0.sqrt() + eps)
-    elif opt == Optimizer_t.Adam:
-        b1, b2 = hp.get("beta1", 0.9), hp.get("beta2", 0.999)
-        s0.mul_(b1).add_((1 - b1) * g)
-        s1.mul_(b2).add_((1 - b2) * g * g)
-        alpha = lr * (1 - b2 ** step) ** 0.5 / (1 - b1 ** step)
-        w -= alpha * s0 / (s1.sqrt() + eps)
-    elif opt == Optimizer_t.Ftrl:
-        fb, l1, l2 = hp.get("ftrl_beta", 0.0), hp.get("lambda1", 0.0), hp.get("lambda2", 0.0)
-        n_new = s1 + g * g
-        s0 += g + ((s1 + fb).sqrt() - (n_new + fb).sqrt()) * w / lr
-        s1.copy_(n_new)
-        p = torch.where(s0 > 0, l1 - s0, -l1 - s0)
-        q = (n_new + fb).sqrt() / lr + l2
-        w.copy_(torch.where(s0.abs() > l1, p / q, torch.zeros_like(w)))
-    elif opt == Optimizer_t.MomentumSGD:
-        s0.mul_(hp.get("momentum", 0.0)).sub_(lr * g)
-        w += s0
-    elif opt == Optimizer_t.Nesterov:
-        mu = hp.get("momentum", 0.0)
-        an = mu * s0 - lr * g
-        w += -mu * s0 + (1 + mu) * an
-        s0.copy_(an)
-    elif opt == Optimizer_t.RMSProp:
-        b2 = hp.get("beta2", 0.999)
-        s0.mul_(b2).add_((1 - b2) * g * g)
-        w -= lr * g / (s0.sqrt() + eps)
-
-
-def sr_seed(hp: dict) -> int:
-    """32-bit seed of the stochastic rounding of bf16 weights (``hp["sr_seed"]``, default 0)"""
-    return int(hp.get("sr_seed", 0)) & 0xFFFFFFFF
-
-
-def _opt_hyper(hp: dict, lr_t, step_t) -> COptHyper:
-    """Kernel hyper-parameters: the device learning rate ``lr_t`` and step counter ``step_t`` (None: the
-    kernels take step 1) with the optimizer's values from ``hp``."""
-    return COptHyper(lr_t.data_ptr(), 1.0, hp.get("scaler", 1.0), hp.get("beta1", 0.9),
-                     hp.get("beta2", 0.999), hp.get("epsilon", 1e-7), hp.get("lambda1", 0.0),
-                     hp.get("lambda2", 0.0), hp.get("ftrl_beta", 0.0), hp.get("momentum", 0.0),
-                     hp.get("initial_accu_value", 0.0), None if step_t is None else step_t.data_ptr(),
-                     sr_seed(hp), 0)
-
-
 def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: dict, lr_t, step_t,
            num_sms: int = 132):
     """Fused per-unique-row optimizer; consumes and clears the workspace."""
     if table.is_cuda:
-        h = _opt_hyper(hp, lr_t, step_t)
+        h = opt_hyper(hp, lr_t, step_t)
         sbf = int(s0 is not None and s0.dtype == torch.bfloat16)
         rc = lib().hctr_emb_update(table.data_ptr(), 0 if s0 is None else s0.data_ptr(),
                                    0 if s1 is None else s1.data_ptr(), ws.wgrad.data_ptr(),
@@ -680,7 +614,7 @@ def dp_rowwise_update(table, s0, wgrad, pitch, hp: dict, lr_t, num_sms: int = 13
     weights and accumulator (``s0`` [rows] fp32)."""
     rows = table.numel() // pitch
     if table.is_cuda:
-        h = _opt_hyper(hp, lr_t, None)
+        h = opt_hyper(hp, lr_t, None)
         rc = lib().hctr_emb_dp_rowwise_update(table.data_ptr(), s0.data_ptr(), wgrad.data_ptr(), rows,
                                               pitch, C.byref(h), num_sms, _st(table.device))
         if rc:
@@ -762,7 +696,7 @@ def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_
                          "(see vec4_aligned); use backward_accum + update")
     p, kb, gbf = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch,
                               my_rank, nnz_bufs, key_bytes, act_bf16)
-    h = _opt_hyper(hp, lr_t, step_t)
+    h = opt_hyper(hp, lr_t, step_t)
     sbf = int(s0 is not None and s0.dtype == torch.bfloat16)
     rc = lib().hctr_emb_bwd_reduce_update(C.byref(p), C.byref(ws.c), C.byref(ws.ix),
                                           0 if s0 is None else s0.data_ptr(),

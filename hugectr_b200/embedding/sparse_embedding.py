@@ -34,6 +34,7 @@ import torch
 from ..io import filesystem as FS
 
 from ..enums import Embedding_t, Optimizer_t, Update_t
+from ..ops.optim import opt_hp, opt_states
 from . import ops as E
 from .hashtable import HashTable
 
@@ -69,12 +70,7 @@ class SparseEmbeddingRuntime:
                 self.max_rows = max(1024, sum(cfg.slot_size_array) // max(1, self.world) + 1024)
             self.table = torch.zeros(self.max_rows * self.vec, dtype=torch.float32, device=device)
             self._init_table(seed)
-            n = self.table.numel()
-            nst = 2 if opt.optimizer_type in (Optimizer_t.Adam, Optimizer_t.Ftrl) else (1 if ns >= 1 else 0)
-            self.s0 = torch.zeros(n, device=device) if nst >= 1 else None
-            self.s1 = torch.zeros(n, device=device) if nst >= 2 else None
-            if self.s0 is not None and opt.optimizer_type == Optimizer_t.AdaGrad:
-                self.s0.fill_(opt.initial_accu_value)
+            self.s0, self.s1 = opt_states(opt, self.table.numel(), device=device)
             self.hash = HashTable(self.max_rows, device)
             # (one spare entry behind the table: the write target of batch entries this rank does not own)
             self.slot_of_row = torch.full((self.max_rows + 1,), -1, dtype=torch.int64, device=device) \
@@ -245,9 +241,7 @@ class SparseEmbeddingRuntime:
             self.comm.all_gather(self.grads_all, g.reshape(-1))
         kb = list(self.rows_all.unbind(0))
         gb = list(self.grads_all.unbind(0))
-        hp = {"scaler": self.scaler, "beta1": self.opt.beta1, "beta2": self.opt.beta2,
-              "epsilon": self.opt.epsilon, "lambda1": self.opt.lambda1, "lambda2": self.opt.lambda2,
-              "ftrl_beta": self.opt.beta, "momentum": self.opt.momentum_factor}
+        hp = opt_hp(self.opt, self.scaler)
         if self.opt.update_type == Update_t.LazyGlobal and self.opt.optimizer_type == Optimizer_t.Adam:
             return self._lazy_adam(lr_t, step_t)
         if self.indexed:

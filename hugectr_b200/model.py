@@ -20,20 +20,16 @@ from . import metrics as M
 from .data.batch import HostBatch
 from .data.readers import SparseLayout
 from .embedding.collection import EmbeddingCollection, EmbeddingCollectionConfig
-from .enums import MetricsRawType, MetricsType, Optimizer_t, Tensor_t
+from .enums import MetricsRawType, MetricsType, Tensor_t
 from .layers import BuildCtx, ParamArena, TensorBag
 from .lr_scheduler import LearningRateScheduler
 from .network import Network, insert_fanout_slices
 from .ops import dense as D
+from .ops.optim import opt_hp, opt_states
 from .parallel.comm import Comm
 from .solver import (DataReaderParams, DenseLayer, Input, OptParamsPy, Solver, SparseEmbedding,
                      check_not_rowwise)
 from .utils import logger
-
-DENSE_OPT_CODE = {Optimizer_t.SGD: D.D_SGD, Optimizer_t.AdaGrad: D.D_ADAGRAD,
-                  Optimizer_t.Adam: D.D_ADAM, Optimizer_t.Ftrl: D.D_FTRL,
-                  Optimizer_t.MomentumSGD: D.D_MOMENTUM, Optimizer_t.Nesterov: D.D_NESTEROV,
-                  Optimizer_t.RMSProp: D.D_RMSPROP}
 
 
 class TrainingCallback:
@@ -266,19 +262,10 @@ class Model:
     def _create_dense_optimizer(self):
         o = self.opt_params
         dev = self.device
-        n = self.arena.weights.numel()
-        ns = o.num_states
-        if o.optimizer_type == Optimizer_t.Adam:
-            ns = 2
-        self.opt_s0 = torch.zeros(n, device=dev) if ns >= 1 else None
-        self.opt_s1 = torch.zeros(n, device=dev) if ns >= 2 else None
-        if o.optimizer_type == Optimizer_t.AdaGrad and o.initial_accu_value != 0 and self.opt_s0 is not None:
-            self.opt_s0.fill_(o.initial_accu_value)
+        self.opt_s0, self.opt_s1 = opt_states(o, self.arena.weights.numel(), device=dev)
         self.lr_t = torch.full((1,), float(self.solver.lr), device=dev)
         self.step_t = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.dense_hp = {"scaler": self.solver.scaler if self.mixed else 1.0, "beta1": o.beta1,
-                         "beta2": o.beta2, "epsilon": o.epsilon, "lambda1": o.lambda1,
-                         "lambda2": o.lambda2, "ftrl_beta": o.beta, "momentum": o.momentum_factor}
+        self.dense_hp = opt_hp(o, self.solver.scaler if self.mixed else 1.0)
 
     def _create_metrics(self):
         ncls = self.input.label_dim
@@ -546,7 +533,7 @@ class Model:
         """fused dense optimizer over arena elements [lo, hi) (also zeroes that wgrad range)"""
         a = self.arena
         sl = lambda t: None if t is None else t[lo:hi]
-        D.dense_opt_step(DENSE_OPT_CODE[self.opt_params.optimizer_type], a.weights[lo:hi],
+        D.dense_opt_step(self.opt_params.optimizer_type, a.weights[lo:hi],
                          a.wgrad[lo:hi], sl(a.weights16), sl(self.opt_s0), sl(self.opt_s1),
                          self.lr_t, self.step_t, self.dense_hp, zero_grad=True)
 

@@ -6,11 +6,16 @@ import ctypes as C
 import torch
 
 from .. import _native
+from ..enums import Optimizer_t
+from .optim import OPT_CODE, COptHyper, opt_hyper, opt_reference
 
 EW_RELU, EW_RELU_BWD, EW_SIGMOID, EW_SIGMOID_BWD, EW_ADD, EW_SUB, EW_MUL, EW_SCALE, EW_ELU, \
     EW_ELU_BWD, EW_COPY, EW_ADD_INPLACE = range(12)
 
-D_SGD, D_ADAGRAD, D_ADAM, D_FTRL, D_MOMENTUM, D_NESTEROV, D_RMSPROP = range(7)
+# short names of the element-wise rules that dense_opt_step takes
+D_SGD, D_ADAGRAD, D_ADAM, D_FTRL, D_MOMENTUM, D_NESTEROV, D_RMSPROP = (
+    Optimizer_t.SGD, Optimizer_t.AdaGrad, Optimizer_t.Adam, Optimizer_t.Ftrl, Optimizer_t.MomentumSGD,
+    Optimizer_t.Nesterov, Optimizer_t.RMSProp)
 
 launch_count = 0  # number of native kernel launches issued through this package
 
@@ -22,11 +27,7 @@ def _count(n=1):
 
 class DenseOptArgs(C.Structure):
     _fields_ = [("w", C.c_void_p), ("g", C.c_void_p), ("w16", C.c_void_p), ("s0", C.c_void_p),
-                ("s1", C.c_void_p), ("n", C.c_longlong), ("lr_ptr", C.c_void_p),
-                ("step_ptr", C.c_void_p), ("scaler", C.c_float), ("beta1", C.c_float),
-                ("beta2", C.c_float), ("epsilon", C.c_float), ("lambda1", C.c_float),
-                ("lambda2", C.c_float), ("ftrl_beta", C.c_float), ("momentum", C.c_float),
-                ("zero_grad", C.c_int)]
+                ("s1", C.c_void_p), ("n", C.c_longlong), ("hp", COptHyper), ("zero_grad", C.c_int)]
 
 
 _lib = None
@@ -258,54 +259,20 @@ def add3(a, b, c, out):
 
 # ----------------------------------------------------------------------------- optimizers
 def dense_opt_step(opt, w, g, w16, s0, s1, lr_t, step_t, hp, zero_grad=True):
-    """One fused launch over the flat arena. hp: dict of hyper-parameters."""
+    """One fused launch over the flat arena with the element-wise rule of ``opt`` (an Optimizer_t).
+    hp: dict of hyper-parameters (optim.opt_hp)."""
     if w.is_cuda:
         a = DenseOptArgs(w.data_ptr(), g.data_ptr(), 0 if w16 is None else w16.data_ptr(),
                          0 if s0 is None else s0.data_ptr(), 0 if s1 is None else s1.data_ptr(),
-                         w.numel(), lr_t.data_ptr(), step_t.data_ptr(), hp.get("scaler", 1.0),
-                         hp.get("beta1", 0.9), hp.get("beta2", 0.999), hp.get("epsilon", 1e-7),
-                         hp.get("lambda1", 0.0), hp.get("lambda2", 0.0), hp.get("ftrl_beta", 0.0),
-                         hp.get("momentum", 0.0), int(zero_grad))
-        _chk(lib().hctr_dense_opt(C.byref(a), opt, _st(w)), "dense_opt")
+                         w.numel(), opt_hyper(hp, lr_t, step_t), int(zero_grad))
+        _chk(lib().hctr_dense_opt(C.byref(a), OPT_CODE[opt], _st(w)), "dense_opt")
         return
     dense_opt_reference(opt, w, g, w16, s0, s1, float(lr_t.item()), int(step_t.item()), hp, zero_grad)
 
 
 def dense_opt_reference(opt, w, g, w16, s0, s1, lr, step, hp, zero_grad=True):
     """fp32 PyTorch implementation of the Appendix A.2 update rules (oracle + CPU path)."""
-    gg = g / hp.get("scaler", 1.0)
-    eps = hp.get("epsilon", 1e-7)
-    if opt == D_SGD:
-        w.sub_(lr * gg)
-    elif opt == D_ADAGRAD:
-        s0.add_(gg * gg)
-        w.sub_(lr * gg / (s0.sqrt() + eps))
-    elif opt == D_ADAM:
-        b1, b2 = hp.get("beta1", 0.9), hp.get("beta2", 0.999)
-        alpha = lr * (1 - b2 ** step) ** 0.5 / (1 - b1 ** step)
-        s0.mul_(b1).add_((1 - b1) * gg)
-        s1.mul_(b2).add_((1 - b2) * gg * gg)
-        w.sub_(alpha * s0 / (s1.sqrt() + eps))
-    elif opt == D_FTRL:
-        fb, l1, l2 = hp.get("ftrl_beta", 0.0), hp.get("lambda1", 0.0), hp.get("lambda2", 0.0)
-        n_new = s1 + gg * gg
-        s0.add_(gg + ((s1 + fb).sqrt() - (n_new + fb).sqrt()) * w / lr)
-        s1.copy_(n_new)
-        p = torch.where(s0 > 0, l1 - s0, -l1 - s0)
-        q = (n_new + fb).sqrt() / lr + l2
-        w.copy_(torch.where(s0.abs() > l1, p / q, torch.zeros_like(w)))
-    elif opt == D_MOMENTUM:
-        s0.mul_(hp.get("momentum", 0.0)).sub_(lr * gg)
-        w.add_(s0)
-    elif opt == D_NESTEROV:
-        mu = hp.get("momentum", 0.0)
-        an = mu * s0 - lr * gg
-        w.add_(-mu * s0 + (1 + mu) * an)
-        s0.copy_(an)
-    elif opt == D_RMSPROP:
-        b2 = hp.get("beta2", 0.999)
-        s0.mul_(b2).add_((1 - b2) * gg * gg)
-        w.sub_(lr * gg / (s0.sqrt() + eps))
+    opt_reference(opt, w, s0, s1, g, hp, lr, step)
     if w16 is not None:
         w16.copy_(w.to(w16.dtype))
     if zero_grad:

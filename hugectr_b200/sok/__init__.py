@@ -21,7 +21,7 @@ import numpy as np
 import torch
 
 from ..embedding.hashtable import HashTable
-from ..embedding.ops import sparse_opt_reference
+from ..ops.optim import opt_reference
 from ..enums import Optimizer_t
 from ..parallel.comm import Comm
 
@@ -503,7 +503,7 @@ class OptimizerWrapper:
                     v.states[k] = ns
             w = v.weight[u].float()
             a, b = v.states["s0"][u].clone(), v.states["s1"][u].clone()
-            sparse_opt_reference(self.opt, w, a, b, gg, self.hp, self.lr, self.step)
+            opt_reference(self.opt, w, a, b, gg, self.hp, self.lr, self.step)
             v.weight[u] = w.to(v.weight.dtype)
             v.states["s0"][u], v.states["s1"][u] = a, b
             v.last_touch[u.cpu()] = time.time()

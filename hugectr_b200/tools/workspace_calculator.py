@@ -9,16 +9,15 @@ from __future__ import annotations
 
 import math
 
-from ..enums import OPT_STATES_PER_WEIGHT, Embedding_t, Optimizer_t, Update_t
+from ..enums import Embedding_t, Optimizer_t, Update_t
+from ..solver import OptParamsPy
 
 
 def calculate(slot_size_array, vec_size: int, optimizer: Optimizer_t = Optimizer_t.Adam,
               update_type: Update_t = Update_t.Global, num_gpus: int = 1,
               embedding_type: Embedding_t = Embedding_t.DistributedSlotSparseEmbeddingHash,
               load_factor: float = 1.0) -> int:
-    ns = OPT_STATES_PER_WEIGHT[optimizer]
-    if optimizer == Optimizer_t.Adam and update_type == Update_t.LazyGlobal:
-        ns += 1
+    ns = OptParamsPy(optimizer, update_type).num_states
     if embedding_type == Embedding_t.DistributedSlotSparseEmbeddingHash:
         rows = math.ceil(sum(slot_size_array) / num_gpus)
     else:
@@ -48,8 +47,6 @@ def cal_vocabulary_size_per_gpu_for_localized_slot(slot_size_array, num_gpus):
 
 def cal_workspace_size_per_gpu_from_vocabulary_size_per_gpu(vocabulary_size_per_gpu, emb_vec_size, num_gpus,
                                                             optimizer, optimizer_update_type):
-    ns = OPT_STATES_PER_WEIGHT[_OPT[optimizer]]
-    if optimizer == "adam" and optimizer_update_type == "lazy_global":
-        ns += 1
     assert optimizer_update_type in _UPD
+    ns = OptParamsPy(_OPT[optimizer], _UPD[optimizer_update_type]).num_states
     return math.ceil(vocabulary_size_per_gpu * emb_vec_size * 4 * (1 + ns) / (1024 * 1024))

@@ -2,7 +2,10 @@
 roofline in MEASURED_PEAKS.json)."""
 import json, sys, torch
 sys.path.insert(0, ".")
+from hugectr_b200.enums import OPT_STATES_PER_WEIGHT, Optimizer_t as O
 from hugectr_b200.ops import dense as D
+from hugectr_b200.ops.optim import opt_hp
+from hugectr_b200.solver import OptParamsPy
 
 def timeit(fn, iters=20, warm=5):
     for _ in range(warm): fn()
@@ -35,11 +38,16 @@ for (r, c) in [(b, 1024), (b, 512), (b, 256), (b, 3456)]:
     x = bf(r, c); o = torch.zeros(c, device="cuda")
     rep(f"colsum {r}x{c}", timeit(lambda: D.colsum_accum(x, o)), r * c * 2)
 n = 16_500_000 // 64 * 64
-wt, g, w16, s0 = (torch.randn(n, device="cuda"), torch.randn(n, device="cuda"),
-                  torch.zeros(n, device="cuda", dtype=torch.bfloat16), torch.ones(n, device="cuda"))
+wt, g, w16, s0, s1 = (torch.randn(n, device="cuda"), torch.randn(n, device="cuda"),
+                      torch.zeros(n, device="cuda", dtype=torch.bfloat16), torch.ones(n, device="cuda"),
+                      torch.ones(n, device="cuda"))
 lr_t = torch.full((1,), 0.01, device="cuda"); st = torch.ones(1, dtype=torch.int32, device="cuda")
-hp = {"scaler": 1.0, "beta1": .9, "beta2": .999, "epsilon": 1e-8, "lambda1": 0, "lambda2": 0, "ftrl_beta": 0, "momentum": 0}
-rep("dense_opt adagrad", timeit(lambda: D.dense_opt_step(D.D_ADAGRAD, wt, g, w16, s0, None, lr_t, st, hp)), n * (4 * 5 + 2))
+hp = opt_hp(OptParamsPy(epsilon=1e-8))
+for o in (O.SGD, O.AdaGrad, O.Adam, O.Ftrl, O.MomentumSGD, O.Nesterov, O.RMSProp):
+    ns = OPT_STATES_PER_WEIGHT[o]
+    st0, st1 = s0 if ns >= 1 else None, s1 if ns >= 2 else None
+    rep(f"dense_opt {o.name.lower()}", timeit(lambda: D.dense_opt_step(o, wt, g, w16, st0, st1, lr_t, st, hp)),
+        n * (4 * (3 + 2 * ns) + 2))
 src = bf(b, 128); dst = bf(b, 3456)
 rep("copy2d 128->3456 slice", timeit(lambda: D.copy2d(src, dst[:, :128])), b * 128 * 4)
 rep("torch copy ref 48MB", timeit(lambda: dt.copy_(dy)), b * w * 4)
