@@ -109,13 +109,16 @@ HCTR_DEVICE void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster.  Release at CTA scope (the
+// default): the arrival only reports that this thread's reads of a stage are done, which is ordered before the
+// peer's next TMA write into it by the barrier itself.  A .release.cluster arrive compiles to a GPU-wide memory
+// barrier (MEMBAR.ALL.GPU) ahead of every arrival, i.e. once per consumer warp and k block of the GEMM main loop.
 HCTR_DEVICE void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
   asm volatile(
       "{\n\t"
       ".reg .b32 remote;\n\t"
       "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t"
       "}\n" ::"r"(smem_u32(bar)),
       "r"(cta)
       : "memory");
