@@ -9,10 +9,19 @@
 // (X^T*dY) all run from the same row-major tensors without any transposed copies.
 //
 // CTA = three warpgroups: warpgroup 0 is the TMA producer, warpgroups 1 and 2 each own 64 rows of the
-// 128 x BN tile (one m64nBNk16 wgmma per 16-wide K step) and run the epilogue of their rows.  The
-// accumulators leave the registers through a per-warpgroup [64 x 64] fp32 staging slab, so the fused
-// epilogue works on one row x 32 columns per thread with vectorised global accesses.
+// 128 x BN tile (one m64nBNk16 wgmma per 16-wide K step) and run the epilogue of their rows.
+//
+// Two epilogues, chosen on the host per call:
+//  * TMA epilogue (TMA_EPI; bf16 outputs whose epilogue tensors TMA can address).  Warp 1 of the producer
+//    warpgroup TMA-loads the x0 / xl / mask boxes of each 64-column group into a per-warpgroup ring while the
+//    tile's main loop runs.  The consumers combine them with the accumulators in place, at the wgmma fragment
+//    positions, and one thread TMA-stores the bf16 box (and aux) asynchronously; the slot is handed back to the
+//    producer once the store has read it, which for a tile's last group happens in the next tile's main loop.
+//  * Slab epilogue (fp32 / atomic / accumulating outputs, addf, tensors TMA cannot address): the accumulators
+//    leave the registers through a per-warpgroup [64 x 64] fp32 staging slab, so the fused epilogue works on
+//    one row x 32 columns per thread with vectorised global accesses.
 #include <cstdio>
+#include <cstring>
 
 #include "gemm_epilogue.cuh"
 
@@ -24,17 +33,129 @@ constexpr int WG_K = 16;
 constexpr int kNumThreads = 384;
 constexpr int kSmemLimit = 232448;  // 227 KB opt-in shared memory per block on sm_90
 
-template <int BN>
+// TMA epilogue ring: kEpiBoxes [64 rows x 64 columns] bf16 boxes (SWIZZLE_128B) per consumer warpgroup.  A
+// 64-column group takes one box per tensor it reads (epi_in_boxes, at least one for the output), so the ring has
+// 4 slots for EPI_ADD / EPI_MASK / output-only flag sets and 2 for EPI_CROSS.
+constexpr int kEpiBoxBytes = 64 * 64 * 2;
+constexpr int kEpiBoxes = 4;
+
+// boxes of x0 / xl / mask (in that order within a slot) the TMA epilogue loads per 64-column group
+__host__ __device__ inline int epi_in_boxes(int flags) {
+  return ((flags & EPI_CROSS) ? 2 : (flags & EPI_ADD) ? 1 : 0) + ((flags & EPI_MASK) ? 1 : 0);
+}
+
+// Operand stages that fit beside the epilogue staging (slab / TMA ring): BN = 64: 7 / 6, BN = 128: 5 / 5,
+// BN = 256: 3 / 3.
+template <int BN, bool TMA_EPI>
 struct SmemLayout {
   static constexpr int kABytes = BLOCK_M * BLOCK_K * 2;
   static constexpr int kBBytes = BN * BLOCK_K * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kEpiBytes = 2 * kEpiSlabBytes;
+  static constexpr int kEpiBytes = TMA_EPI ? 2 * kEpiBoxes * kEpiBoxBytes : 2 * kEpiSlabBytes;
   static constexpr int kBarBytes = 1024;
   static constexpr int kFit = (kSmemLimit - kEpiBytes - kBarBytes - 1024) / kStageBytes;
   static constexpr int kStages = kFit < 8 ? kFit : 8;
   static constexpr int kTotal = kStages * kStageBytes + kEpiBytes + kBarBytes + 1024;  // +1024 align slack
+  static_assert(kStages == (BN == 64 ? (TMA_EPI ? 6 : 7) : BN == 128 ? 5 : 3), "stage count per BN changed");
+  static_assert((kStageBytes % 1024) == 0, "the TMA ring needs 1024-byte aligned boxes");
 };
+
+// TMA epilogue of one warpgroup's m64 x BN accumulator tile (rows m_base.., columns n_base..).  `ring` holds the
+// warpgroup's kEpiBoxes boxes; slot / phase walk it in step with the producer (full / empty barriers, used only
+// when the flags read tensors), and `pending` is the slot whose TMA store has not been confirmed to have read it.
+// Every element goes through the same fp32 expressions, in the same order, as epilogue_chunk.
+template <int BN>
+HCTR_DEVICE void epilogue_tile_tma(const GemmParams& p, const int flags, const float (&acc)[BN / 2],
+                                   uint8_t* ring, uint64_t* full, uint64_t* empty, const CUtensorMap* tm_out,
+                                   const CUtensorMap* tm_aux, const int m_base, const int n_base, const int wg,
+                                   int& slot, uint32_t& phase, int& pending) {
+  const int n_in = epi_in_boxes(flags);
+  const int nbox = n_in > 0 ? n_in : 1;
+  const int slots = kEpiBoxes / nbox;
+  const int xl_box = (flags & EPI_CROSS) ? 1 : 0;
+  const int mask_box = n_in - 1;
+  const bool aux = (flags & EPI_CROSS) && p.aux != nullptr;
+  const bool leader = (threadIdx.x & 127) == 0;
+  const int lane = threadIdx.x & 31;
+  const int r0 = ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);
+  // SWIZZLE_128B: the 16-byte chunk j of box row r sits at chunk j ^ (r % 8); r % 8 == lane / 4 for both rows
+  const uint32_t lane_off = static_cast<uint32_t>(r0 * 128 + (lane & 3) * 4);
+  const int sw = lane >> 2;
+#pragma unroll
+  for (int g = 0; g < BN / 64; ++g) {
+    const int n0 = n_base + g * 64;
+    if (n0 >= p.N) break;
+    uint8_t* box = ring + slot * nbox * kEpiBoxBytes;
+    float2 bv[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int n = n0 + 8 * j + 2 * (lane & 3);
+      bv[j] = make_float2(0.f, 0.f);
+      if (p.bias != nullptr) {
+        if (n + 1 < p.N) bv[j] = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+        else if (n < p.N) bv[j].x = __ldg(p.bias + n);
+      }
+    }
+    if (n_in > 0) mbar_wait(&full[slot], phase);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t off = lane_off + h * (8 * 128) + ((j ^ sw) << 4);
+        const float* a2 = acc + (8 * g + j) * 4 + 2 * h;
+        float v0 = a2[0] * p.alpha, v1 = a2[1] * p.alpha;
+        if (p.bias != nullptr) {
+          v0 += bv[j].x;
+          v1 += bv[j].y;
+        }
+        if (flags & EPI_CROSS) {
+          const uint32_t xa = *reinterpret_cast<const uint32_t*>(box + off);
+          const uint32_t xb = *reinterpret_cast<const uint32_t*>(box + kEpiBoxBytes + off);
+          if (aux) *reinterpret_cast<uint32_t*>(box + kEpiBoxBytes + off) = pack_bf16x2(v0, v1);
+          v0 = bf16_lo(xa) * v0 + bf16_lo(xb);
+          v1 = bf16_hi(xa) * v1 + bf16_hi(xb);
+        }
+        if (flags & EPI_ADD) {
+          const uint32_t xb = *reinterpret_cast<const uint32_t*>(box + xl_box * kEpiBoxBytes + off);
+          v0 += bf16_lo(xb);
+          v1 += bf16_hi(xb);
+        }
+        if (flags & EPI_MASK) {
+          const uint32_t mk = *reinterpret_cast<const uint32_t*>(box + mask_box * kEpiBoxBytes + off);
+          if (!(bf16_lo(mk) > 0.f)) v0 = 0.f;
+          if (!(bf16_hi(mk) > 0.f)) v1 = 0.f;
+        }
+        if (flags & EPI_RELU) {
+          v0 = fmaxf(v0, 0.f);
+          v1 = fmaxf(v1, 0.f);
+        }
+        if (flags & EPI_SIGMOID) {
+          v0 = 1.f / (1.f + __expf(-v0));
+          v1 = 1.f / (1.f + __expf(-v1));
+        }
+        *reinterpret_cast<uint32_t*>(box + off) = pack_bf16x2(v0, v1);
+      }
+    }
+    fence_proxy_async();  // the box writes above become visible to the TMA store
+    if (leader) {
+      // every earlier store has read its box: the slot of the previous group goes back to the producer, and
+      // (output-only flag sets) the next group may write into its slot once past the barrier below
+      bulk_wait_read<0>();
+      if (pending >= 0 && n_in > 0) mbar_arrive(&empty[pending]);
+    }
+    named_bar_sync(1 + wg, 128);
+    if (leader) {
+      tma_store_2d(tm_out, box, n0, m_base);
+      if (aux) tma_store_2d(tm_aux, box + kEpiBoxBytes, n0, m_base);
+      bulk_commit();
+    }
+    pending = slot;
+    if (++slot == slots) {
+      slot = 0;
+      phase ^= 1;
+    }
+  }
+}
 
 template <int BN, int TA, int TB>
 HCTR_DEVICE void wgmma_tile(float (&acc)[BN / 2], uint64_t a, uint64_t b, uint32_t accumulate) {
@@ -45,21 +166,28 @@ HCTR_DEVICE void wgmma_tile(float (&acc)[BN / 2], uint64_t a, uint64_t b, uint32
 
 // MC == 2: thread-block cluster of two CTAs stacked along M that share the B tile -- each CTA loads
 // half of it and TMA-multicasts it into both shared memories (halves the L2->SM operand traffic of B).
-template <int BN, bool A_MN, bool B_MN, int MC>
+// TMA_EPI: bf16 output through the TMA epilogue; tmOut / tmAux / tmX0 / tmXl / tmMask are the [64 x 64] box maps of
+// the tensors the flags use (the others are not read).
+template <int BN, bool A_MN, bool B_MN, int MC, bool TMA_EPI>
 __global__ void __launch_bounds__(kNumThreads, 1)
     gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                   const GemmParams p) {
-  using L = SmemLayout<BN>;
+                   const __grid_constant__ CUtensorMap tmOut, const __grid_constant__ CUtensorMap tmAux,
+                   const __grid_constant__ CUtensorMap tmX0, const __grid_constant__ CUtensorMap tmXl,
+                   const __grid_constant__ CUtensorMap tmMask, const GemmParams p) {
+  using L = SmemLayout<BN, TMA_EPI>;
   constexpr int kStages = L::kStages;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * L::kABytes;
-  uint32_t* epi = reinterpret_cast<uint32_t*>(smem + kStages * L::kStageBytes);
+  uint8_t* epi = smem + kStages * L::kStageBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStages * L::kStageBytes + L::kEpiBytes);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + kStages;
+  // TMA epilogue ring barriers, kEpiBoxes per consumer warpgroup (one per slot at most)
+  uint64_t* epi_full = bars + 2 * kStages;
+  uint64_t* epi_empty = epi_full + 2 * kEpiBoxes;
 
   const int wg = threadIdx.x >> 7;
   const int warp_idx = threadIdx.x >> 5;
@@ -74,11 +202,18 @@ __global__ void __launch_bounds__(kNumThreads, 1)
   if (warp_idx == 0 && elect_one()) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (TMA_EPI) tma_prefetch_desc(&tmOut);
   }
   if (warp_idx == 1 && elect_one()) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8 * MC);  // every consumer warp of every CTA of the cluster
+    }
+    if constexpr (TMA_EPI) {
+      for (int i = 0; i < 2 * kEpiBoxes; ++i) {
+        mbar_init(&epi_full[i], 1);
+        mbar_init(&epi_empty[i], 1);  // the store-issuing thread of the warpgroup
+      }
     }
     fence_barrier_init();
   }
@@ -145,16 +280,58 @@ __global__ void __launch_bounds__(kNumThreads, 1)
           }
         }
       }
+    } else if (TMA_EPI && warp_idx == 1 && epi_in_boxes(p.flags) > 0 && elect_one()) {
+      // epilogue operands: the x0 / xl / mask boxes of every 64-column group of this CTA's rows, in the order
+      // the consumers walk them; skipped where the group or the warpgroup's rows lie wholly outside the output
+      const int flags = p.flags;
+      const int n_in = epi_in_boxes(flags);
+      const int slots = kEpiBoxes / n_in;
+      if (flags & EPI_CROSS) tma_prefetch_desc(&tmX0);
+      if (flags & (EPI_CROSS | EPI_ADD)) tma_prefetch_desc(&tmXl);
+      if (flags & EPI_MASK) tma_prefetch_desc(&tmMask);
+      int slot[2] = {0, 0};
+      uint32_t phase[2] = {0, 0};
+      for (int t = cluster_id; t < total_tiles; t += num_clusters) {
+        const int n_blk = t % p.n_tiles;
+        const int m_blk = ((t / p.n_tiles) % m_groups) * MC + cta_rank;
+        for (int g = 0; g < BN / 64; ++g) {
+          const int n0 = n_blk * BN + g * 64;
+          if (n0 >= p.N) break;
+#pragma unroll
+          for (int cw = 0; cw < 2; ++cw) {
+            const int m0 = m_blk * BLOCK_M + cw * 64;
+            if (m0 >= p.M) continue;
+            const int s = cw * kEpiBoxes + slot[cw];
+            mbar_wait(&epi_empty[s], phase[cw] ^ 1);
+            mbar_arrive_expect_tx(&epi_full[s], n_in * kEpiBoxBytes);
+            uint8_t* box = epi + (cw * kEpiBoxes + slot[cw] * n_in) * kEpiBoxBytes;
+            if (flags & EPI_CROSS) {
+              tma_load_2d(box, &tmX0, &epi_full[s], n0, m0);
+              tma_load_2d(box + kEpiBoxBytes, &tmXl, &epi_full[s], n0, m0);
+            } else if (flags & EPI_ADD) {
+              tma_load_2d(box, &tmXl, &epi_full[s], n0, m0);
+            }
+            if (flags & EPI_MASK) tma_load_2d(box + (n_in - 1) * kEpiBoxBytes, &tmMask, &epi_full[s], n0, m0);
+            if (++slot[cw] == slots) {
+              slot[cw] = 0;
+              phase[cw] ^= 1;
+            }
+          }
+        }
+      }
     }
   } else {
     // ===================== wgmma consumers + epilogue (64 rows each) =====================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int cw = wg - 1;                       // 0 / 1: rows [64 cw, 64 cw + 64) of the tile
     const int lane = threadIdx.x & 31;
-    uint32_t* slab = epi + cw * (kEpiSlabBytes / 4);
+    uint32_t* slab = reinterpret_cast<uint32_t*>(epi + cw * kEpiSlabBytes);
+    uint8_t* ring = epi + cw * kEpiBoxes * kEpiBoxBytes;
     const int flags = p.flags;
     int stage = 0;
     uint32_t phase = 0;
+    int epi_slot = 0, epi_pending = -1;
+    uint32_t epi_phase = 0;
     float acc[BN / 2];
     for (int t = cluster_id; t < total_tiles; t += num_clusters) {
       const int n_blk = t % p.n_tiles;
@@ -184,6 +361,14 @@ __global__ void __launch_bounds__(kNumThreads, 1)
                                                       (kb > kb0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_fence_regs(acc);
+        if (TMA_EPI && epi_pending >= 0) {
+          // the previous tile's last TMA store, deferred to here so that it overlaps this tile's first wgmma
+          if ((threadIdx.x & 127) == 0) {
+            bulk_wait_read<0>();
+            if (epi_in_boxes(flags) > 0) mbar_arrive(&epi_empty[cw * kEpiBoxes + epi_pending]);
+          }
+          epi_pending = -1;
+        }
         if (prev >= 0) {
           wgmma_wait<1>();  // the previous k block's wgmma has finished reading its slot
           if (lane == 0) {
@@ -205,8 +390,16 @@ __global__ void __launch_bounds__(kNumThreads, 1)
         else
           for (int r = 0; r < MC; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
       }
-      epilogue_tile_wg<BN>(p, flags, acc, slab, m_blk * BLOCK_M + cw * 64, n_blk * BN, cw);
+      if constexpr (TMA_EPI) {
+        if (m_blk * BLOCK_M + cw * 64 < p.M)
+          epilogue_tile_tma<BN>(p, flags, acc, ring, epi_full + cw * kEpiBoxes, epi_empty + cw * kEpiBoxes,
+                                &tmOut, &tmAux, m_blk * BLOCK_M + cw * 64, n_blk * BN, cw, epi_slot, epi_phase,
+                                epi_pending);
+      } else {
+        epilogue_tile_wg<BN>(p, flags, acc, slab, m_blk * BLOCK_M + cw * 64, n_blk * BN, cw);
+      }
     }
+    if (TMA_EPI && (threadIdx.x & 127) == 0) bulk_wait<0>();  // the stores are complete before the CTA exits
   }
 
   __syncthreads();
@@ -248,12 +441,17 @@ static int make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t inner, uint6
   return r == CUDA_SUCCESS ? 0 : -2;
 }
 
-template <int BN, bool A_MN, bool B_MN, int MC>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams& p,
+// [64 x 64] boxes of the TMA epilogue's bf16 tensors; only the maps the flags use are encoded
+struct EpiMaps {
+  CUtensorMap out, aux, x0, xl, mask;
+};
+
+template <int BN, bool A_MN, bool B_MN, int MC, bool TMA_EPI>
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& em, const GemmParams& p,
                   cudaStream_t stream) {
-  using L = SmemLayout<BN>;
+  using L = SmemLayout<BN, TMA_EPI>;
   static bool attr_set = false;
-  auto kern = gemm_tc_kernel<BN, A_MN, B_MN, MC>;
+  auto kern = gemm_tc_kernel<BN, A_MN, B_MN, MC, TMA_EPI>;
   if (!attr_set) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal) !=
         cudaSuccess)
@@ -276,8 +474,52 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const GemmParams
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  if (cudaLaunchKernelEx(&cfg, kern, ta, tb, p) != cudaSuccess) return -4;
+  if (cudaLaunchKernelEx(&cfg, kern, ta, tb, em.out, em.aux, em.x0, em.xl, em.mask, p) != cudaSuccess)
+    return -4;
   return cudaGetLastError() == cudaSuccess ? 0 : -4;
+}
+
+template <bool TMA_EPI>
+static int dispatch(int BN, int mc, int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb,
+                    const EpiMaps& em, const GemmParams& p, cudaStream_t stream) {
+#define HCTR_DISPATCH(BNV, MCV)                                                             \
+  if (a_mn) {                                                                               \
+    if (b_mn) return launch<BNV, true, true, MCV, TMA_EPI>(ta, tb, em, p, stream);          \
+    return launch<BNV, true, false, MCV, TMA_EPI>(ta, tb, em, p, stream);                   \
+  } else {                                                                                  \
+    if (b_mn) return launch<BNV, false, true, MCV, TMA_EPI>(ta, tb, em, p, stream);         \
+    return launch<BNV, false, false, MCV, TMA_EPI>(ta, tb, em, p, stream);                  \
+  }
+  if (mc == 2) {
+    if (BN == 256) { HCTR_DISPATCH(256, 2) }
+    if (BN == 64) { HCTR_DISPATCH(64, 2) }
+    HCTR_DISPATCH(128, 2)
+  }
+  if (BN == 256) { HCTR_DISPATCH(256, 1) }
+  if (BN == 64) { HCTR_DISPATCH(64, 1) }
+  HCTR_DISPATCH(128, 1)
+#undef HCTR_DISPATCH
+}
+
+// The TMA epilogue takes bf16 outputs without addf whose slot holds at most two boxes, and whose epilogue tensors
+// TMA can address (16-byte bases and pitches) and bias, if any, is 8-byte aligned (float2 loads); it encodes
+// their maps into em.  Everything else runs the slab epilogue.
+static bool tma_epilogue_maps(EpiMaps* em, int M, int N, int flags, const void* out, long long ldo, const void* aux,
+                              long long ldaux, const void* x0, const void* xl, long long ldx, const void* mask,
+                              long long ldmask, const float* bias, const float* addf) {
+  if ((flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)) || addf != nullptr || epi_in_boxes(flags) > 2) return false;
+  if (bias != nullptr && reinterpret_cast<uintptr_t>(bias) % 8) return false;
+  auto map = [&](CUtensorMap* m, const void* ptr, long long ld) {
+    return ptr != nullptr && reinterpret_cast<uintptr_t>(ptr) % 16 == 0 && ld >= N &&
+           make_tmap_bf16(m, ptr, N, M, ld, 64, 64) == 0;
+  };
+  memset(em, 0, sizeof(*em));
+  if (!map(&em->out, out, ldo)) return false;
+  if ((flags & EPI_CROSS) && aux != nullptr && !map(&em->aux, aux, ldaux)) return false;
+  if ((flags & EPI_CROSS) && !map(&em->x0, x0, ldx)) return false;
+  if ((flags & (EPI_CROSS | EPI_ADD)) && !map(&em->xl, xl, ldx)) return false;
+  if ((flags & EPI_MASK) && !map(&em->mask, mask, ldmask)) return false;
+  return true;
 }
 
 }  // namespace hctr
@@ -326,21 +568,8 @@ extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, in
   else      rc = make_tmap_bf16(&tb, B, K, N, ldb, BLOCK_K, BN / mc);
   if (rc) return rc - 10;
 
-#define HCTR_DISPATCH(BNV, MCV)                                                   \
-  if (a_mn) {                                                                     \
-    if (b_mn) return launch<BNV, true, true, MCV>(ta, tb, p, stream);             \
-    return launch<BNV, true, false, MCV>(ta, tb, p, stream);                      \
-  } else {                                                                        \
-    if (b_mn) return launch<BNV, false, true, MCV>(ta, tb, p, stream);            \
-    return launch<BNV, false, false, MCV>(ta, tb, p, stream);                     \
-  }
-  if (mc == 2) {
-    if (BN == 256) { HCTR_DISPATCH(256, 2) }
-    if (BN == 64) { HCTR_DISPATCH(64, 2) }
-    HCTR_DISPATCH(128, 2)
-  }
-  if (BN == 256) { HCTR_DISPATCH(256, 1) }
-  if (BN == 64) { HCTR_DISPATCH(64, 1) }
-  HCTR_DISPATCH(128, 1)
-#undef HCTR_DISPATCH
+  EpiMaps em;
+  if (tma_epilogue_maps(&em, M, N, flags, out, ldo, aux, ldaux, x0, xl, ldx, mask, ldmask, bias, addf))
+    return dispatch<true>(BN, mc, a_mn, b_mn, ta, tb, em, p, stream);
+  return dispatch<false>(BN, mc, a_mn, b_mn, ta, tb, em, p, stream);
 }

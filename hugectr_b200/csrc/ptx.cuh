@@ -100,6 +100,24 @@ HCTR_DEVICE void tma_load_2d_mc(void* smem_dst, const CUtensorMap* m, uint64_t* 
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
+// 2D tile store shared -> global, tracked by this thread's bulk async-groups (out-of-bounds parts are not written)
+HCTR_DEVICE void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+HCTR_DEVICE void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N>
+HCTR_DEVICE void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// at most N of this thread's bulk groups are still in flight (writes included)
+template <int N>
+HCTR_DEVICE void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
+}
 HCTR_DEVICE uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));

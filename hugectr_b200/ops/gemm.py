@@ -55,6 +55,24 @@ def tc_eligible(a: torch.Tensor, b: torch.Tensor, a_mn: bool, b_mn: bool) -> boo
     return True
 
 
+def epi_eligible(M: int, N: int, out, bias=None, mask=None, x0=None, xl=None, aux=None, addf=None) -> bool:
+    """The kernel's epilogue reads and writes its tensors row-major with unit column stride, and from N >= 32 on in
+    16-byte vectors or TMA boxes at every 32-column chunk of a row: 16-byte bases and row pitches.  x0 and xl
+    share one pitch."""
+    for t in (out, mask, x0, xl, aux, addf):
+        if t is None:
+            continue
+        if t.dim() != 2 or t.stride(1) != 1:
+            return False
+        if N >= 32 and (t.data_ptr() % 16 or (M > 1 and (t.stride(0) * t.element_size()) % 16)):
+            return False
+    if bias is not None and ((N > 1 and bias.stride(-1) != 1) or (N >= 32 and bias.data_ptr() % 16)):
+        return False
+    if x0 is not None and xl is not None and x0.stride(0) != xl.stride(0):
+        return False
+    return True
+
+
 def gemm_reference(a, b, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, xl=None,
                    alpha=1.0, flags=0, out=None, aux=None, addf=None):
     """fp32 PyTorch oracle with the same epilogue semantics as the kernel."""
@@ -187,17 +205,19 @@ def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x
         if colsum is not None:
             colsum.add_(out.float().sum(0))
         return r
-    if not tc_eligible(a, b, a_mn, b_mn) or out.stride(1) != 1:
+    operands_ok = tc_eligible(a, b, a_mn, b_mn)
+    if not operands_ok or not epi_eligible(M, N, out, bias, mask, x0, xl, aux, addf):
         if a.is_cuda:
-            # never silent: a misaligned / non-bf16 operand moves this GEMM off the wgmma kernel
+            # never silent: a misaligned / non-bf16 operand or epilogue tensor moves this GEMM off the wgmma kernel
             sig = (M, N, K, str(a.dtype), tuple(a.stride()), tuple(b.stride()), a.data_ptr() % 16,
-                   b.data_ptr() % 16)
+                   b.data_ptr() % 16, operands_ok)
             if sig not in _fallback_logged:
                 _fallback_logged.add(sig)
                 from ..utils import logger
-                logger.warning(f"gemm_bf16: M={M} N={N} K={K} dtype={a.dtype} strides a={tuple(a.stride())} "
-                               f"b={tuple(b.stride())} is not TMA-addressable (16-byte base / pitch, bf16): "
-                               "running the library matmul instead of the wgmma kernel")
+                what = (f"an epilogue tensor (out / bias / mask / x0 / xl / aux / addf, flags={flags})" if operands_ok
+                        else f"dtype={a.dtype} strides a={tuple(a.stride())} b={tuple(b.stride())}")
+                logger.warning(f"gemm_bf16: M={M} N={N} K={K} {what} is not TMA-addressable (16-byte base / pitch, "
+                               "bf16): running the library matmul instead of the wgmma kernel")
         r = gemm_reference(a, b, a_mn, b_mn, bias, mask, x0, xl, alpha, flags, out, aux, addf)
         if colsum is not None:
             colsum.add_(out.float().sum(0))
@@ -250,6 +270,9 @@ def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alph
     if torch.cuda.is_current_stream_capturing():
         return heur
     cands = [1128, 1256] if N >= 256 else [1128]
+    if not (flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)):
+        # with the TMA epilogue, memory-bound bf16-output calls can win on more, narrower tiles
+        cands = [1064] + cands + [64, 128, 256]
     if len(cands) == 1:
         _TUNE_CACHE[key] = cands[0]
         return cands[0]
@@ -258,18 +281,20 @@ def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alph
         so.zero_()
     sa = (torch.empty_strided(aux.size(), aux.stride(), dtype=aux.dtype, device=aux.device)
           if aux is not None else None)
-    best, best_t = heur, float("inf")
     for bn in cands:
         for _ in range(2):
             _launch(a, b, so, M, N, K, a_mn, b_mn, bias, mask, x0, xl, sa, alpha, flags, splits, bn, addf)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(5):
-            _launch(a, b, so, M, N, K, a_mn, b_mn, bias, mask, x0, xl, sa, alpha, flags, splits, bn, addf)
-        e1.record()
-        e1.synchronize()
-        t = e0.elapsed_time(e1)
-        if t < best_t:
-            best, best_t = bn, t
+    # candidates alternate over the rounds so that a slow spell of a shared GPU does not decide the pick
+    times = {bn: [] for bn in cands}
+    for _ in range(3):
+        for bn in cands:
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            for _ in range(5):
+                _launch(a, b, so, M, N, K, a_mn, b_mn, bias, mask, x0, xl, sa, alpha, flags, splits, bn, addf)
+            e1.record()
+            e1.synchronize()
+            times[bn].append(e0.elapsed_time(e1))
+    best = min(cands, key=lambda bn: sorted(times[bn])[1])
     _TUNE_CACHE[key] = best
     return best

@@ -2,6 +2,7 @@
 torch.mm alone and against gemm_library (torch.mm + the same epilogue in eager PyTorch).
 
   python tools_dev/bench_gemm.py [--batch 6912] [--iters 20] [--rounds 7] [--out DIR] [--tree DIR]
+  python tools_dev/bench_gemm.py --check-bits OTHER_TREE [--tree DIR] [--batch 6912]
 
 The call list is recorded, not hand-written: build_dlrm_dcnv2 (batch --batch, small tables; GEMM shapes depend
 on the batch and the dense widths only) runs one eager training step with gemm_bf16 wrapped, and every call is
@@ -13,8 +14,14 @@ sheet.  Bytes are one pass over every operand and epilogue tensor (fp32 accumula
 
 --tree DIR imports hugectr_b200 from another checkout (built in place), so that two builds can be timed one
 process per run in one session.  Without a CUDA device the tool exits with an error and measures nothing.
+
+--check-bits OTHER_TREE times nothing: it replays every recorded call that does not accumulate into its output
+(no EPI_ATOMIC / EPI_ACCUM, no split K) on the same seeded operands under this tree and under OTHER_TREE, one
+process each, and reports per call whether `out` and `aux` are equal bit for bit.  The K order of the
+accumulation does not depend on the tile, so two builds that tune to different tiles still agree.
 """
 import argparse
+import hashlib
 import json
 import os
 import subprocess
@@ -126,6 +133,56 @@ def time_arms(arms, iters, rounds):
     return {k: sorted(v)[len(v) // 2] for k, v in ts.items()}
 
 
+def output_digests(batch):
+    """sha256 of `out` and `aux` of every non-accumulating recorded call, replayed on seeded operands."""
+    from hugectr_b200.ops import gemm as G
+    calls = record_calls(batch)
+    gen = torch.Generator().manual_seed(0)
+    res = []
+    for i, c in enumerate(calls):
+        ts = make_operands(c, gen)
+        if c["flags"] & (G.EPI_ATOMIC | G.EPI_ACCUM) or c["splits"] > 1:
+            continue
+        kw = dict(a_mn=c["a_mn"], b_mn=c["b_mn"], flags=c["flags"], splits=c["splits"], alpha=c["alpha"])
+        kw.update({k: ts[k] for k in TENSORS[3:] if k in ts and k != "colsum"})
+        G.gemm_bf16(ts["a"], ts["b"], ts["out"], **kw)
+        torch.cuda.synchronize()
+        d = {"call": i, "M": shape_of(c)[0], "N": shape_of(c)[1], "K": shape_of(c)[2], "flags": c["flags"]}
+        for k in ("out", "aux"):
+            if k in ts:
+                d[k] = hashlib.sha256(ts[k].contiguous().view(torch.uint8).cpu().numpy().tobytes()).hexdigest()
+        res.append(d)
+    return res
+
+
+def check_bits(a):
+    """Run output_digests under this tree and a.check_bits, one process each, and compare."""
+    runs = {}
+    for tree in (a.tree, a.check_bits):
+        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--tree", tree, "--batch", str(a.batch),
+                            "--digests"], capture_output=True, text=True)
+        if r.returncode != 0:
+            print(r.stdout[-2000:] + r.stderr[-4000:], file=sys.stderr)
+            return 1
+        runs[tree] = json.loads(r.stdout.strip().splitlines()[-1])
+    mine, other = runs[a.tree], runs[a.check_bits]
+    bad = 0
+    if len(mine) != len(other):
+        print(json.dumps({"error": "different call lists", "calls": [len(mine), len(other)]}))
+        return 1
+    for x, y in zip(mine, other):
+        same = {k: x.get(k) == y.get(k) for k in ("out", "aux") if k in x or k in y}
+        bad += not all(same.values())
+        print(json.dumps({k: x[k] for k in ("call", "M", "N", "K", "flags")} | {"equal": same}), flush=True)
+    summary = {"check_bits": os.path.abspath(a.check_bits), "calls": len(mine), "mismatches": bad}
+    print(json.dumps(summary), flush=True)
+    if a.out:
+        os.makedirs(a.out, exist_ok=True)
+        with open(os.path.join(a.out, "check_bits.json"), "w") as f:
+            json.dump(summary, f)
+    return 1 if bad else 0
+
+
 def main(argv):
     ap = argparse.ArgumentParser()
     ap.add_argument("--batch", type=int, default=6912)
@@ -133,13 +190,23 @@ def main(argv):
     ap.add_argument("--rounds", type=int, default=7)
     ap.add_argument("--out", default="", help="also write the JSON lines to DIR/bench_gemm.jsonl")
     ap.add_argument("--tree", default=ROOT)
+    ap.add_argument("--check-bits", default="", metavar="OTHER_TREE",
+                    help="compare the outputs of every non-accumulating call with OTHER_TREE's, bit for bit")
+    ap.add_argument("--digests", action="store_true", help=argparse.SUPPRESS)
     a = ap.parse_args(argv)
+    if a.check_bits and not os.path.isdir(os.path.join(a.check_bits, "hugectr_b200")):
+        raise SystemExit(f"bench_gemm: {a.check_bits} holds no hugectr_b200 package")
     if not os.path.isdir(os.path.join(a.tree, "hugectr_b200")):
         raise SystemExit(f"bench_gemm: {a.tree} holds no hugectr_b200 package")
     if not torch.cuda.is_available():
         print("bench_gemm: needs a CUDA device (an H100); nothing was measured", file=sys.stderr)
         return 1
+    if a.check_bits:
+        return check_bits(a)
     sys.path.insert(0, os.path.abspath(a.tree))
+    if a.digests:
+        print(json.dumps(output_digests(a.batch)))
+        return 0
     from hugectr_b200.ops import gemm as G
     name, info = card()
     head = {"device": name, "power_limit,sm_clock,max_sm_clock": info, "tree": os.path.abspath(a.tree),
