@@ -32,14 +32,8 @@ __global__ void __launch_bounds__(256) dense_opt_kernel(const DenseOptArgs a) {
   constexpr bool kHasS0 = OPT != OPT_SGD;
   constexpr bool kHasS1 = OPT == OPT_ADAM || OPT == OPT_FTRL;
   const OptHyper& hp = a.hp;
-  const float lr = *hp.lr_ptr * hp.lr_scale;
+  const OptStep step = opt_step<OPT>(hp);
   const float inv_scaler = 1.f / hp.scaler;
-  float bc1 = 1.f, bc2 = 1.f;
-  if constexpr (OPT == OPT_ADAM) {
-    const float t = static_cast<float>(*hp.step_ptr);
-    bc1 = 1.f - powf(hp.beta1, t);
-    bc2 = 1.f - powf(hp.beta2, t);
-  }
   const long long stride = static_cast<long long>(gridDim.x) * blockDim.x * 4;
   for (long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4; i < a.n;
        i += stride) {
@@ -69,7 +63,7 @@ __global__ void __launch_bounds__(256) dense_opt_kernel(const DenseOptArgs a) {
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j)
-      apply_opt<OPT, float>(w[j], g[j] * inv_scaler, s0 + j, s1 + j, 0, hp, lr, bc1, bc2);
+      apply_opt<OPT, float>(w[j], g[j] * inv_scaler, s0 + j, s1 + j, 0, hp, step);
     if (cnt == 4) {
       *reinterpret_cast<float4*>(a.w + i) = make_float4(w[0], w[1], w[2], w[3]);
       if (a.zero_grad) *reinterpret_cast<float4*>(a.g + i) = make_float4(0.f, 0.f, 0.f, 0.f);

@@ -292,8 +292,7 @@ __global__ void __launch_bounds__(256)
   const KeyT* keys = reinterpret_cast<const KeyT*>(p.keys[0]) + lk.key_off;
   const GradT* grads = reinterpret_cast<const GradT*>(p.grad[0]) + lk.grad_off;
   for (int s = s0 + warp; s < s1; s += 8) {
-    int nnz = lk.hotness;
-    if (lk.nnz_off >= 0) nnz = min(lk.hotness, p.nnz[0][lk.nnz_off + s]);
+    const int nnz = bucket_nnz(p, lk.hotness, lk.nnz_off, 0, s);
     if (nnz <= 0) continue;
     float scale = grad_scale;
     if (lk.combiner == 1) scale /= static_cast<float>(nnz);
@@ -331,8 +330,8 @@ __global__ void __launch_bounds__(256)
 }
 
 // Row-wise AdaGrad on one row by one warp (accumulate path and data-parallel tables): a warp-reduced
-// pass over the row's fp32 gradient gives sum g^2, lane 0 updates the row's accumulator *s, then the
-// update pass applies the factor to every column and zeroes the gradient.
+// pass over the row's fp32 gradient gives sum g^2, rowwise_row_step updates the row's accumulator *s,
+// then the update pass applies the factor to every column and zeroes the gradient.
 template <typename WT>
 HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, float* gsrc, long long base, int ev,
                                       float inv_scaler, const OptHyper& hp, float lr,
@@ -342,7 +341,7 @@ HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, float* gsrc, long long
   if (v4) {
     for (int col = lane * 4; col < ev; col += 128) {
       const float4 g = *reinterpret_cast<const float4*>(gsrc + col);
-      sq += sumsq4(make_float4(g.x * inv_scaler, g.y * inv_scaler, g.z * inv_scaler, g.w * inv_scaler));
+      sq += sumsq4(scale4(g, inv_scaler));
     }
   } else {
     for (int col = lane; col < ev; col += 32) {
@@ -350,21 +349,14 @@ HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, float* gsrc, long long
       sq += g * g;
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-  float f = 0.f;
-  if (lane == 0) {
-    const float s_new = rowwise_accumulate(*s, sq, ev);
-    *s = s_new;
-    f = rowwise_factor(s_new, hp, lr);
-  }
-  f = __shfl_sync(0xffffffffu, f, 0);
+  const float s_old = lane == 0 ? *s : 0.f;
+  const float f = rowwise_row_step<32>(0xffffffffu, 0, lane, sq, s_old, s, ev, hp, lr);
   if (v4) {
     for (int col = lane * 4; col < ev; col += 128) {
       const float4 g = *reinterpret_cast<float4*>(gsrc + col);
       *reinterpret_cast<float4*>(gsrc + col) = make_float4(0.f, 0.f, 0.f, 0.f);
       float4 w = load_vec4<WT>(table + base + col);
-      apply_rowwise4(w, make_float4(g.x * inv_scaler, g.y * inv_scaler, g.z * inv_scaler, g.w * inv_scaler), f);
+      apply_rowwise4(w, scale4(g, inv_scaler), f);
       store_w4<WT>(table + base + col, w, srk, base + col);
     }
   } else {
@@ -386,13 +378,7 @@ __global__ void __launch_bounds__(256)
                       float* __restrict__ wgrad_unique, const UniqueTable ut, const int ev,
                       const OptHyper hp) {
   const unsigned int n = min(*ut.counter, ut.max_unique);
-  const float lr = (hp.lr_ptr ? *hp.lr_ptr : 1.f) * hp.lr_scale;
-  float bc1 = 1.f, bc2 = 1.f;
-  if constexpr (OPT == OPT_ADAM) {
-    const float t = static_cast<float>(hp.step_ptr ? *hp.step_ptr : 1u);
-    bc1 = 1.f - powf(hp.beta1, t);
-    bc2 = 1.f - powf(hp.beta2, t);
-  }
+  const OptStep step = opt_step<OPT>(hp);
   const float inv_scaler = 1.f / hp.scaler;
   const unsigned long long srk = sr_key<WT>(hp.sr_seed, hp.step_ptr);
   const int lane = threadIdx.x & 31;
@@ -402,13 +388,13 @@ __global__ void __launch_bounds__(256)
     float* gsrc = wgrad_unique + static_cast<long long>(uid) * ev;
     const long long base = static_cast<long long>(row) * ev;
     if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
-      rowwise_update_warp<WT>(table, s0 + row, gsrc, base, ev, inv_scaler, hp, lr, srk, lane);
+      rowwise_update_warp<WT>(table, s0 + row, gsrc, base, ev, inv_scaler, hp, step.lr, srk, lane);
     } else if ((ev & 3) == 0) {
       for (int col = lane * 4; col < ev; col += 128) {
         float4 g = *reinterpret_cast<float4*>(gsrc + col);
         *reinterpret_cast<float4*>(gsrc + col) = make_float4(0.f, 0.f, 0.f, 0.f);
         float4 w = load_vec4<WT>(table + base + col);
-        apply_opt4<OPT, StateT>(w, make_float4(g.x * inv_scaler, g.y * inv_scaler, g.z * inv_scaler, g.w * inv_scaler), s0, s1, base + col, hp, lr, bc1, bc2);
+        apply_opt4<OPT, StateT>(w, scale4(g, inv_scaler), s0, s1, base + col, hp, step);
         store_w4<WT>(table + base + col, w, srk, base + col);
       }
     } else {
@@ -416,15 +402,11 @@ __global__ void __launch_bounds__(256)
         const float g = gsrc[col];
         gsrc[col] = 0.f;
         float w = to_f<WT>(table[base + col]);
-        apply_opt<OPT, StateT>(w, g * inv_scaler, s0, s1, base + col, hp, lr, bc1, bc2);
+        apply_opt<OPT, StateT>(w, g * inv_scaler, s0, s1, base + col, hp, step);
         store_w<WT>(table + base + col, w, srk, base + col);
       }
     }
-    if (lane == 0) {
-      const unsigned int slot = ut.slots[uid];
-      ut.keys[slot] = kEmptyKey;
-      ut.vals[slot] = kInvalidVal;
-    }
+    if (lane == 0) unique_release(ut, uid);
   }
 }
 
@@ -435,7 +417,7 @@ __global__ void __launch_bounds__(256)
     emb_dp_rowwise_update_kernel(float* __restrict__ table, float* __restrict__ s,
                                  float* __restrict__ wgrad, const long long rows, const int pitch,
                                  const OptHyper hp) {
-  const float lr = (hp.lr_ptr ? *hp.lr_ptr : 1.f) * hp.lr_scale;
+  const float lr = opt_step<OPT_ROWWISE_ADAGRAD>(hp).lr;
   const float inv_scaler = 1.f / hp.scaler;
   const int lane = threadIdx.x & 31;
   const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
@@ -497,22 +479,16 @@ extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, i
   // passes of 256 columns (keeps the accumulators of the scalar kernel in registers)
   const int pass = (vec == 4) ? max_ev : 8 * G;
   for (int c0 = 0; c0 < max_ev; c0 += pass) {
-#define LAUNCH(K, O, V, UU)                                                                       \
-  if (table_bf16) emb_fwd_kernel<K, O, V, UU, __nv_bfloat16><<<blocks, threads, 0, st>>>(*p, G, c0); \
-  else emb_fwd_kernel<K, O, V, UU, float><<<blocks, threads, 0, st>>>(*p, G, c0)
-#define LAUNCH_U(K, O, V)            \
-  if (narrow) { LAUNCH(K, O, V, 4); } \
-  else { LAUNCH(K, O, V, 8); }
-  if (vec == 4) {
-    if (key_bytes == 8) { if (out_bf16) { LAUNCH_U(long long, __nv_bfloat16, 4) } else { LAUNCH_U(long long, float, 4) } }
-    else { if (out_bf16) { LAUNCH_U(int, __nv_bfloat16, 4) } else { LAUNCH_U(int, float, 4) } }
-  } else {
-    if (key_bytes == 8) { if (out_bf16) { LAUNCH(long long, __nv_bfloat16, 1, 8); } else { LAUNCH(long long, float, 1, 8); } }
-    else { if (out_bf16) { LAUNCH(int, __nv_bfloat16, 1, 8); } else { LAUNCH(int, float, 1, 8); } }
+    with_key(key_bytes, [&](auto k) { with_elem(out_bf16, [&](auto o) { with_elem(table_bf16, [&](auto w) {
+      auto launch = [&](auto v, auto u) {   // vector width, rows in flight per gather round
+        emb_fwd_kernel<type_of<decltype(k)>, type_of<decltype(o)>, decltype(v)::value, decltype(u)::value,
+                       type_of<decltype(w)>><<<blocks, threads, 0, st>>>(*p, G, c0);
+      };
+      if (vec == 1) launch(Int<1>{}, Int<8>{});
+      else if (narrow) launch(Int<4>{}, Int<4>{});
+      else launch(Int<4>{}, Int<8>{});
+    }); }); });
   }
-  }
-#undef LAUNCH_U
-#undef LAUNCH
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
@@ -550,12 +526,11 @@ extern "C" int hctr_emb_shard_split(const void* keys, void* out, int* nnz, int b
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (batch <= 0 || hotness <= 0 || k <= 1) return 0;
   const int blocks = (batch * 32 + 255) / 256;
-  if (key_bytes == 8)
-    emb_shard_split_kernel<long long><<<blocks, 256, 0, st>>>(
-        reinterpret_cast<const long long*>(keys), reinterpret_cast<long long*>(out), nnz, batch, hotness, k);
-  else
-    emb_shard_split_kernel<int><<<blocks, 256, 0, st>>>(reinterpret_cast<const int*>(keys),
-                                                        reinterpret_cast<int*>(out), nnz, batch, hotness, k);
+  with_key(key_bytes, [&](auto kt) {
+    using KeyT = type_of<decltype(kt)>;
+    emb_shard_split_kernel<KeyT><<<blocks, 256, 0, st>>>(
+        reinterpret_cast<const KeyT*>(keys), reinterpret_cast<KeyT*>(out), nnz, batch, hotness, k);
+  });
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
@@ -572,40 +547,33 @@ extern "C" int hctr_emb_backward_accum(const EmbParams* p, const UniqueTable* ut
   if (ut->keys == nullptr && p->num_ranks == 1 && dp_ev4 && p->ev_size % 4 == 0) {
     // dense wgrad of replicated tables: privatised block-level accumulation
     constexpr int kSmem = 96 * 1024;
-    static bool attr_set = false;
-    if (!attr_set) {
-      cudaFuncSetAttribute(emb_dp_wgrad_kernel<int, __nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-      cudaFuncSetAttribute(emb_dp_wgrad_kernel<int, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-      cudaFuncSetAttribute(emb_dp_wgrad_kernel<long long, __nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-      cudaFuncSetAttribute(emb_dp_wgrad_kernel<long long, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
-      attr_set = true;
-    }
     int chunks = (2 * num_sms() + p->num_lookups - 1) / p->num_lookups;
     if (chunks > 64) chunks = 64;
     if (chunks * 8 > p->batch) chunks = (p->batch + 7) / 8;
     if (chunks < 1) chunks = 1;
     const dim3 grid(chunks, p->num_lookups);
-#define LAUNCH_DP(K, O) \
-  emb_dp_wgrad_kernel<K, O><<<grid, 256, kSmem, st>>>(*p, wgrad_unique, grad_scale, kSmem / 4)
-    if (key_bytes == 8) { if (grad_bf16) LAUNCH_DP(long long, __nv_bfloat16); else LAUNCH_DP(long long, float); }
-    else { if (grad_bf16) LAUNCH_DP(int, __nv_bfloat16); else LAUNCH_DP(int, float); }
-#undef LAUNCH_DP
+    with_key(key_bytes, [&](auto k) { with_elem(grad_bf16, [&](auto g) {
+      const auto kernel = emb_dp_wgrad_kernel<type_of<decltype(k)>, type_of<decltype(g)>>;
+      // once per instantiation: this static belongs to the (k, g) instance of the lambda
+      static const cudaError_t attr =
+          cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
+      (void)attr;
+      kernel<<<grid, 256, kSmem, st>>>(*p, wgrad_unique, grad_scale, kSmem / 4);
+    }); });
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
   }
   if (max_ev > kMaxEmbWidth) return -4;
   const long long warps = (items + (32 / G) - 1) / (32 / G);
   const int threads = 256;
   const long long blocks = (warps * 32 + threads - 1) / threads;
-#define LAUNCH(K, O, V) \
-  emb_bwd_accum_kernel<K, O, V><<<(unsigned)blocks, threads, 0, st>>>(*p, *ut, wgrad_unique, grad_scale, G, items)
-  if (vec == 4) {
-    if (key_bytes == 8) { if (grad_bf16) LAUNCH(long long, __nv_bfloat16, 4); else LAUNCH(long long, float, 4); }
-    else { if (grad_bf16) LAUNCH(int, __nv_bfloat16, 4); else LAUNCH(int, float, 4); }
-  } else {
-    if (key_bytes == 8) { if (grad_bf16) LAUNCH(long long, __nv_bfloat16, 1); else LAUNCH(long long, float, 1); }
-    else { if (grad_bf16) LAUNCH(int, __nv_bfloat16, 1); else LAUNCH(int, float, 1); }
-  }
-#undef LAUNCH
+  with_key(key_bytes, [&](auto k) { with_elem(grad_bf16, [&](auto g) {
+    auto launch = [&](auto v) {
+      emb_bwd_accum_kernel<type_of<decltype(k)>, type_of<decltype(g)>, decltype(v)::value>
+          <<<(unsigned)blocks, threads, 0, st>>>(*p, *ut, wgrad_unique, grad_scale, G, items);
+    };
+    if (vec == 4) launch(Int<4>{});
+    else launch(Int<1>{});
+  }); });
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
@@ -617,8 +585,8 @@ extern "C" int hctr_emb_update(void* table, void* s0, void* s1, float* wgrad_uni
   const int threads = 256;
   const int blocks = num_sms * 8;
   const int rc = dispatch_opt(opt, state_bf16, table_bf16, [&](auto o, auto s, auto w) {
-    using StateT = typename decltype(s)::type;
-    using WT = typename decltype(w)::type;
+    using StateT = type_of<decltype(s)>;
+    using WT = type_of<decltype(w)>;
     emb_update_kernel<decltype(o)::value, StateT, WT><<<blocks, threads, 0, st>>>(
         (WT*)table, (StateT*)s0, (StateT*)s1, wgrad_unique, *ut, ev, *hp);
   });
@@ -645,13 +613,10 @@ extern "C" int hctr_emb_gather_rows(const void* table, const long long* rows, vo
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (n == 0) return 0;
   const unsigned blocks = static_cast<unsigned>((n * 32 + 255) / 256);
-#define LAUNCH(O, W) \
-  emb_gather_rows_kernel<O, W><<<blocks, 256, 0, st>>>((const W*)table, rows, (O*)out, n, ev)
-  if (table_bf16) {
-    if (out_bf16) LAUNCH(__nv_bfloat16, __nv_bfloat16); else LAUNCH(float, __nv_bfloat16);
-  } else {
-    if (out_bf16) LAUNCH(__nv_bfloat16, float); else LAUNCH(float, float);
-  }
-#undef LAUNCH
+  with_elem(out_bf16, [&](auto o) { with_elem(table_bf16, [&](auto w) {
+    using OutT = type_of<decltype(o)>;
+    using WT = type_of<decltype(w)>;
+    emb_gather_rows_kernel<OutT, WT><<<blocks, 256, 0, st>>>((const WT*)table, rows, (OutT*)out, n, ev);
+  }); });
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

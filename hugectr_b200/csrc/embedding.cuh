@@ -181,27 +181,56 @@ HCTR_DEVICE unsigned int unique_get_insert(const UniqueTable& t, unsigned long l
   }
 }
 
+// An update kernel is done with unique row uid: empties its hash slot for the next step
+HCTR_DEVICE void unique_release(const UniqueTable& t, unsigned int uid) {
+  const unsigned int slot = t.slots[uid];
+  t.keys[slot] = kEmptyKey;
+  t.vals[slot] = kInvalidVal;
+}
+
+// Keys of bucket (src rank, sample s) of a lookup with the given hotness and nnz_off: the hotness, or
+// the bucket's own count below it for a variable-hotness lookup
+HCTR_DEVICE int bucket_nnz(const EmbParams& p, int hotness, long long nnz_off, int src, int s) {
+  int nnz = hotness;
+  if (nnz_off >= 0) nnz = min(hotness, p.nnz[src][nnz_off + s]);
+  return nnz;
+}
+
 // Clears the counter of unique rows after an update and records an overflow of it (the update kernels
 // release their rows' hash slots, so the table is empty again)
 __global__ void emb_finish_kernel(unsigned int* counter, unsigned int* overflow_flag, unsigned int max_unique);
 
-// Host dispatch of the sparse optimizers: calls fn(std::integral_constant<int, OPT>, Tag<StateT>,
-// Tag<WT>) with the kernels' template arguments for optimizer `opt`, state type (bf16 when state_bf16)
-// and weight type (bf16 when table_bf16).  SGD (no state) and row-wise AdaGrad (a [rows] fp32
-// accumulator, never bf16: a value that only grows would drop small increments) run with the fp32 state
-// type.  Returns 0, -2 for an unknown optimizer, or -7 for row-wise AdaGrad with bf16 state.
+// Host dispatch of the kernels' template arguments: each helper calls a generic lambda with a tag
+// (type_of<decltype(tag)> is the type, decltype(tag)::value the integer).
 template <typename T>
 struct Tag {
   using type = T;
 };
+template <typename TagT>
+using type_of = typename TagT::type;
+template <int V>
+using Int = std::integral_constant<int, V>;
+// element type of activations, gradients, state or weights
+template <typename Fn>
+inline void with_elem(int is_bf16, Fn&& fn) {
+  if (is_bf16) fn(Tag<__nv_bfloat16>{});
+  else fn(Tag<float>{});
+}
+// key type: 8-byte or 4-byte integers
+template <typename Fn>
+inline void with_key(int key_bytes, Fn&& fn) {
+  if (key_bytes == 8) fn(Tag<long long>{});
+  else fn(Tag<int>{});
+}
+// The sparse optimizers: calls fn(Int<OPT>, Tag<StateT>, Tag<WT>) for optimizer `opt`, state type (bf16
+// when state_bf16) and weight type (bf16 when table_bf16).  SGD (no state) and row-wise AdaGrad (a
+// [rows] fp32 accumulator, never bf16: a value that only grows would drop small increments) run with the
+// fp32 state type.  Returns 0, -2 for an unknown optimizer, or -7 for row-wise AdaGrad with bf16 state.
 template <typename Fn>
 inline int dispatch_opt(int opt, int state_bf16, int table_bf16, Fn&& fn) {
   auto run = [&](auto o) {
     constexpr int O = decltype(o)::value;
-    auto with_w = [&](auto s) {
-      if (table_bf16) fn(o, s, Tag<__nv_bfloat16>{});
-      else fn(o, s, Tag<float>{});
-    };
+    auto with_w = [&](auto s) { with_elem(table_bf16, [&](auto w) { fn(o, s, w); }); };
     if constexpr (O != OPT_SGD && O != OPT_ROWWISE_ADAGRAD) {
       if (state_bf16) return with_w(Tag<__nv_bfloat16>{});
     }
@@ -209,14 +238,14 @@ inline int dispatch_opt(int opt, int state_bf16, int table_bf16, Fn&& fn) {
   };
   if (opt == OPT_ROWWISE_ADAGRAD && state_bf16) return -7;
   switch (opt) {
-    case OPT_SGD: run(std::integral_constant<int, OPT_SGD>{}); break;
-    case OPT_ADAGRAD: run(std::integral_constant<int, OPT_ADAGRAD>{}); break;
-    case OPT_ADAM: run(std::integral_constant<int, OPT_ADAM>{}); break;
-    case OPT_FTRL: run(std::integral_constant<int, OPT_FTRL>{}); break;
-    case OPT_MOMENTUM: run(std::integral_constant<int, OPT_MOMENTUM>{}); break;
-    case OPT_NESTEROV: run(std::integral_constant<int, OPT_NESTEROV>{}); break;
-    case OPT_RMSPROP: run(std::integral_constant<int, OPT_RMSPROP>{}); break;
-    case OPT_ROWWISE_ADAGRAD: run(std::integral_constant<int, OPT_ROWWISE_ADAGRAD>{}); break;
+    case OPT_SGD: run(Int<OPT_SGD>{}); break;
+    case OPT_ADAGRAD: run(Int<OPT_ADAGRAD>{}); break;
+    case OPT_ADAM: run(Int<OPT_ADAM>{}); break;
+    case OPT_FTRL: run(Int<OPT_FTRL>{}); break;
+    case OPT_MOMENTUM: run(Int<OPT_MOMENTUM>{}); break;
+    case OPT_NESTEROV: run(Int<OPT_NESTEROV>{}); break;
+    case OPT_RMSPROP: run(Int<OPT_RMSPROP>{}); break;
+    case OPT_ROWWISE_ADAGRAD: run(Int<OPT_ROWWISE_ADAGRAD>{}); break;
     default: return -2;
   }
   return 0;

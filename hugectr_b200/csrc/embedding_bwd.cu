@@ -44,6 +44,27 @@ struct BwdIndex {
   unsigned int* class_count;  // [2] light / medium list lengths
 };
 
+// ---------------------------------------------------------------- scans
+HCTR_DEVICE unsigned int warp_inclusive_scan(unsigned int x, int lane) {
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  return x;
+}
+// Exclusive scan of one value per thread of a 1024-thread block.  w: 32 words of shared memory, free
+// again after the caller's next __syncthreads.  Thread 1023's result plus its v is the block's total.
+HCTR_DEVICE unsigned int block_exclusive_scan_1024(unsigned int v, unsigned int* w) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned int x = warp_inclusive_scan(v, lane);
+  if (lane == 31) w[warp] = x;
+  __syncthreads();
+  if (warp == 0) w[lane] = warp_inclusive_scan(w[lane], lane);
+  __syncthreads();
+  return (warp ? w[warp - 1] : 0u) + x - v;
+}
+
 // ---------------------------------------------------------------- A: unique ids + counts
 // Block-aggregated: a block de-duplicates its kPairsPerBlock (bucket,key) pairs in a shared-memory
 // hash first, so a power-law head row costs ONE global CAS + ONE global atomicAdd per block instead
@@ -96,10 +117,7 @@ __global__ void __launch_bounds__(kIdxThreads)
     if (pair >= total_pairs) continue;
     const PairInfo pi = decode_pair(p, s_pair_off, pair);
     const EmbLookup* lk = p.lookups + pi.l;
-    int nnz = __ldg(&lk->hotness);
-    const long long no = __ldg(&lk->nnz_off);
-    if (no >= 0) nnz = min(nnz, p.nnz[pi.src][no + pi.s]);
-    if (pi.h >= nnz) continue;
+    if (pi.h >= bucket_nnz(p, __ldg(&lk->hotness), __ldg(&lk->nnz_off), pi.src, pi.s)) continue;
     const KeyT* kp = reinterpret_cast<const KeyT*>(p.keys[pi.src]) + __ldg(&lk->key_off) +
                      static_cast<long long>(pi.s) * __ldg(&lk->key_stride) + pi.h;
     const long long key = static_cast<long long>(*kp);
@@ -152,12 +170,7 @@ __global__ void __launch_bounds__(kIdxThreads)
   }
   __shared__ unsigned int s_warp_sum[kIdxThreads / 32];
   __shared__ unsigned int s_base;
-  unsigned int incl = nnew;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned int v = __shfl_up_sync(0xffffffffu, incl, o);
-    if ((threadIdx.x & 31) >= o) incl += v;
-  }
+  const unsigned int incl = warp_inclusive_scan(nnew, threadIdx.x & 31);
   if ((threadIdx.x & 31) == 31) s_warp_sum[threadIdx.x >> 5] = incl;
   __syncthreads();
   if (threadIdx.x == 0) {
@@ -259,30 +272,11 @@ __global__ void __launch_bounds__(1024)
   for (unsigned int base = 0; base < nb; base += 1024) {
     const unsigned int i = base + threadIdx.x;
     const unsigned int v = i < nb ? sums[i] : 0u;
-    unsigned int x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned int y = __shfl_up_sync(0xffffffffu, x, o);
-      if ((threadIdx.x & 31) >= o) x += y;
-    }
-    if ((threadIdx.x & 31) == 31) w[threadIdx.x >> 5] = x;
+    const unsigned int scan = block_exclusive_scan_1024(v, w);
+    const unsigned int excl = carry_s + scan;
+    if (i < nb) sums[i] = excl;
     __syncthreads();
-    if (threadIdx.x < 32) {
-      unsigned int z = w[threadIdx.x];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const unsigned int y = __shfl_up_sync(0xffffffffu, z, o);
-        if (threadIdx.x >= o) z += y;
-      }
-      w[threadIdx.x] = z;
-    }
-    __syncthreads();
-    const unsigned int warp_prefix = (threadIdx.x >> 5) ? w[(threadIdx.x >> 5) - 1] : 0u;
-    const unsigned int incl = x + warp_prefix;
-    const unsigned int carry = carry_s;
-    if (i < nb) sums[i] = carry + incl - v;
-    __syncthreads();
-    if (threadIdx.x == 1023) carry_s = carry + incl;
+    if (threadIdx.x == 1023) carry_s = excl + v;
     __syncthreads();
   }
 }
@@ -294,27 +288,9 @@ __global__ void __launch_bounds__(1024)
   if (blockIdx.x * 1024 >= n) return;
   const unsigned int i = blockIdx.x * 1024 + threadIdx.x;
   const unsigned int v = i < n ? in[i] : 0u;
-  unsigned int x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const unsigned int y = __shfl_up_sync(0xffffffffu, x, o);
-    if ((threadIdx.x & 31) >= o) x += y;
-  }
   __shared__ unsigned int w[32];
-  if ((threadIdx.x & 31) == 31) w[threadIdx.x >> 5] = x;
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    unsigned int z = w[threadIdx.x];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const unsigned int y = __shfl_up_sync(0xffffffffu, z, o);
-      if (threadIdx.x >= o) z += y;
-    }
-    w[threadIdx.x] = z;
-  }
-  __syncthreads();
-  const unsigned int warp_prefix = (threadIdx.x >> 5) ? w[(threadIdx.x >> 5) - 1] : 0u;
-  const unsigned int excl = sums[blockIdx.x] + warp_prefix + x - v;
+  const unsigned int scan = block_exclusive_scan_1024(v, w);
+  const unsigned int excl = sums[blockIdx.x] + scan;
   if (i < n) offsets[i] = excl;
   if (i == n - 1) offsets[n] = excl + v;
 }
@@ -373,9 +349,7 @@ __global__ void __launch_bounds__(kIdxThreads)
     if (ix.bucket_scale != nullptr) {
       float sc = 1.f;
       if (__ldg(&lk->combiner) == 1) {
-        int nnz = __ldg(&lk->hotness);
-        const long long no = __ldg(&lk->nnz_off);
-        if (no >= 0) nnz = min(nnz, p.nnz[pi.src][no + pi.s]);
+        const int nnz = bucket_nnz(p, __ldg(&lk->hotness), __ldg(&lk->nnz_off), pi.src, pi.s);
         sc = 1.f / static_cast<float>(max(nnz, 1));
       }
       ix.bucket_scale[pos] = sc;
@@ -387,6 +361,47 @@ __global__ void __launch_bounds__(kIdxThreads)
 template <typename GradT>
 HCTR_DEVICE const GradT* locate_grad(const EmbParams& p, unsigned int e) {
   return reinterpret_cast<const GradT*>(p.grad[e >> 28]) + (static_cast<long long>(e & 0x0FFFFFFFu) << 2);
+}
+
+// The gather of the update kernels: gather_add issues the gradient loads of N bucket-list entries at one
+// column, then adds the scaled rows to acc in index order (kNoEntry: an absent entry, adds zero).  Every
+// caller walks a row's entries in list order, which fixes the fp32 sum bit for bit.
+constexpr unsigned int kNoEntry = 0xFFFFFFFFu;
+template <typename GradT, int N>
+HCTR_DEVICE void gather_add(float4& acc, const EmbParams& p, const unsigned int (&ent)[N],
+                            const float (&sc)[N], int col) {
+  float4 g[N];
+#pragma unroll
+  for (int u = 0; u < N; ++u)
+    g[u] = ent[u] != kNoEntry ? load_vec4<GradT>(locate_grad<GradT>(p, ent[u]) + col)
+                              : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int u = 0; u < N; ++u) {
+    acc.x += g[u].x * sc[u]; acc.y += g[u].y * sc[u];
+    acc.z += g[u].z * sc[u]; acc.w += g[u].w * sc[u];
+  }
+}
+// Sum at one column of the list entries first, first + stride, ... below `end`, N in flight per round
+// (the scale of an entry is 1 when the index has none)
+template <typename GradT, int N>
+HCTR_DEVICE float4 gather_list(const EmbParams& p, const BwdIndex& ix, bool has_scale, unsigned int first,
+                               unsigned int stride, unsigned int end, int col) {
+  float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (unsigned int j = first; j < end; j += N * stride) {
+    unsigned int ent[N];
+    float sc[N];
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      ent[u] = kNoEntry;
+      sc[u] = 1.f;
+      if (u * stride < end - j) {
+        ent[u] = ix.bucket_list[j + u * stride];
+        if (has_scale) sc[u] = ix.bucket_scale[j + u * stride];
+      }
+    }
+    gather_add<GradT, N>(acc, p, ent, sc, col);
+  }
+  return acc;
 }
 
 // Unique rows are classified by their number of occurrences right after the offsets are known (during
@@ -443,12 +458,7 @@ __global__ void __launch_bounds__(1024)
     }
     __syncthreads();
     if (warp < 2) {   // warp 0 scans the light counts, warp 1 the medium counts
-      unsigned int v = s_cnt[warp][lane], x = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const unsigned int y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-      }
+      const unsigned int v = s_cnt[warp][lane], x = warp_inclusive_scan(v, lane);
       s_cnt[warp][lane] = x - v;
       if (lane == 31) s_base[warp] = x ? atomicAdd(&ix.class_count[warp], x) : 0u;
     }
@@ -480,13 +490,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
                                  StateT* __restrict__ s0, StateT* __restrict__ s1, const OptHyper hp,
                                  const float grad_scale) {
   constexpr bool kHasS0 = (OPT != OPT_SGD);
-  const float lr = (hp.lr_ptr ? *hp.lr_ptr : 1.f) * hp.lr_scale;
-  float bc1 = 1.f, bc2 = 1.f;
-  if constexpr (OPT == OPT_ADAM) {
-    const float t = static_cast<float>(hp.step_ptr ? *hp.step_ptr : 1u);
-    bc1 = 1.f - powf(hp.beta1, t);
-    bc2 = 1.f - powf(hp.beta2, t);
-  }
+  const OptStep step = opt_step<OPT>(hp);
   const float inv_scaler = grad_scale / hp.scaler;
   const unsigned long long srk = sr_key<WT>(hp.sr_seed, hp.step_ptr);
   const int lane = threadIdx.x & 31;
@@ -516,7 +520,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       row[ka] = 0ull;
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
-        ent[ka][u] = 0xFFFFFFFFu;
+        ent[ka][u] = kNoEntry;
         esc[ka][u] = 1.f;
       }
       if (i < n_light) {
@@ -562,30 +566,12 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
           const int col = (c * G + gl) * 4;
           acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
           if (col < ev) {
-            float4 g[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u)
-              g[u] = ent[0][u] != 0xFFFFFFFFu ? load_vec4<GradT>(locate_grad<GradT>(p, ent[0][u]) + col)
-                                              : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              acc[c].x += g[u].x * esc[0][u]; acc[c].y += g[u].y * esc[0][u];
-              acc[c].z += g[u].z * esc[0][u]; acc[c].w += g[u].w * esc[0][u];
-            }
-            acc[c] = make_float4(acc[c].x * inv_scaler, acc[c].y * inv_scaler, acc[c].z * inv_scaler,
-                                 acc[c].w * inv_scaler);
+            gather_add<GradT, 4>(acc[c], p, ent[0], esc[0], col);
+            acc[c] = scale4(acc[c], inv_scaler);
             sq += sumsq4(acc[c]);
           }
         }
-#pragma unroll
-        for (int o = G / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(gmask, sq, o);
-        float f = 0.f;
-        if (gl == 0) {
-          const float s_new = rowwise_accumulate(s_old, sq, ev);
-          s0[row[0]] = s_new;
-          f = rowwise_factor(s_new, hp, lr);
-        }
-        f = __shfl_sync(gmask, f, gi * G);
+        const float f = rowwise_row_step<G>(gmask, gi * G, lane, sq, s_old, s0 + row[0], ev, hp, step.lr);
 #pragma unroll
         for (int c = 0; c < NC; ++c) {
           const int col = (c * G + gl) * 4;
@@ -598,56 +584,39 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
           }
         }
       } else {
-      // the row in passes of at most 4 chunks: weights, state and sums of one pass stay within the
-      // 128 registers of two resident blocks per SM for G == 32 (8 chunks per lane)
+        // the row in passes of at most 4 chunks: weights, state and sums of one pass stay within the
+        // 128 registers of two resident blocks per SM for G == 32 (8 chunks per lane)
 #pragma unroll
-      for (int c0 = 0; c0 < NC; c0 += 4) {
-      typename Row4<WT>::type wv[4];
-      float4 sv[4], acc[4];
+        for (int c0 = 0; c0 < NC; c0 += 4) {
+          typename Row4<WT>::type wv[4];
+          float4 sv[4], acc[4];
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int col = ((c0 + c) * G + gl) * 4;
-        wv[c] = {};
-        sv[c] = acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (col < ev) {
-          wv[c] = load_row4<WT>(static_cast<const WT*>(p.table) + base + col);
-          if constexpr (kHasS0) sv[c] = load_vec4<StateT>(s0 + base + col);
-        }
-      }
+          for (int c = 0; c < 4; ++c) {
+            const int col = ((c0 + c) * G + gl) * 4;
+            wv[c] = {};
+            sv[c] = acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (col < ev) {
+              wv[c] = load_row4<WT>(static_cast<const WT*>(p.table) + base + col);
+              if constexpr (kHasS0) sv[c] = load_vec4<StateT>(s0 + base + col);
+            }
+          }
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int col = ((c0 + c) * G + gl) * 4;
-        if (col < ev) {
-          float4 g[4];
+          for (int c = 0; c < 4; ++c) {
+            const int col = ((c0 + c) * G + gl) * 4;
+            if (col < ev) gather_add<GradT, 4>(acc[c], p, ent[0], esc[0], col);
+          }
 #pragma unroll
-          for (int u = 0; u < 4; ++u)
-            g[u] = ent[0][u] != 0xFFFFFFFFu ? load_vec4<GradT>(locate_grad<GradT>(p, ent[0][u]) + col)
-                                            : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            acc[c].x += g[u].x * esc[0][u]; acc[c].y += g[u].y * esc[0][u];
-            acc[c].z += g[u].z * esc[0][u]; acc[c].w += g[u].w * esc[0][u];
+          for (int c = 0; c < 4; ++c) {
+            const int col = ((c0 + c) * G + gl) * 4;
+            if (col < ev) {
+              float4 w = widen4(wv[c]);
+              apply_opt4_pre<OPT, StateT>(w, scale4(acc[c], inv_scaler), sv[c], s0, s1, base + col, hp, step);
+              store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
+            }
           }
         }
       }
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        const int col = ((c0 + c) * G + gl) * 4;
-        if (col < ev) {
-          float4 w = widen4(wv[c]);
-          apply_opt4_pre<OPT, StateT>(w, make_float4(acc[c].x * inv_scaler, acc[c].y * inv_scaler,
-                                                     acc[c].z * inv_scaler, acc[c].w * inv_scaler),
-                                      sv[c], s0, s1, base + col, hp, lr, bc1, bc2);
-          store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
-        }
-      }
-      }
-      }
-      if (gl == 0) {
-        const unsigned int slot = ut.slots[uid];
-        ut.keys[slot] = kEmptyKey;
-        ut.vals[slot] = kInvalidVal;
-      }
+      if (gl == 0) unique_release(ut, uid);
       rec[0] = rec[1];
       rec[1] = rec[2];
       row[0] = row[1];
@@ -678,38 +647,11 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
         const int col = lane * 4 + c * 128;
         acc[c] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (col < ev) {
-          for (unsigned int j = o0; j < o1; j += 8) {
-            float4 g[8];
-            float sc[8];
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              g[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-              sc[u] = 0.f;
-              if (j + u < o1) {
-                g[u] = load_vec4<GradT>(locate_grad<GradT>(p, ix.bucket_list[j + u]) + col);
-                sc[u] = has_scale ? ix.bucket_scale[j + u] : 1.f;
-              }
-            }
-#pragma unroll
-            for (int u = 0; u < 8; ++u) {
-              acc[c].x += g[u].x * sc[u]; acc[c].y += g[u].y * sc[u];
-              acc[c].z += g[u].z * sc[u]; acc[c].w += g[u].w * sc[u];
-            }
-          }
-          acc[c] = make_float4(acc[c].x * inv_scaler, acc[c].y * inv_scaler, acc[c].z * inv_scaler,
-                               acc[c].w * inv_scaler);
+          acc[c] = scale4(gather_list<GradT, 8>(p, ix, has_scale, o0, 1u, o1, col), inv_scaler);
           sq += sumsq4(acc[c]);
         }
       }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
-      float f = 0.f;
-      if (lane == 0) {
-        const float s_new = rowwise_accumulate(s_old, sq, ev);
-        s0[arow] = s_new;
-        f = rowwise_factor(s_new, hp, lr);
-      }
-      f = __shfl_sync(0xffffffffu, f, 0);
+      const float f = rowwise_row_step<32>(0xffffffffu, 0, lane, sq, s_old, s0 + arow, ev, hp, step.lr);
 #pragma unroll
       for (int c = 0; c < kIters; ++c) {
         const int col = lane * 4 + c * 128;
@@ -724,35 +666,11 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       float4 w = load_vec4<WT>(static_cast<const WT*>(p.table) + base + col);
       float4 sv = make_float4(0.f, 0.f, 0.f, 0.f);
       if constexpr (kHasS0) sv = load_vec4<StateT>(s0 + base + col);
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (unsigned int j = o0; j < o1; j += 8) {
-        float4 g[8];
-        float sc[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          g[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-          sc[u] = 0.f;
-          if (j + u < o1) {
-            g[u] = load_vec4<GradT>(locate_grad<GradT>(p, ix.bucket_list[j + u]) + col);
-            sc[u] = has_scale ? ix.bucket_scale[j + u] : 1.f;
-          }
-        }
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          acc.x += g[u].x * sc[u]; acc.y += g[u].y * sc[u];
-          acc.z += g[u].z * sc[u]; acc.w += g[u].w * sc[u];
-        }
-      }
-      apply_opt4_pre<OPT, StateT>(w, make_float4(acc.x * inv_scaler, acc.y * inv_scaler,
-                                                 acc.z * inv_scaler, acc.w * inv_scaler),
-                                  sv, s0, s1, base + col, hp, lr, bc1, bc2);
+      const float4 acc = gather_list<GradT, 8>(p, ix, has_scale, o0, 1u, o1, col);
+      apply_opt4_pre<OPT, StateT>(w, scale4(acc, inv_scaler), sv, s0, s1, base + col, hp, step);
       store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
     }
-    if (lane == 0) {
-      const unsigned int slot = ut.slots[uid];
-      ut.keys[slot] = kEmptyKey;
-      ut.vals[slot] = kInvalidVal;
-    }
+    if (lane == 0) unique_release(ut, uid);
   }
 }
 
@@ -767,14 +685,9 @@ __global__ void __launch_bounds__(256)
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   extern __shared__ float sm[];  // [8 warps][ev]
   __shared__ unsigned int last_s;
-  const float lr = (hp.lr_ptr ? *hp.lr_ptr : 1.f) * hp.lr_scale;
-  float bc1 = 1.f, bc2 = 1.f;
-  if constexpr (OPT == OPT_ADAM) {
-    const float t = static_cast<float>(hp.step_ptr ? *hp.step_ptr : 1u);
-    bc1 = 1.f - powf(hp.beta1, t);
-    bc2 = 1.f - powf(hp.beta2, t);
-  }
+  const OptStep step = opt_step<OPT>(hp);
   const float inv_scaler = grad_scale / hp.scaler;
+  const bool has_scale = ix.bucket_scale != nullptr;
   for (unsigned int it = blockIdx.x; it < nitems; it += gridDim.x) {
     const unsigned int uid = ix.heavy_items[2 * it];
     if (uid == kInvalidVal) continue;   // reserved by a row that fell back to the medium list
@@ -786,30 +699,10 @@ __global__ void __launch_bounds__(256)
     float* scratch = ix.heavy_scratch + static_cast<long long>(slot) * ev;
     for (int col0 = 0; col0 < ev; col0 += 128) {
       const int col = col0 + lane * 4;
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (col < ev) {
-        unsigned int j = o0 + warp;
-        for (; j + 24 < o1; j += 32) {
-          float sc[4];
-          float4 g[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            g[u] = load_vec4<GradT>(locate_grad<GradT>(p, ix.bucket_list[j + 8 * u]) + col);
-            sc[u] = ix.bucket_scale ? ix.bucket_scale[j + 8 * u] : 1.f;
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            acc.x += g[u].x * sc[u]; acc.y += g[u].y * sc[u];
-            acc.z += g[u].z * sc[u]; acc.w += g[u].w * sc[u];
-          }
-        }
-        for (; j < o1; j += 8) {
-          const float sc = ix.bucket_scale ? ix.bucket_scale[j] : 1.f;
-          const float4 g = load_vec4<GradT>(locate_grad<GradT>(p, ix.bucket_list[j]) + col);
-          acc.x += g.x * sc; acc.y += g.y * sc; acc.z += g.z * sc; acc.w += g.w * sc;
-        }
-        *reinterpret_cast<float4*>(sm + warp * ev + col) = acc;
-      }
+      // warp w sums the chunk's entries w, w + 8, ..., four in flight per round
+      if (col < ev)
+        *reinterpret_cast<float4*>(sm + warp * ev + col) =
+            gather_list<GradT, 4>(p, ix, has_scale, o0 + warp, 8u, o1, col);
     }
     __syncthreads();
     for (int c = threadIdx.x; c < ev; c += blockDim.x) {
@@ -845,9 +738,7 @@ __global__ void __launch_bounds__(256)
           float t = 0.f;
 #pragma unroll
           for (int w = 0; w < 8; ++w) t += sq_s[w];
-          const float s_new = rowwise_accumulate(s0[row], t, ev);
-          s0[row] = s_new;
-          f_s = rowwise_factor(s_new, hp, lr);
+          f_s = rowwise_state_step(s0[row], t, s0 + row, ev, hp, step.lr);
         }
         __syncthreads();
         const float f = f_s;
@@ -863,14 +754,12 @@ __global__ void __launch_bounds__(256)
         const float g = __ldcg(scratch + c);
         scratch[c] = 0.f;
         float w = to_f<WT>(static_cast<const WT*>(p.table)[base + c]);
-        apply_opt<OPT, StateT>(w, g * inv_scaler, s0, s1, base + c, hp, lr, bc1, bc2);
+        apply_opt<OPT, StateT>(w, g * inv_scaler, s0, s1, base + c, hp, step);
         store_w<WT>(static_cast<WT*>(p.table) + base + c, w, srk, base + c);
       }
       if (threadIdx.x == 0) {
         ix.heavy_ticket[slot] = 0;
-        const unsigned int hs = ut.slots[uid];
-        ut.keys[hs] = kEmptyKey;
-        ut.vals[hs] = kInvalidVal;
+        unique_release(ut, uid);
       }
     }
     __syncthreads();
@@ -899,10 +788,9 @@ extern "C" int hctr_emb_bwd_index(const EmbParams* p, const UniqueTable* ut, con
   if (p->num_lookups > kMaxSmemLookups) return -5;
   if (ix->max_heavy_rows > (1u << 20)) return -6;   // 20-bit scratch slot field of a heavy item
   const unsigned int blocks = static_cast<unsigned int>((total_pairs + kPairsPerBlock - 1) / kPairsPerBlock);
-  if (key_bytes == 8)
-    emb_bwd_index_kernel<long long><<<blocks, kIdxThreads, 0, st>>>(*p, *ut, *ix, total_pairs);
-  else
-    emb_bwd_index_kernel<int><<<blocks, kIdxThreads, 0, st>>>(*p, *ut, *ix, total_pairs);
+  with_key(key_bytes, [&](auto k) {
+    emb_bwd_index_kernel<type_of<decltype(k)>><<<blocks, kIdxThreads, 0, st>>>(*p, *ut, *ix, total_pairs);
+  });
   const unsigned int nb = (ut->max_unique + 1023) / 1024;
   scan_block_sums_kernel<<<nb, 1024, 0, st>>>(ix->count, ix->block_sums, ut->counter, ut->max_unique);
   scan_sums_kernel<<<1, 1024, 0, st>>>(ix->block_sums, ut->counter, ut->max_unique, ix->heavy_count,
@@ -948,28 +836,18 @@ static void launch_reduce(const EmbParams* p, const UniqueTable* ut, const BwdIn
     cudaEventRecord(g_heavy_side.fork, st);
     cudaStreamWaitEvent(hs, g_heavy_side.fork, 0);
   }
-  if (grad_bf16)
-    emb_bwd_heavy_kernel<OPT, StateT, __nv_bfloat16, WT><<<num_sms * 4, 256, smem, hs>>>(
+  with_elem(grad_bf16, [&](auto g) {
+    using GradT = type_of<decltype(g)>;
+    emb_bwd_heavy_kernel<OPT, StateT, GradT, WT><<<num_sms * 4, 256, smem, hs>>>(
         *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
-  else
-    emb_bwd_heavy_kernel<OPT, StateT, float, WT><<<num_sms * 4, 256, smem, hs>>>(
-        *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
-  if (fork) cudaEventRecord(g_heavy_side.join, hs);
-  if (grad_bf16) {
-    if (g8)
-      emb_bwd_reduce_update_kernel<OPT, StateT, __nv_bfloat16, 8, WT><<<blocks, 256, 0, st>>>(
+    if (fork) cudaEventRecord(g_heavy_side.join, hs);
+    auto light = [&](auto lanes) {
+      emb_bwd_reduce_update_kernel<OPT, StateT, GradT, decltype(lanes)::value, WT><<<blocks, 256, 0, st>>>(
           *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
-    else
-      emb_bwd_reduce_update_kernel<OPT, StateT, __nv_bfloat16, 32, WT><<<blocks, 256, 0, st>>>(
-          *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
-  } else {
-    if (g8)
-      emb_bwd_reduce_update_kernel<OPT, StateT, float, 8, WT><<<blocks, 256, 0, st>>>(
-          *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
-    else
-      emb_bwd_reduce_update_kernel<OPT, StateT, float, 32, WT><<<blocks, 256, 0, st>>>(
-          *p, *ut, *ix, (StateT*)s0, (StateT*)s1, *hp, grad_scale);
-  }
+    };
+    if (g8) light(Int<8>{});
+    else light(Int<32>{});
+  });
   if (fork) cudaStreamWaitEvent(st, g_heavy_side.join, 0);
 }
 
@@ -982,7 +860,7 @@ extern "C" int hctr_emb_bwd_reduce_update(const EmbParams* p, const UniqueTable*
   if (p->ev_size % 4) return -3;
   if (p->ev_size > kMaxEmbWidth) return -4;
   const int rc = dispatch_opt(opt, state_bf16, table_bf16, [&](auto o, auto s, auto w) {
-    launch_reduce<decltype(o)::value, typename decltype(s)::type, typename decltype(w)::type>(
+    launch_reduce<decltype(o)::value, type_of<decltype(s)>, type_of<decltype(w)>>(
         p, ut, ix, s0, s1, hp, grad_scale, grad_bf16, num_sms, st);
   });
   if (rc) return rc;

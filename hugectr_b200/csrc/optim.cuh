@@ -61,9 +61,26 @@ struct OptHyper {
   unsigned int pad_;
 };
 
+// Scalars every element of one optimizer step shares: the learning rate and Adam's bias corrections
+// (1 elsewhere).  A null lr_ptr / step_ptr reads as learning rate 1 / step 1.
+struct OptStep {
+  float lr, bc1, bc2;
+};
+template <int OPT>
+HCTR_DEVICE OptStep opt_step(const OptHyper& hp) {
+  OptStep st = {(hp.lr_ptr ? *hp.lr_ptr : 1.f) * hp.lr_scale, 1.f, 1.f};
+  if constexpr (OPT == OPT_ADAM) {
+    const float t = static_cast<float>(hp.step_ptr ? *hp.step_ptr : 1u);
+    st.bc1 = 1.f - powf(hp.beta1, t);
+    st.bc2 = 1.f - powf(hp.beta2, t);
+  }
+  return st;
+}
+
 template <int OPT, typename StateT>
 HCTR_DEVICE void apply_opt(float& w, float g, StateT* s0, StateT* s1, long long idx,
-                           const OptHyper& hp, float lr, float bc1, float bc2) {
+                           const OptHyper& hp, const OptStep& st) {
+  const float lr = st.lr;
   if constexpr (OPT == OPT_SGD) {
     w -= lr * g;
   } else if constexpr (OPT == OPT_ADAGRAD) {
@@ -75,7 +92,7 @@ HCTR_DEVICE void apply_opt(float& w, float g, StateT* s0, StateT* s1, long long 
     float v = hp.beta2 * to_f<StateT>(s1[idx]) + (1.f - hp.beta2) * g * g;
     s0[idx] = from_f<StateT>(m);
     s1[idx] = from_f<StateT>(v);
-    const float alpha = lr * sqrtf(bc2) / bc1;
+    const float alpha = lr * sqrtf(st.bc2) / st.bc1;
     w -= alpha * m / (sqrtf(v) + hp.epsilon);
   } else if constexpr (OPT == OPT_FTRL) {
     // state0 = z, state1 = n (reference ftrl_optimizer.cu:28-42)
@@ -104,12 +121,11 @@ HCTR_DEVICE void apply_opt(float& w, float g, StateT* s0, StateT* s1, long long 
   }
 }
 
-
 // 4-wide variant: optimizer state is loaded / stored as one vector (16 B fp32, 8 B bf16) instead of
 // four scalar accesses per lane.
 template <int OPT, typename StateT>
 HCTR_DEVICE void apply_opt4(float4& w, const float4 g, StateT* s0, StateT* s1, long long idx,
-                            const OptHyper& hp, float lr, float bc1, float bc2) {
+                            const OptHyper& hp, const OptStep& st) {
   constexpr bool kHasS0 = (OPT != OPT_SGD);
   constexpr bool kHasS1 = (OPT == OPT_ADAM || OPT == OPT_FTRL);
   float a[4] = {0.f, 0.f, 0.f, 0.f}, b[4] = {0.f, 0.f, 0.f, 0.f};
@@ -127,7 +143,7 @@ HCTR_DEVICE void apply_opt4(float4& w, const float4 g, StateT* s0, StateT* s1, l
   for (int j = 0; j < 4; ++j) {
     // run the scalar rule on local copies of the state
     float sa = a[j], sb = b[j];
-    apply_opt<OPT, float>(ww[j], gg[j], &sa, &sb, 0, hp, lr, bc1, bc2);
+    apply_opt<OPT, float>(ww[j], gg[j], &sa, &sb, 0, hp, st);
     a[j] = sa; b[j] = sb;
   }
   w = make_float4(ww[0], ww[1], ww[2], ww[3]);
@@ -139,7 +155,7 @@ HCTR_DEVICE void apply_opt4(float4& w, const float4 g, StateT* s0, StateT* s1, l
 // their latency overlaps the gradient gather); the caller stores w, this stores the states.
 template <int OPT, typename StateT>
 HCTR_DEVICE void apply_opt4_pre(float4& w, const float4 g, const float4 s0v, StateT* s0, StateT* s1,
-                                long long idx, const OptHyper& hp, float lr, float bc1, float bc2) {
+                                long long idx, const OptHyper& hp, const OptStep& st) {
   constexpr bool kHasS0 = (OPT != OPT_SGD);
   constexpr bool kHasS1 = (OPT == OPT_ADAM || OPT == OPT_FTRL);
   float a[4] = {s0v.x, s0v.y, s0v.z, s0v.w}, b[4] = {0.f, 0.f, 0.f, 0.f};
@@ -152,7 +168,7 @@ HCTR_DEVICE void apply_opt4_pre(float4& w, const float4 g, const float4 s0v, Sta
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     float sa = a[j], sb = b[j];
-    apply_opt<OPT, float>(ww[j], gg[j], &sa, &sb, 0, hp, lr, bc1, bc2);
+    apply_opt<OPT, float>(ww[j], gg[j], &sa, &sb, 0, hp, st);
     a[j] = sa; b[j] = sb;
   }
   w = make_float4(ww[0], ww[1], ww[2], ww[3]);
@@ -162,9 +178,9 @@ HCTR_DEVICE void apply_opt4_pre(float4& w, const float4 g, const float4 s0v, Sta
 
 // Row-wise AdaGrad (OPT_ROWWISE_ADAGRAD): ONE fp32 accumulator per row, s[row] (never bf16).
 //   s += (1/ev) * sum_c g[c]^2 ;  w[c] -= lr * g[c] / (sqrt(s) + eps)  for every column of the row
-// The caller reduces sum_c g[c]^2 over the whole row first (its lanes / warps / block), then calls
-// rowwise_factor once per row, and applies the returned factor f = lr / (sqrt(s) + eps) to every
-// column.  Square root and divisions round to nearest even whatever the fast-math flags, so a row
+// The caller reduces sum_c g[c]^2 over the whole row first (rowwise_row_step over the row's lanes, or
+// its own block reduction followed by rowwise_state_step), and applies the returned factor
+// f = lr / (sqrt(s) + eps) to every column.  Square root and divisions round to nearest even whatever the fast-math flags, so a row
 // whose update is exact in fp32 is reproduced bit for bit by the CPU path (ops/optim.py).
 HCTR_DEVICE float rowwise_accumulate(float s, float sumsq, int ev) {
   return s + __fdiv_rn(sumsq, static_cast<float>(ev));
@@ -172,9 +188,28 @@ HCTR_DEVICE float rowwise_accumulate(float s, float sumsq, int ev) {
 HCTR_DEVICE float rowwise_factor(float s_new, const OptHyper& hp, float lr) {
   return __fdiv_rn(lr, __fsqrt_rn(s_new) + hp.epsilon);
 }
+// one thread per row: *s = s_old + sumsq / ev, returns the row's factor
+HCTR_DEVICE float rowwise_state_step(float s_old, float sumsq, float* s, int ev, const OptHyper& hp, float lr) {
+  const float s_new = rowwise_accumulate(s_old, sumsq, ev);
+  *s = s_new;
+  return rowwise_factor(s_new, hp, lr);
+}
+// The WIDTH lanes of `mask` (a power of two, aligned) own one row and hold partial sums of g^2 in sq;
+// lane `leader`, the first of them, has s_old = *s (loaded early by the caller) and updates *s.  Every
+// lane returns the row's factor.
+template <int WIDTH>
+HCTR_DEVICE float rowwise_row_step(unsigned int mask, int leader, int lane, float sq, float s_old, float* s,
+                                   int ev, const OptHyper& hp, float lr) {
+#pragma unroll
+  for (int o = WIDTH / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(mask, sq, o);
+  float f = 0.f;
+  if (lane == leader) f = rowwise_state_step(s_old, sq, s, ev, hp, lr);
+  return __shfl_sync(mask, f, leader);
+}
 HCTR_DEVICE void apply_rowwise4(float4& w, const float4 g, float f) {
   w.x -= f * g.x; w.y -= f * g.y; w.z -= f * g.z; w.w -= f * g.w;
 }
 HCTR_DEVICE float sumsq4(const float4 g) { return g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w; }
+HCTR_DEVICE float4 scale4(const float4 g, float a) { return make_float4(g.x * a, g.y * a, g.z * a, g.w * a); }
 
 }  // namespace hctr

@@ -4,6 +4,7 @@ bwd_reduce_update) at DLRM-DCNv2 shapes, per optimizer, optimizer-state dtype an
 
   python tools_dev/bench_emb_update.py [--opts adagrad,rowwise_adagrad] [--ev 128] [--iters 20] [--rounds 5]
                                        [--max-rows N] [--tree DIR]
+  python tools_dev/bench_emb_update.py --check-bits TREE [--keys uniform] [--opts all] [--ev 128] [--steps 3]
   python tools_dev/bench_emb_update.py --full-model [--steps 20] [--warmup 3]
 
 Kernel mode: one arena of the 26 Criteo-TB tables, ev 128 by default (the DLRM-DCNv2 width, which runs the
@@ -19,6 +20,16 @@ and per arm, with the median over rounds and the nominal bytes computed from the
 
 --tree DIR imports hugectr_b200 from another checkout (built in place), so that two builds can be timed
 alternately, one process per run, in one session.
+
+--check-bits TREE times nothing: it runs --steps seeded fused-backward steps of every selected arm, each from
+the same initial weights and zero state, under this tree, under TREE and under TREE a second time (one process
+each), and compares 64-bit checksums of the arena and of both state arrays (computed on the device, position
+weighted).  Rows are capped at 500 k unless --max-rows says otherwise.  The gradients are multiples of 2^-12, so
+every row's fp32 sum is exact and the result does not depend on the order in which the counting sort lists a row's
+buckets or the heavy rows' atomics land: every arm must agree bit for bit, and TREE against TREE is the control
+(an arm that differs there is reported and not counted).  --keys uniform draws uniform keys and keeps only the
+tables whose rows then occur 16 times on average at most (and stops if a row has more than 64 occurrences), so
+that only the light- and medium-row code runs; the default power-law keys add the heavy rows.
 
 Full-model mode: build_dlrm_dcnv2(num_gpus=1, batchsize=6912, embedding_optimizer="rowwise_adagrad",
 weight_dtype="bf16") with the full table sizes, CUDA-graph training steps timed with CUDA events; prints
@@ -62,6 +73,16 @@ def parse_opts(s):
     return opts
 
 
+def checksum(t):
+    """Position-weighted 64-bit sum of a tensor's 32-bit words (wraps), computed on the device in chunks."""
+    w = t.view(torch.int32) if t.element_size() == 4 else t.view(torch.int16)
+    tot = torch.zeros((), dtype=torch.int64, device=t.device)
+    for o in range(0, w.numel(), 1 << 26):
+        c = w[o:o + (1 << 26)].to(torch.int64)
+        tot += (c * (torch.arange(o, o + c.numel(), device=t.device) * 2 + 1)).sum()
+    return format(int(tot.item()) & 0xFFFFFFFFFFFFFFFF, "016x")
+
+
 def kernels(a, name, plim):
     from hugectr_b200.data.batch import power_law_keys
     from hugectr_b200.embedding import ops as E
@@ -72,9 +93,12 @@ def kernels(a, name, plim):
              "rmsprop": Optimizer_t.RMSProp, "rowwise_adagrad": Optimizer_t.RowWiseAdaGrad}
     dev = torch.device("cuda")
     EV = a.ev
-    max_rows = a.max_rows or 4_000_000 * 128 // EV
+    max_rows = a.max_rows or (500_000 if a.digests else 4_000_000 * 128 // EV)
     rows = [min(s, max_rows) for s in CRITEO_TB_TABLE_SIZES]
     hot = list(CRITEO_TB_MULTI_HOT)
+    if a.keys == "uniform":      # no heavy rows: tables whose rows occur 16 times on average at most
+        keep = [i for i in range(len(rows)) if BATCH * hot[i] <= 16 * rows[i]]
+        rows, hot = [rows[i] for i in keep], [hot[i] for i in keep]
     n = len(rows)
     gen = torch.Generator().manual_seed(0)
     lookups, roff, koff, keys = [], 0, 0, []
@@ -83,7 +107,13 @@ def kernels(a, name, plim):
         lookups.append(E.LookupDesc(table_row_off=roff, key_off=koff, out_off=i * EV, grad_off=i * EV,
                                     hotness=hot[i], key_stride=hot[i], num_shards=1, shard_idx=0,
                                     out_stride=width, grad_stride=width, combiner=0, ev_size=EV, rows=rows[i]))
-        keys.append(power_law_keys(BATCH * hot[i], rows[i], 1.1, gen, torch.int32))
+        if a.keys == "uniform":
+            keys.append(torch.randint(0, rows[i], (BATCH * hot[i],), generator=gen, dtype=torch.int32))
+            most = int(torch.unique(keys[-1], return_counts=True)[1].max())
+            if most > 64:
+                raise SystemExit(f"bench_emb_update: a row of table {i} occurs {most} times: it would be heavy")
+        else:
+            keys.append(power_law_keys(BATCH * hot[i], rows[i], 1.1, gen, torch.int32))
         roff += rows[i]
         koff += BATCH * hot[i]
     po = 0
@@ -95,7 +125,11 @@ def kernels(a, name, plim):
     key_d = torch.cat(keys).to(dev)
     ld = E.lookups_to_device(lookups, dev)
     out = torch.zeros(BATCH * width, dtype=torch.bfloat16, device=dev)
-    grad = (torch.randn(BATCH * width, device=dev) * 1e-3).to(torch.bfloat16)
+    torch.manual_seed(0)
+    if a.digests:     # multiples of 2^-12: a row's sum is exact, whatever order the index lists its buckets in
+        grad = (torch.randint(-64, 65, (BATCH * width,), device=dev) / 4096).to(torch.bfloat16)
+    else:
+        grad = (torch.randn(BATCH * width, device=dev) * 1e-3).to(torch.bfloat16)
     w32 = torch.empty(total_rows * EV, device=dev).uniform_(-0.01, 0.01)
     tables = {"fp32": w32, "bf16": w32.to(torch.bfloat16)}
     opts = parse_opts(a.opts)
@@ -131,6 +165,24 @@ def kernels(a, name, plim):
         E.bwd_index(lookups, ld, tables[w], EV, [key_d], BATCH, ws)
         E.bwd_reduce_update(opt_t[o], lookups, ld, tables[w], s0, s1, EV, [key_d], [grad], BATCH, ws, hp,
                             lr_t, st_t)
+
+    if a.digests:       # every arm from the same weights and zero state; one JSON object on the last line
+        res = {}
+        for w in tables:
+            first = tables[w].clone()
+            for arm in arms:
+                tables[w].copy_(first)
+                for s in states(*arm):
+                    if s is not None:
+                        s.zero_()
+                for _ in range(a.steps):
+                    bwd(arm, w)
+                torch.cuda.synchronize()
+                res[f"{arm_name(*arm)}/{w}"] = {k: checksum(t) for k, t in
+                                                zip(("table", "s0", "s1"), [tables[w]] + states(*arm)) if t is not None}
+        E.check_workspace_overflow(ws, "benchmark")
+        print(json.dumps(res))
+        return 0
 
     def timed(fn, *args):
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -186,6 +238,30 @@ def kernels(a, name, plim):
     return 0
 
 
+def check_bits(a):
+    """Digests of every arm under this tree and (twice) under a.check_bits, one process each, compared."""
+    runs = []
+    for tree in (a.tree, a.check_bits, a.check_bits):
+        r = subprocess.run([sys.executable, os.path.abspath(__file__), "--tree", tree, "--digests", "--opts", a.opts,
+                            "--ev", str(a.ev), "--steps", str(a.steps), "--max-rows", str(a.max_rows),
+                            "--keys", a.keys], capture_output=True, text=True)
+        if r.returncode != 0:
+            print(r.stdout[-2000:] + r.stderr[-4000:], file=sys.stderr)
+            return 1
+        runs.append(json.loads(r.stdout.strip().splitlines()[-1]))
+    mine, other, again = runs
+    bad = 0
+    for arm in other:
+        same = {k: mine.get(arm, {}).get(k) == v for k, v in other[arm].items()}
+        stable = {k: again[arm][k] == v for k, v in other[arm].items()}
+        fail = any(stable[k] and not same[k] for k in same)
+        bad += fail
+        print(json.dumps({"arm": arm, "equal": same, "other_tree_equals_itself": stable, "fail": fail}), flush=True)
+    print(json.dumps({"check_bits": os.path.abspath(a.check_bits), "keys": a.keys, "ev": a.ev, "steps": a.steps,
+                      "arms": len(other), "failed": bad}), flush=True)
+    return 1 if bad or set(mine) != set(other) else 0
+
+
 def full_model(a, name, plim):
     from hugectr_b200.models.dlrm import CRITEO_TB_TABLE_SIZES, build_dlrm_dcnv2
     torch.cuda.set_device(0)
@@ -226,14 +302,23 @@ def main(argv):
     ap.add_argument("--max-rows", type=int, default=0)
     ap.add_argument("--tree", default=ROOT)
     ap.add_argument("--full-model", action="store_true")
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=0, help="full model: 20 training steps; --check-bits: 3 updates")
+    ap.add_argument("--check-bits", default="", metavar="TREE",
+                    help="compare the updated weights and states of every arm with TREE's, bit for bit")
+    ap.add_argument("--keys", default="power-law", choices=("power-law", "uniform"))
+    ap.add_argument("--digests", action="store_true", help=argparse.SUPPRESS)
     a = ap.parse_args(argv)
+    a.steps = a.steps or (3 if a.check_bits or a.digests else 20)
     parse_opts(a.opts)
+    if a.check_bits and not os.path.isdir(os.path.join(a.check_bits, "hugectr_b200")):
+        raise SystemExit(f"bench_emb_update: {a.check_bits} holds no hugectr_b200 package")
     if not os.path.isdir(os.path.join(a.tree, "hugectr_b200")):
         raise SystemExit(f"bench_emb_update: {a.tree} holds no hugectr_b200 package")
     if not torch.cuda.is_available():
         print("bench_emb_update: needs a CUDA device (an H100); nothing was measured", file=sys.stderr)
         return 1
+    if a.check_bits:
+        return check_bits(a)
     sys.path.insert(0, os.path.abspath(a.tree))
     name, plim = card()
     print(f"# device: {name}, power limit {plim}, tree {os.path.abspath(a.tree)}", flush=True)
