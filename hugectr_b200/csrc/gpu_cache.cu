@@ -9,6 +9,7 @@
 #include <stdint.h>
 
 #include "embedding.cuh"
+#include "set_assoc.cuh"
 
 namespace hctr {
 
@@ -27,12 +28,7 @@ HCTR_DEVICE int set_of(const CacheView& c, long long key) {
 
 // warp-cooperative find: returns slot index inside the set or -1 (uniform across the warp)
 HCTR_DEVICE int warp_find(const CacheView& c, int set, long long key, int lane) {
-  const long long* k = c.keys + static_cast<long long>(set) * c.ways;
-  for (int w = 0; w < c.ways; w += 32) {
-    const unsigned m = __ballot_sync(0xffffffffu, k[w + lane] == key);
-    if (m) return w + __ffs(m) - 1;
-  }
-  return -1;
+  return warp_find(c.keys + static_cast<long long>(set) * c.ways, c.ways, key, lane);
 }
 
 __global__ void __launch_bounds__(256)
@@ -57,21 +53,8 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-HCTR_DEVICE void lock_set(const CacheView& c, int set, int lane) {
-  if (lane == 0) {
-    while (atomicCAS(&c.locks[set], 0, 1) != 0) {
-    }
-    __threadfence();
-  }
-  __syncwarp();
-}
-HCTR_DEVICE void unlock_set(const CacheView& c, int set, int lane) {
-  __syncwarp();
-  if (lane == 0) {
-    __threadfence();
-    atomicExch(&c.locks[set], 0);
-  }
-}
+HCTR_DEVICE void lock_set(const CacheView& c, int set, int lane) { lock_set(c.locks, set, lane); }
+HCTR_DEVICE void unlock_set(const CacheView& c, int set, int lane) { unlock_set(c.locks, set, lane); }
 
 // insert-or-evict (LRU); already-present keys are refreshed with the new value
 __global__ void __launch_bounds__(256)

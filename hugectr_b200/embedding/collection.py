@@ -69,6 +69,18 @@ class EmbeddingTableConfig:
         if self.weight_dtype not in WEIGHT_DTYPES:
             raise ValueError(f"table {self.name}: weight_dtype must be one of {sorted(WEIGHT_DTYPES)}, "
                              f"not {self.weight_dtype!r}")
+        # "lru" | "lfu": a dynamic table of a fixed max_capacity rows per shard that evicts cold keys
+        # instead of growing (see docs/embedding.md); None keeps the growing table
+        self.evict_strategy = kw.get("evict_strategy", None)
+        if self.evict_strategy is not None:
+            from .hashtable import EVICT_STRATEGIES
+            if self.evict_strategy not in EVICT_STRATEGIES:
+                raise ValueError(f"table {self.name}: evict_strategy must be one of {EVICT_STRATEGIES} or None, "
+                                 f"not {self.evict_strategy!r}")
+            if not self.dynamic:
+                raise ValueError(f"table {self.name}: evict_strategy needs a dynamic table (max_vocabulary_size=-1)")
+            if self.max_capacity <= 0:
+                raise ValueError(f"table {self.name}: evict_strategy needs max_capacity > 0 (rows per shard)")
 
 
 class EmbeddingCollectionConfig:
@@ -228,6 +240,11 @@ class EmbeddingCollection:
         self.tables = cfg.tables()
         self.tmap = {t.name: t for t in self.tables}
         self.placement = resolve_placement(cfg, self.world)
+        for t in self.tables:
+            pl = self.placement[t.name]
+            if t.evict_strategy is not None and (pl.kind != "mp" or pl.col_factor > 1):
+                raise ValueError(f"table {t.name}: an evicting table is model parallel, table-wise or row-wise "
+                                 f"(placement {pl.kind!r}, column factor {pl.col_factor})")
         self.native = device.type == "cuda"
         self.has_dynamic = any(t.dynamic for t in self.tables)
         self.fused = (self.native and self.world > 1 and comm.p2p_available) if fused is None else fused
@@ -253,6 +270,9 @@ class EmbeddingCollection:
         self._unique_tables = self._resolve_unique_tables()
         self._kb = 8 if key_dtype == torch.int64 else 4
         self._abf = act_dtype == torch.bfloat16
+        # clock of the evicting tables: ticked once per training step inside the step (not Model.step_t,
+        # which a learning-rate scheduler reset zeroes and Adam's bias correction reads)
+        self.evict_clock = torch.zeros(1, dtype=torch.int64, device=device)
         self._build_layout(hotness)
         self._build_storage(seed)
         self._alloc_buffers()
@@ -342,8 +362,9 @@ class EmbeddingCollection:
                 # no owner-side lookup descriptors, no per-shard partial blocks
                 gl["unique"], gl["unique_owners"] = True, list(pl.shard_gpus)
                 continue
+            # (not for evicting tables: their owners translate the raw keys of the whole bag)
             if getattr(self, "shard_split", False) and pl.kind == "mp" and k > 1 and pl.col_factor == 1 \
-                    and gl["combiner"] == "sum":
+                    and gl["combiner"] == "sum" and self.tmap[gl["table"]].evict_strategy is None:
                 # Requester-side split: every rank rewrites its bag of a row-sharded table into k
                 # compacted per-shard lists of LOCAL ROW INDICES (key // k) plus their lengths, stored
                 # behind the user keys in the (symmetric) key slab.  A shard owner then reads only
@@ -407,10 +428,13 @@ class EmbeddingCollection:
                     # never shares an arena (and its first table's optimizer) with another optimizer
                     key += ("rowwise", float(o.epsilon), float(o.initial_accu_value))
                 grp = groups.setdefault(key, _Group(pl.kind, ev_part, wdt, rowwise))
-                rows = t.init_capacity if t.dynamic else shard_rows(t.max_vocabulary_size, k, s)
+                if t.evict_strategy is not None:
+                    rows = (t.max_capacity + 31) // 32 * 32       # whole 32-way sets, allocated once
+                else:
+                    rows = t.init_capacity if t.dynamic else shard_rows(t.max_vocabulary_size, k, s)
                 grp.table_slices.append({"table": t.name, "cpart": cpart, "row_off": grp.rows,
                                          "rows": rows, "k": k, "s": s, "col0": cpart * ev_part,
-                                         "ev": ev_part, "dynamic": t.dynamic})
+                                         "ev": ev_part, "dynamic": t.dynamic, "evict": t.evict_strategy})
                 grp.rows += rows
                 if grp.opt is None:
                     grp.opt = o
@@ -482,6 +506,9 @@ class EmbeddingCollection:
                 l.pair_off = po
                 po += R * self.b * l.hotness
             grp.lookups_dev = E.lookups_to_device(grp.lookups, dev)
+            for sl in grp.table_slices:
+                if sl["evict"]:
+                    self._dyn_hash(sl["table"], sl)
             pairs = po
             if self.is_train:
                 if grp.kind == "mp":
@@ -563,6 +590,15 @@ class EmbeddingCollection:
                     self.grads_all = torch.zeros(W, max(self.grad_slab_elems, 1), dtype=self.act_dtype,
                                                  device=dev)
                 self._build_packed_exchange()
+        # evicting tables: the ways admitted by one step (at most one per key position), re-initialised
+        # after the table's last insert
+        self._evict_adm = {}
+        if self.is_train:
+            for name, gls in self._evicting_lookups().items():
+                if self._evict_local(name) is not None:
+                    n = sum(W * b * gl["hotness"] for gl in gls)
+                    self._evict_adm[name] = (torch.zeros(n, dtype=torch.int64, device=dev),
+                                             torch.zeros(1, dtype=torch.int32, device=dev))
         uq = [gi for gi, gl in enumerate(self.glookups) if gl.get("unique")]
         self._uniq = None
         if uq:
@@ -779,9 +815,86 @@ class EmbeddingCollection:
             owner._dyn_tables = {}
         key = (name, sl["cpart"], sl["s"])
         if key not in owner._dyn_tables:
-            from .hashtable import HashTable
-            owner._dyn_tables[key] = HashTable(sl["rows"], self.device)
+            if sl.get("evict"):
+                from .hashtable import SetAssocTable
+                owner._dyn_tables[key] = SetAssocTable(sl["rows"], sl["evict"], owner.evict_clock, self.device)
+            else:
+                from .hashtable import HashTable
+                owner._dyn_tables[key] = HashTable(sl["rows"], self.device)
         return owner._dyn_tables[key]
+
+    def _evicting_lookups(self):
+        """{evicting table name: [its global lookups]}"""
+        res = {}
+        for gl in self.glookups:
+            if self.tmap[gl["table"]].evict_strategy is not None:
+                res.setdefault(gl["table"], []).append(gl)
+        return res
+
+    def _evict_local(self, name):
+        """(group, slice) of this rank's shard of evicting table ``name``, or None"""
+        for grp in self.groups:
+            for sl in grp.table_slices:
+                if sl["table"] == name:
+                    return grp, sl
+        return None
+
+    def _evict_reinit(self, grp, sl, ht, adm):
+        """fresh weights and initial optimizer state for the ways ``adm`` admitted"""
+        t = self.tmap[sl["table"]]
+        bound = math.sqrt(1.0 / max(t.init_capacity, 1))
+        if t.init_param is not None and t.init_param.up_bound > 0:
+            bound = t.init_param.up_bound
+        o = grp.opt
+        s0_init = o.initial_accu_value if (o is not None and o.optimizer_type in
+                                           (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad)) else 0.0
+        ht.reinit(adm, adm[0].numel(), grp.table, grp.s0, grp.s1, sl["row_off"], grp.pitch, grp.state_pitch,
+                  s0_init, bound, self.evict_init_key(t.name), sl["col0"])
+
+    def evict_init_key(self, name: str) -> int:
+        """key of the stateless initializer of table ``name``'s admitted rows (ops.evict_init_rows)"""
+        return E.evict_init_key(self.seed, _stable_seed("evict_init", name))
+
+    def _translate_evicting(self, buf):
+        """Evicting tables (see csrc/evict_table.cu): a training lookup ticks the clock, touches every key
+        region of a table, then inserts into every region (rows in place over the keys), then re-initialises
+        the admitted rows; an evaluation lookup only reads.  No host synchronisation."""
+        b = self.b
+        owner = getattr(self, "_shared", self)
+        if self.is_train:
+            owner.evict_clock.add_(1)
+        for name, gls in self._evicting_lookups().items():
+            regs = [(gl["key_off"], b * gl["hotness"]) for gl in gls]
+            loc = self._evict_local(name)
+            if loc is None:
+                for off, n in regs:
+                    buf[:, off:off + n].fill_(-1)
+                continue
+            grp, sl = loc
+            ht = self._dyn_hash(name, sl)
+            if not self.is_train:
+                for off, n in regs:
+                    ht.get(buf, off, n, sl["k"], sl["s"])
+                continue
+            for off, n in regs:
+                ht.touch(buf, off, n, sl["k"], sl["s"])
+            adm = self._evict_adm[name]
+            adm[1].zero_()
+            for off, n in regs:
+                ht.insert(buf, off, n, sl["k"], sl["s"], adm=adm)
+            self._evict_reinit(grp, sl, ht, adm)
+
+    def eviction_stats(self):
+        """{(table, shard): {live, admitted, evicted, dropped}} of the evicting tables held here: cumulative
+        device counters, read with one host synchronisation (call it outside the step)"""
+        from .hashtable import SetAssocTable
+        owner = getattr(self, "_shared", self)
+        items = [(k, ht) for k, ht in getattr(owner, "_dyn_tables", {}).items() if isinstance(ht, SetAssocTable)]
+        if not items:
+            return {}
+        vals = torch.stack([torch.cat([ht.live().view(1), ht.stats]) for _, ht in items]).cpu().tolist()
+        return {(name, s_): dict(zip(("live", "admitted", "evicted", "dropped"), (int(x) for x in v)))
+                for ((name, _, s_), _), v in zip(items, vals)}
 
     def _translate_dynamic_keys(self):
         """Dynamic tables: overwrite the (gathered) keys of their lookups with local row indices -- new
@@ -791,7 +904,7 @@ class EmbeddingCollection:
         buf = self.key_slab.view(1, -1) if self.world == 1 else self.keys_all
         for gl in self.glookups:
             t = self.tmap[gl["table"]]
-            if not t.dynamic:
+            if not t.dynamic or t.evict_strategy is not None:
                 continue
             region = buf[:, gl["key_off"]:gl["key_off"] + b * gl["hotness"]]
             keys = region.to(torch.int64)
@@ -808,13 +921,15 @@ class EmbeddingCollection:
                     rows = (ht.get_insert(k) if self.is_train else ht.get(k)).reshape(keys.shape)
                     out = torch.where(own & (rows >= 0), rows.to(torch.int64), out)
             region.copy_(out.to(region.dtype))
+        if any(t.evict_strategy is not None for t in self.tables):
+            self._translate_evicting(buf)
 
     def check_overflow(self):
         """Raise if a dynamic table ran out of rows (reads device flags: a host sync -- called by
         ``Model`` at display / evaluation / checkpoint time, never inside the captured step)."""
         owner = getattr(self, "_shared", self)
         for (name, cpart, s_), ht in getattr(owner, "_dyn_tables", {}).items():
-            if ht.overflowed():
+            if self.tmap[name].evict_strategy is None and ht.overflowed():
                 raise RuntimeError(f"dynamic embedding table {name}: more than init_capacity="
                                    f"{ht.max_rows} distinct keys on one shard (shard {s_})")
         for grp in self.groups:
@@ -831,7 +946,7 @@ class EmbeddingCollection:
         owner = getattr(self, "_shared", self)
         grown = []
         for (name, cpart, s_), ht in list(getattr(owner, "_dyn_tables", {}).items()):
-            if not ht.overflowed():
+            if self.tmap[name].evict_strategy is not None or not ht.overflowed():
                 continue
             old = ht.max_rows
             new = owner._grow_to(name, cpart, s_, int(old * factor) + 1)
@@ -1123,7 +1238,12 @@ class EmbeddingCollection:
             for sl in grp.table_slices:
                 if sl["table"] != name:
                     continue
-                if sl.get("dynamic"):
+                if sl.get("evict"):
+                    m = (keys % sl["k"] == sl["s"]) & (keys >= 0)
+                    if not bool(m.any()):
+                        continue
+                    rows = sl["row_off"] + self._evict_admit(grp, sl, keys[m])
+                elif sl.get("dynamic"):
                     m = (keys % sl["k"] == sl["s"]) & (keys >= 0)
                     if not bool(m.any()):
                         continue
@@ -1154,6 +1274,25 @@ class EmbeddingCollection:
                                 # (exact for a row-wise file, the natural conversion of an AdaGrad one)
                                 v = v.double().mean(1, keepdim=True).float()
                             dst.view(-1, grp.state_pitch)[rows] = v.to(dst.device, dst.dtype)
+
+    def _evict_admit(self, grp, sl, keys):
+        """(checkpoint load) local rows of ``keys`` in an evicting shard: present keys keep theirs, the
+        others take empty ways with the clock as stamp and a count of 1, and start from fresh weights and
+        state (overwritten by the caller).  Never evicts: raises when a key finds no free way."""
+        ht = self._dyn_hash(sl["table"], sl)
+        dev = self.device
+        kk = keys.to(dev, torch.int64).view(1, -1).clone()
+        n = kk.shape[1]
+        adm = (torch.zeros(n, dtype=torch.int64, device=dev), torch.zeros(1, dtype=torch.int32, device=dev))
+        ht.insert(kk, 0, n, adm=adm, evict=False, stats=torch.zeros(3, dtype=torch.int64, device=dev))
+        slots = kk.view(-1)
+        dropped = int((slots < 0).sum())
+        if dropped:
+            raise RuntimeError(f"evicting embedding table {sl['table']}: shard {sl['s']} cannot hold the loaded keys: "
+                               f"{dropped} of {n} found no free way (capacity {ht.capacity}, "
+                               f"{int(ht.live())} live keys)")
+        self._evict_reinit(grp, sl, ht, adm)
+        return slots.to(grp.table.device)
 
     def table_parts(self, name: str):
         """Metadata of the local shards of table ``name`` in ``dump_table_local`` order (no data is

@@ -2,6 +2,10 @@
 semantics).  GPU: csrc/hashtable.cu (open addressing, atomicCAS); CPU: python dict reference.
 Parity: HugeCTR/src/hashtable/nv_hashtable.cu:36-306 (get_insert / get(get_mark) / set / dump /
 get_size), capacity = max_vocabulary_size / 0.75 (nv_hashtable.hpp:179).
+
+SetAssocTable: the fixed-capacity, evicting key -> row map of a dynamic table with an
+``evict_strategy`` (LRU / LFU over 32-way sets).  GPU: csrc/evict_table.cu; CPU: the same rules
+in Python, the oracle of the tests.
 """
 from __future__ import annotations
 
@@ -26,6 +30,14 @@ def lib():
         l.hctr_ht_translate.argtypes = [vp, vp, vp, ull, ll, vp, vp, ll, i, vp, ll, i, i, i, i, vp]
         l.hctr_ht_translate.restype = i
         for n in ("hctr_ht_get_insert", "hctr_ht_set", "hctr_ht_dump"):
+            getattr(l, n).restype = i
+        l.hctr_evict_touch.argtypes = [vp, vp, vp]
+        l.hctr_evict_insert.argtypes = [vp, vp, vp, vp, i, vp]
+        l.hctr_evict_get.argtypes = [vp, vp, vp]
+        l.hctr_evict_dump.argtypes = [vp, ll, vp, vp, vp, vp]
+        l.hctr_evict_reinit.argtypes = [vp, ll, i, vp]
+        for n in ("hctr_evict_touch", "hctr_evict_insert", "hctr_evict_get", "hctr_evict_dump",
+                  "hctr_evict_reinit"):
             getattr(l, n).restype = i
         _lib = l
     return _lib
@@ -170,3 +182,224 @@ class HashTable:
         else:
             self.map = {}
             self._overflowed = False
+
+
+# ------------------------------------------------------------------------- evicting tables
+EVICT_STRATEGIES = ("lru", "lfu")
+WAYS = 32
+COUNT_MAX = (1 << 32) - 1
+
+
+class _EvictTableView(C.Structure):
+    _fields_ = [("keys", C.c_void_p), ("stamps", C.c_void_p), ("counts", C.c_void_p), ("locks", C.c_void_p),
+                ("clock", C.c_void_p), ("stats", C.c_void_p), ("num_sets", C.c_int), ("lfu", C.c_int)]
+
+
+class _KeyRegion(C.Structure):
+    _fields_ = [("base", C.c_void_p), ("n", C.c_longlong), ("stride", C.c_longlong), ("ranks", C.c_int),
+                ("key_mod", C.c_int), ("key_rem", C.c_int), ("key_bytes", C.c_int)]
+
+
+class _EvictReinit(C.Structure):
+    _fields_ = [("keys", C.c_void_p), ("adm", C.c_void_p), ("adm_n", C.c_void_p), ("table", C.c_void_p),
+                ("s0", C.c_void_p), ("s1", C.c_void_p), ("row_off", C.c_longlong), ("init_key", C.c_ulonglong),
+                ("bound", C.c_float), ("s0_init", C.c_float), ("pitch", C.c_int), ("col0", C.c_int),
+                ("s0_pitch", C.c_int), ("state_bf16", C.c_int)]
+
+
+def evict_set_of(keys, num_sets: int):
+    """set of every key: the low 32 bits of fmix64(key), modulo the number of sets (hash64 in
+    csrc/embedding.cuh); int64 numpy array"""
+    import numpy as np
+    from .ops import _fmix64
+    h = _fmix64(np.asarray(keys, dtype=np.int64).astype(np.uint64)) & np.uint64(0xFFFFFFFF)
+    return (h % np.uint64(num_sets)).astype(np.int64)
+
+
+class SetAssocTable:
+    """One evicting shard: ``capacity`` (``max_capacity`` rounded up to 32) ways in sets of 32.  A key
+    lives only in set ``evict_set_of(key)``; its local row is ``set * 32 + way``.  ``clock`` is the
+    collection's device clock (int64 [1]), ticked once per training step by the caller.
+
+    A training lookup of a table calls ``touch`` on every key region of the table, then ``insert`` on
+    every region (rows written in place over the keys), then ``reinit`` on the admitted ways; an
+    evaluation lookup calls ``get``.  Regions are 2-D slabs [ranks, stride]: columns
+    [key_off, key_off + n) of every row, keys with key >= 0 and key % key_mod == key_rem are handled,
+    the others become -1.  Rules in docs/embedding.md; the CPU implementation is the reference."""
+
+    def __init__(self, max_capacity: int, strategy: str, clock: torch.Tensor, device):
+        if strategy not in EVICT_STRATEGIES:
+            raise ValueError(f"evict_strategy must be one of {EVICT_STRATEGIES}, not {strategy!r}")
+        self.capacity = (int(max_capacity) + WAYS - 1) // WAYS * WAYS
+        self.num_sets = self.capacity // WAYS
+        self.strategy, self.clock = strategy, clock
+        self.device = torch.device(device)
+        dev = self.device
+        self.keys = torch.full((self.capacity,), -1, dtype=torch.int64, device=dev)
+        self.stamps = torch.zeros(self.capacity, dtype=torch.int64, device=dev)
+        self.counts = torch.zeros(self.capacity, dtype=torch.int64, device=dev)
+        self.locks = torch.zeros(self.num_sets, dtype=torch.int32, device=dev)
+        self.stats = torch.zeros(3, dtype=torch.int64, device=dev)      # admitted, evicted, dropped
+
+    # ---- device plumbing
+    def _view(self, stats=None):
+        return _EvictTableView(self.keys.data_ptr(), self.stamps.data_ptr(), self.counts.data_ptr(),
+                               self.locks.data_ptr(), self.clock.data_ptr(),
+                               (self.stats if stats is None else stats).data_ptr(), self.num_sets,
+                               int(self.strategy == "lfu"))
+
+    @staticmethod
+    def _region(buf, key_off, n, key_mod, key_rem):
+        assert buf.dim() == 2 and buf.stride(1) == 1 and buf.dtype in (torch.int32, torch.int64)
+        return _KeyRegion(buf.data_ptr() + key_off * buf.element_size(), int(n), buf.stride(0), buf.shape[0],
+                          int(key_mod), int(key_rem), buf.element_size())
+
+    def _st(self):
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def _call(self, name, *args):
+        if getattr(lib(), name)(*args):
+            raise RuntimeError(f"{name} failed")
+        D._count()
+
+    # ---- CPU rules (the reference the kernels are tested against)
+    def _owned_keys(self, region, key_mod, key_rem):
+        k = region.to(torch.int64).contiguous()
+        own = k >= 0
+        if key_mod > 1:
+            own &= (k % key_mod) == key_rem
+        return k, own
+
+    def _find(self, base, key):
+        hit = (self.keys[base:base + WAYS] == key).nonzero()
+        return int(hit[0, 0]) if hit.numel() else -1
+
+    def _insert_one(self, key, now, evict, adm, stats):
+        import numpy as np
+        base = int(evict_set_of([key], self.num_sets)[0]) * WAYS
+        slot = self._find(base, key)
+        if slot >= 0:
+            return base + slot
+        k = self.keys[base:base + WAYS].numpy()
+        empty = np.nonzero(k < 0)[0]
+        if empty.size:
+            slot, victim = int(empty[0]), False
+        else:
+            st = self.stamps[base:base + WAYS].numpy()
+            cand = [w for w in range(WAYS) if evict and st[w] != now]
+            if not cand:
+                stats[2] += 1
+                return -1
+            lfu = self.strategy == "lfu"
+            cnt = self.counts[base:base + WAYS].numpy()
+            slot = min(cand, key=lambda w: ((min(int(cnt[w]), COUNT_MAX) if lfu else 0), int(st[w]), int(k[w])))
+            victim = True
+        g = base + slot
+        stats[0] += 1
+        stats[1] += int(victim)
+        self.keys[g], self.stamps[g], self.counts[g] = key, now, 1
+        if adm is not None:
+            adm.append(g)
+        return g
+
+    # ---- lookups
+    def touch(self, buf, key_off: int, n: int, key_mod: int = 1, key_rem: int = 0):
+        """stamp the ways of the present keys with the clock, count the occurrences"""
+        if self.device.type == "cuda":
+            self._call("hctr_evict_touch", C.byref(self._view()),
+                       C.byref(self._region(buf, key_off, n, key_mod, key_rem)), self._st())
+            return
+        now = int(self.clock[0])
+        k, own = self._owned_keys(buf[:, key_off:key_off + n], key_mod, key_rem)
+        for key in k[own].tolist():
+            base = int(evict_set_of([key], self.num_sets)[0]) * WAYS
+            slot = self._find(base, key)
+            if slot >= 0:
+                g = base + slot
+                self.stamps[g] = now
+                self.counts[g] += 1
+
+    def insert(self, buf, key_off: int, n: int, key_mod: int = 1, key_rem: int = 0, adm=None, evict=True,
+               stats=None):
+        """rows of the keys written in place over them: present keys keep their way, missing keys are
+        admitted (an empty way, else the victim of the strategy among the unprotected ways) or dropped
+        (-1).  ``adm``: (list [m] int64, count [1] int32) collecting the admitted ways.  ``evict=False``
+        takes empty ways only (checkpoint load)."""
+        stats = self.stats if stats is None else stats
+        if self.device.type == "cuda":
+            a, an = (adm[0].data_ptr(), adm[1].data_ptr()) if adm is not None else (None, None)
+            self._call("hctr_evict_insert", C.byref(self._view(stats)),
+                       C.byref(self._region(buf, key_off, n, key_mod, key_rem)), a, an, int(evict), self._st())
+            return
+        now = int(self.clock[0])
+        region = buf[:, key_off:key_off + n]
+        k, own = self._owned_keys(region, key_mod, key_rem)
+        out = torch.full_like(k, -1)
+        got = [] if adm is not None else None
+        for idx in own.reshape(-1).nonzero()[:, 0].tolist():
+            out.view(-1)[idx] = self._insert_one(int(k.view(-1)[idx]), now, evict, got, stats)
+        region.copy_(out.to(region.dtype))
+        if adm is not None and got:
+            m = int(adm[1][0])
+            adm[0][m:m + len(got)] = torch.tensor(got, dtype=torch.int64)
+            adm[1][0] = m + len(got)
+
+    def get(self, buf, key_off: int, n: int, key_mod: int = 1, key_rem: int = 0):
+        """rows of the present keys in place, -1 for the others (no touch, no insert)"""
+        if self.device.type == "cuda":
+            self._call("hctr_evict_get", C.byref(self._view()),
+                       C.byref(self._region(buf, key_off, n, key_mod, key_rem)), self._st())
+            return
+        region = buf[:, key_off:key_off + n]
+        k, own = self._owned_keys(region, key_mod, key_rem)
+        out = torch.full_like(k, -1)
+        for idx in own.reshape(-1).nonzero()[:, 0].tolist():
+            key = int(k.view(-1)[idx])
+            base = int(evict_set_of([key], self.num_sets)[0]) * WAYS
+            slot = self._find(base, key)
+            out.view(-1)[idx] = base + slot if slot >= 0 else -1
+        region.copy_(out.to(region.dtype))
+
+    def reinit(self, adm, max_adm: int, table, s0, s1, row_off: int, pitch: int, s0_pitch: int, s0_init: float,
+               bound: float, init_key: int, col0: int = 0):
+        """fresh weights (ops.evict_init_rows) and initial optimizer state for the admitted ways"""
+        if self.device.type == "cuda":
+            sbf = int(any(s is not None and s.dtype == torch.bfloat16 for s in (s0, s1)))
+            p = _EvictReinit(self.keys.data_ptr(), adm[0].data_ptr(), adm[1].data_ptr(), table.data_ptr(),
+                             None if s0 is None else s0.data_ptr(), None if s1 is None else s1.data_ptr(),
+                             int(row_off), int(init_key) & ((1 << 64) - 1), float(bound), float(s0_init),
+                             int(pitch), int(col0), int(s0_pitch), sbf)
+            from .ops import table_bf16
+            self._call("hctr_evict_reinit", C.byref(p), int(max_adm), table_bf16(table), self._st())
+            return
+        from .ops import evict_init_rows
+        ways = adm[0][:int(adm[1][0])]
+        if ways.numel() == 0:
+            return
+        rows = ways + row_off
+        table.view(-1, pitch)[rows] = evict_init_rows(init_key, self.keys[ways], col0, pitch, bound, table.dtype)
+        if s0 is not None:
+            s0.view(-1, s0_pitch)[rows] = s0_init
+        if s1 is not None:
+            s1.view(-1, pitch)[rows] = 0
+
+    # ---- whole-table views (host synchronisation: outside the step)
+    def dump(self):
+        """-> (keys int64 [n], local rows int64 [n]) of the live keys, by key, on CPU"""
+        if self.device.type == "cuda":
+            ok = torch.empty(self.capacity, dtype=torch.int64, device=self.device)
+            os_ = torch.empty(self.capacity, dtype=torch.int64, device=self.device)
+            cnt = torch.zeros(1, dtype=torch.int64, device=self.device)
+            self._call("hctr_evict_dump", self.keys.data_ptr(), self.capacity, ok.data_ptr(), os_.data_ptr(),
+                       cnt.data_ptr(), self._st())
+            c = int(cnt.item())
+            k, s = ok[:c].cpu(), os_[:c].cpu()
+        else:
+            s = (self.keys >= 0).nonzero()[:, 0]
+            k = self.keys[s].clone()
+        order = torch.argsort(k)
+        return k[order], s[order]
+
+    def live(self) -> torch.Tensor:
+        """number of live keys, as a device scalar"""
+        return (self.keys >= 0).sum()

@@ -556,6 +556,24 @@ def sr_round_bf16(x, seed: int, step: int, idx):
     return res.to(x.device)
 
 
+def evict_init_key(seed: int, table_id: int) -> int:
+    """key of the stateless initializer of an evicting table's admitted rows (EvictReinit::init_key)"""
+    return sr_step_key(seed, table_id)
+
+
+def evict_init_rows(init_key: int, keys, col0: int, width: int, bound: float, dtype=torch.float32):
+    """initial weights [n, width] of the admitted ``keys`` of an evicting table, bit for bit as
+    evict_init_value in csrc/evict_table.cu: bound * (2u - 1) in fp32, u = the top 24 bits of
+    fmix64(fmix64(init_key ^ key) ^ global column) / 2^24; a bf16 arena rounds to nearest"""
+    import numpy as np
+    k = np.asarray(keys.cpu().numpy() if torch.is_tensor(keys) else keys, dtype=np.int64).astype(np.uint64)
+    cols = np.arange(col0, col0 + width, dtype=np.uint64)
+    h = _fmix64(_fmix64(np.uint64(init_key & _M64) ^ k)[:, None] ^ cols[None, :])
+    u = (h >> np.uint64(40)).astype(np.float32) * np.float32(1.0 / 16777216.0)
+    w = np.float32(bound) * (np.float32(2.0) * u - np.float32(1.0))
+    return torch.from_numpy(w.astype(np.float32)).to(dtype)
+
+
 def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: dict, lr_t, step_t,
            num_sms: int = 132):
     """Fused per-unique-row optimizer; consumes and clears the workspace."""

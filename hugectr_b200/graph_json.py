@@ -207,6 +207,8 @@ def model_to_json(model) -> dict:
                   "optimizer": t.opt_params.to_json() if t.opt_params else None}
             if t.dynamic:
                 tj.update(init_capacity=t.init_capacity, max_capacity=t.max_capacity)
+                if t.evict_strategy is not None:
+                    tj["evict_strategy"] = t.evict_strategy
             if getattr(t, "weight_dtype", "fp32") != "fp32":
                 tj["weight_dtype"] = t.weight_dtype
             if t.init_param is not None and getattr(t.init_param, "up_bound", 0) > 0:
@@ -257,7 +259,7 @@ def add_from_json(model, graph: dict, include_dense_network: bool = True):
             from .embedding.collection import InitParams
             tabs = {}
             for tt in j["tables"]:
-                kw = {k: tt[k] for k in ("init_capacity", "max_capacity", "weight_dtype") if k in tt}
+                kw = {k: tt[k] for k in ("init_capacity", "max_capacity", "weight_dtype", "evict_strategy") if k in tt}
                 ip = InitParams(up_bound=tt["init_up_bound"]) if "init_up_bound" in tt else None
                 tabs[tt["name"]] = EmbeddingTableConfig(
                     tt["name"], tt["max_vocabulary_size"], tt["ev_size"],

@@ -914,6 +914,18 @@ class Model:
         ebcs = [e for e in getattr(self, "ebcs_train", []) if getattr(e, "has_dynamic", False)]
         if not ebcs:
             return
+        # evicting tables never grow: their counters are logged, the step graph stays
+        seen = self.__dict__.setdefault("_evict_dropped", {})
+        for ei, e in enumerate(ebcs):
+            for (name, shard), st in e.eviction_stats().items():
+                logger.info(f"evicting embedding table {name} shard {shard}: live {st['live']} admitted "
+                            f"{st['admitted']} evicted {st['evicted']} dropped {st['dropped']}")
+                prev = seen.get((ei, name, shard), 0)
+                if st["dropped"] > prev:
+                    logger.warning(f"evicting embedding table {name} shard {shard}: {st['dropped'] - prev} keys "
+                                   "dropped since the last report (every way of their set held a key of the "
+                                   "running step); they read as empty rows and got no update")
+                seen[(ei, name, shard)] = st["dropped"]
         if os.environ.get("HCTR_DYNAMIC_GROW", "1") == "0":
             for e in ebcs:
                 e.check_overflow()
