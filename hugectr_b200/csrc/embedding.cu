@@ -28,7 +28,10 @@ namespace hctr {
 // floats per 32*VEC-wide column chunk.  G*VEC >= ev for ev <= 128 (VEC=4), wider rows loop over
 // up to MAXC chunks per lane: one launch covers columns [col_base, col_base + MAXC * G * VEC).
 // WT: weight type of the arena (fp32, or bf16 loaded 8 bytes per 4 columns); pooling is in fp32.
-template <typename KeyT, typename OutT, int VEC, int U, typename WT>
+// WGT: weighted lookups may be present; a row enters as fma(w, row, acc) (w = 1 for unweighted
+// lookups and 0 for skipped keys: fma(1, v, acc) == acc + v, so all-ones weights pool bit for bit as
+// the unweighted kernel does).
+template <typename KeyT, typename OutT, int VEC, int U, typename WT, bool WGT>
 __global__ void __launch_bounds__(256, 3)
     emb_fwd_kernel(const EmbParams p, const int G, const int col_base) {
   // grid.y = (src rank, lookup): uniform per block, no per-thread integer division
@@ -49,8 +52,12 @@ __global__ void __launch_bounds__(256, 3)
   if (active && lk.nnz_off >= 0) nnz = min(lk.hotness, p.nnz[src][lk.nnz_off + s]);
   if (!active) nnz = 0;
   const WT* table = static_cast<const WT*>(p.table);
+  const bool lw = WGT && lk.weighted;
+  const float* wbase = WGT ? p.weights[src] + lk.key_off + static_cast<long long>(s) * lk.key_stride : nullptr;
 
-  constexpr int MAXC = (U >= 8) ? 8 : 4;  // chunks per lane
+  // chunks per lane.  Weighted vector rows keep 8 chunks at 4 rows in flight: the U weights beside 8 rows' loads
+  // and the accumulators exceed the 80 registers of __launch_bounds__(256, 3) and spill
+  constexpr int MAXC = (U >= 8 || (WGT && VEC == 4)) ? 8 : 4;
   float acc[MAXC][VEC];
 #pragma unroll
   for (int c = 0; c < MAXC; ++c)
@@ -58,8 +65,8 @@ __global__ void __launch_bounds__(256, 3)
     for (int v = 0; v < VEC; ++v) acc[c][v] = 0.f;
   const int nchunk = (ev - col_base + G * VEC - 1) / (G * VEC);
 
-  // gathers U rows (rp[u] == nullptr: skip) into the accumulators
-  auto gather = [&](const WT* const (&rp)[U]) {
+  // gathers U rows (rp[u] == nullptr: skip) with weights wv (WGT only) into the accumulators
+  auto gather = [&](const WT* const (&rp)[U], const float (&wv)[U]) {
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {
       if (c < nchunk) {
@@ -72,14 +79,22 @@ __global__ void __launch_bounds__(256, 3)
               v[u] = rp[u] ? ldg_row4(rp[u] + col) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int u = 0; u < U; ++u) {
-              acc[c][0] += v[u].x; acc[c][1] += v[u].y; acc[c][2] += v[u].z; acc[c][3] += v[u].w;
+              if constexpr (WGT) {
+                acc[c][0] = fmaf(wv[u], v[u].x, acc[c][0]); acc[c][1] = fmaf(wv[u], v[u].y, acc[c][1]);
+                acc[c][2] = fmaf(wv[u], v[u].z, acc[c][2]); acc[c][3] = fmaf(wv[u], v[u].w, acc[c][3]);
+              } else {
+                acc[c][0] += v[u].x; acc[c][1] += v[u].y; acc[c][2] += v[u].z; acc[c][3] += v[u].w;
+              }
             }
           } else {
             float v[U];
 #pragma unroll
             for (int u = 0; u < U; ++u) v[u] = rp[u] ? ldg_row1(rp[u] + col) : 0.f;
 #pragma unroll
-            for (int u = 0; u < U; ++u) acc[c][0] += v[u];
+            for (int u = 0; u < U; ++u) {
+              if constexpr (WGT) acc[c][0] = fmaf(wv[u], v[u], acc[c][0]);
+              else acc[c][0] += v[u];
+            }
           }
         }
       }
@@ -95,6 +110,7 @@ __global__ void __launch_bounds__(256, 3)
     const unsigned int ns = static_cast<unsigned int>(lk.num_shards);
     for (int h0 = 0; h0 < nnz; h0 += KPL * G) {
       unsigned int rowv[4] = {0u, 0u, 0u, 0u};
+      float wtv[4] = {1.f, 1.f, 1.f, 1.f};   // WGT: the weights travel with rowv
       unsigned int m = 0;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -117,6 +133,7 @@ __global__ void __launch_bounds__(256, 3)
               }
               ok = rem == static_cast<unsigned int>(lk.shard_idx) && q < static_cast<unsigned long long>(lk.rows);
               rowv[i] = static_cast<unsigned int>(q);
+              if (lw && ok) wtv[i] = wbase[h];
             }
           }
           const unsigned int bal = (__ballot_sync(gmask, ok) >> (gi * G)) & ((G == 32) ? 0xffffffffu : ((1u << G) - 1u));
@@ -125,6 +142,7 @@ __global__ void __launch_bounds__(256, 3)
       }
       while (m) {               // group-uniform
         const WT* rp[U];
+        float wv[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           rp[u] = nullptr;
@@ -135,8 +153,13 @@ __global__ void __launch_bounds__(256, 3)
           const unsigned int cand = i == 0 ? rowv[0] : (i == 1 ? rowv[1] : (i == 2 ? rowv[2] : rowv[3]));
           const unsigned int r = __shfl_sync(gmask, cand, gi * G + sl);
           if (take) rp[u] = table + (lk.table_row_off + r) * static_cast<long long>(p.ev_size);
+          if constexpr (WGT) {
+            const float cw = i == 0 ? wtv[0] : (i == 1 ? wtv[1] : (i == 2 ? wtv[2] : wtv[3]));
+            const float w = __shfl_sync(gmask, cw, gi * G + sl);
+            wv[u] = take ? w : 0.f;
+          }
         }
-        gather(rp);
+        gather(rp, wv);
       }
     }
   } else {
@@ -144,17 +167,24 @@ __global__ void __launch_bounds__(256, 3)
       // lanes of the group fetch up to G keys at once (coalesced peer/local read)
       long long mykey = -1;
       if (h0 + gl < nnz) mykey = static_cast<long long>(kbase[h0 + gl]);
+      float myw = 1.f;
+      if (lw && h0 + gl < nnz) myw = wbase[h0 + gl];
       const int cnt = min(G, nnz - h0);
       for (int j0 = 0; j0 < cnt; j0 += U) {
         const WT* rp[U];
+        float wv[U];
 #pragma unroll
         for (int u = 0; u < U; ++u) {
           const int j = j0 + u;
           const long long key = __shfl_sync(gmask, mykey, gi * G + (j < cnt ? j : 0));
           const bool ok = (j < cnt) && key >= 0 && key < lk.rows;
           rp[u] = ok ? table + (lk.table_row_off + key) * static_cast<long long>(p.ev_size) : nullptr;
+          if constexpr (WGT) {
+            const float w = __shfl_sync(gmask, myw, gi * G + (j < cnt ? j : 0));
+            wv[u] = ok ? w : 0.f;
+          }
         }
-        gather(rp);
+        gather(rp, wv);
       }
     }
   }
@@ -181,8 +211,9 @@ __global__ void __launch_bounds__(256, 3)
 
 // ------------------------------------------------------------------ backward accumulate
 // Same bucket decomposition as forward.  Each group loads its bucket's gradient row once and
-// red.adds it (fp32) into wgrad_unique[uid] for every owned key of the bucket.
-template <typename KeyT, typename GradT, int VEC>
+// red.adds it (fp32) into wgrad_unique[uid] for every owned key of the bucket; WGT: times the key's
+// weight (weighted lookups).
+template <typename KeyT, typename GradT, int VEC, bool WGT>
 __global__ void __launch_bounds__(256)
     emb_bwd_accum_kernel(const EmbParams p, const UniqueTable ut, float* __restrict__ wgrad_unique,
                          const float grad_scale, const int G, const long long total_items) {
@@ -235,6 +266,8 @@ __global__ void __launch_bounds__(256)
   for (int h0 = 0; h0 < nnz; h0 += G) {
     long long mykey = -1;
     if (h0 + gl < nnz) mykey = static_cast<long long>(kbase[h0 + gl]);
+    float myw = 1.f;
+    if (WGT && h0 + gl < nnz) myw = key_weight(p, lk, src, s, h0 + gl);
     // every lane resolves the unique id of ITS key (parallel hash probes), then broadcast
     unsigned int myuid = kInvalidVal;
     if (mykey >= 0 && (lk.num_shards == 1 || (mykey % lk.num_shards) == lk.shard_idx)) {
@@ -248,6 +281,8 @@ __global__ void __launch_bounds__(256)
     const int cnt = min(G, nnz - h0);
     for (int j = 0; j < cnt; ++j) {
       const unsigned int uid = __shfl_sync(gmask, myuid, gi * G + j);
+      float w = 1.f;
+      if constexpr (WGT) w = __shfl_sync(gmask, myw, gi * G + j);
       if (uid == kInvalidVal || uid >= ut.max_unique) continue;
       float* dst = wgrad_unique + static_cast<long long>(uid) * p.ev_size;
 #pragma unroll
@@ -256,11 +291,17 @@ __global__ void __launch_bounds__(256)
           const int col = (c * G + gl) * VEC;
           if (col < ev) {
             if constexpr (VEC == 4) {
-              asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + col),
-                           "f"(g[c][0]), "f"(g[c][1]), "f"(g[c][2]), "f"(g[c][3])
-                           : "memory");
+              if constexpr (WGT) {
+                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + col),
+                             "f"(g[c][0] * w), "f"(g[c][1] * w), "f"(g[c][2] * w), "f"(g[c][3] * w)
+                             : "memory");
+              } else {
+                asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + col),
+                             "f"(g[c][0]), "f"(g[c][1]), "f"(g[c][2]), "f"(g[c][3])
+                             : "memory");
+              }
             } else {
-              atomicAdd(dst + col, g[c][0]);
+              atomicAdd(dst + col, WGT ? g[c][0] * w : g[c][0]);
             }
           }
         }
@@ -273,7 +314,8 @@ __global__ void __launch_bounds__(256)
 // the LOCAL batch.  Hot rows of tiny tables would serialise global reductions on a handful of L2
 // lines, so a block (one lookup x one chunk of samples) first accumulates into a shared-memory copy
 // of the table when it fits and flushes it with one vector reduction per non-zero 16-byte group.
-template <typename KeyT, typename GradT>
+// WGT: every key's share is scaled by its weight (weighted lookups).
+template <typename KeyT, typename GradT, bool WGT>
 __global__ void __launch_bounds__(256)
     emb_dp_wgrad_kernel(const EmbParams p, float* __restrict__ wgrad, const float grad_scale,
                         const int smem_floats) {
@@ -304,13 +346,15 @@ __global__ void __launch_bounds__(256)
       for (int h = 0; h < nnz; ++h) {
         const long long key = static_cast<long long>(kb[h]);
         if (key < 0 || key >= lk.rows) continue;
+        float4 u = v;
+        if constexpr (WGT) u = scale4(v, key_weight(p, lk, 0, s, h));
         if (priv) {
           float* d = dp_acc + key * ev + col;
-          atomicAdd(d, v.x); atomicAdd(d + 1, v.y); atomicAdd(d + 2, v.z); atomicAdd(d + 3, v.w);
+          atomicAdd(d, u.x); atomicAdd(d + 1, u.y); atomicAdd(d + 2, u.z); atomicAdd(d + 3, u.w);
         } else {
           float* d = wgrad + (lk.table_row_off + key) * pitch + col;
-          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d), "f"(v.x), "f"(v.y),
-                       "f"(v.z), "f"(v.w) : "memory");
+          asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(d), "f"(u.x), "f"(u.y),
+                       "f"(u.z), "f"(u.w) : "memory");
         }
       }
     }
@@ -480,13 +524,15 @@ extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, i
   const int pass = (vec == 4) ? max_ev : 8 * G;
   for (int c0 = 0; c0 < max_ev; c0 += pass) {
     with_key(key_bytes, [&](auto k) { with_elem(out_bf16, [&](auto o) { with_elem(table_bf16, [&](auto w) {
-      auto launch = [&](auto v, auto u) {   // vector width, rows in flight per gather round
-        emb_fwd_kernel<type_of<decltype(k)>, type_of<decltype(o)>, decltype(v)::value, decltype(u)::value,
-                       type_of<decltype(w)>><<<blocks, threads, 0, st>>>(*p, G, c0);
-      };
-      if (vec == 1) launch(Int<1>{}, Int<8>{});
-      else if (narrow) launch(Int<4>{}, Int<4>{});
-      else launch(Int<4>{}, Int<8>{});
+      with_weighted(*p, [&](auto wgt) {
+        auto launch = [&](auto v, auto u) {   // vector width, rows in flight per gather round
+          emb_fwd_kernel<type_of<decltype(k)>, type_of<decltype(o)>, decltype(v)::value, decltype(u)::value,
+                         type_of<decltype(w)>, decltype(wgt)::value><<<blocks, threads, 0, st>>>(*p, G, c0);
+        };
+        if (vec == 1) launch(Int<1>{}, Int<8>{});
+        else if (narrow) launch(Int<4>{}, Int<4>{});
+        else launch(Int<4>{}, Int<decltype(wgt)::value ? 4 : 8>{});
+      });
     }); }); });
   }
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
@@ -552,28 +598,28 @@ extern "C" int hctr_emb_backward_accum(const EmbParams* p, const UniqueTable* ut
     if (chunks * 8 > p->batch) chunks = (p->batch + 7) / 8;
     if (chunks < 1) chunks = 1;
     const dim3 grid(chunks, p->num_lookups);
-    with_key(key_bytes, [&](auto k) { with_elem(grad_bf16, [&](auto g) {
-      const auto kernel = emb_dp_wgrad_kernel<type_of<decltype(k)>, type_of<decltype(g)>>;
-      // once per instantiation: this static belongs to the (k, g) instance of the lambda
+    with_key(key_bytes, [&](auto k) { with_elem(grad_bf16, [&](auto g) { with_weighted(*p, [&](auto wgt) {
+      const auto kernel = emb_dp_wgrad_kernel<type_of<decltype(k)>, type_of<decltype(g)>, decltype(wgt)::value>;
+      // once per instantiation: this static belongs to the (k, g, wgt) instance of the lambda
       static const cudaError_t attr =
           cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem);
       (void)attr;
       kernel<<<grid, 256, kSmem, st>>>(*p, wgrad_unique, grad_scale, kSmem / 4);
-    }); });
+    }); }); });
     return cudaGetLastError() == cudaSuccess ? 0 : -1;
   }
   if (max_ev > kMaxEmbWidth) return -4;
   const long long warps = (items + (32 / G) - 1) / (32 / G);
   const int threads = 256;
   const long long blocks = (warps * 32 + threads - 1) / threads;
-  with_key(key_bytes, [&](auto k) { with_elem(grad_bf16, [&](auto g) {
+  with_key(key_bytes, [&](auto k) { with_elem(grad_bf16, [&](auto g) { with_weighted(*p, [&](auto wgt) {
     auto launch = [&](auto v) {
-      emb_bwd_accum_kernel<type_of<decltype(k)>, type_of<decltype(g)>, decltype(v)::value>
+      emb_bwd_accum_kernel<type_of<decltype(k)>, type_of<decltype(g)>, decltype(v)::value, decltype(wgt)::value>
           <<<(unsigned)blocks, threads, 0, st>>>(*p, *ut, wgrad_unique, grad_scale, G, items);
     };
     if (vec == 4) launch(Int<4>{});
     else launch(Int<1>{});
-  }); });
+  }); }); });
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

@@ -33,7 +33,7 @@ struct EmbLookup {
   int combiner;             // 0 = sum, 1 = mean
   int ev_size;
   int rows;                 // rows of the local shard (bounds guard)
-  int pad_;
+  int weighted;             // 1: every key carries an fp32 weight at its element offset in weights[src]
   long long pair_off;       // first (bucket,key) pair index of this lookup (backward index)
 };
 
@@ -46,7 +46,15 @@ struct EmbParams {
   const EmbLookup* lookups;      // device array [num_lookups]
   void* table;                   // [rows, ev] arena of fp32 or bf16 weights (the launcher's table_bf16)
   int ev_size;                   // row pitch of the arena (all tables of a group share it)
+  // per source rank: fp32 per-key weights in the layout of keys (same element offsets); all null
+  // when no lookup of the launch is weighted, which selects the unweighted kernels
+  const float* weights[kMaxRanks];
 };
+
+// Weight of key h of bucket (src, s) of a lookup: 1 unless the lookup is weighted
+HCTR_DEVICE float key_weight(const EmbParams& p, const EmbLookup& lk, int src, int s, int h) {
+  return lk.weighted ? p.weights[src][lk.key_off + static_cast<long long>(s) * lk.key_stride + h] : 1.f;
+}
 
 struct PeerStage {
   void* dst[kMaxRanks];
@@ -221,6 +229,12 @@ template <typename Fn>
 inline void with_key(int key_bytes, Fn&& fn) {
   if (key_bytes == 8) fn(Tag<long long>{});
   else fn(Tag<int>{});
+}
+// weighted lookups in the launch (p.weights set): the instantiations that read per-key weights
+template <typename Fn>
+inline void with_weighted(const EmbParams& p, Fn&& fn) {
+  if (p.weights[0] != nullptr) fn(std::true_type{});
+  else fn(std::false_type{});
 }
 // The sparse optimizers: calls fn(Int<OPT>, Tag<StateT>, Tag<WT>) for optimizer `opt`, state type (bf16
 // when state_bf16) and weight type (bf16 when table_bf16).  SGD (no state) and row-wise AdaGrad (a

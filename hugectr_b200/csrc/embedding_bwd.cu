@@ -297,6 +297,8 @@ __global__ void __launch_bounds__(1024)
 
 // ---------------------------------------------------------------- C: fill (counting sort)
 // Same block aggregation: positions inside a row's bucket list are reserved once per (block, row).
+// An entry's scale is 1/nnz for a mean bag, times the key's weight for a weighted lookup (WGT).
+template <bool WGT>
 __global__ void __launch_bounds__(kIdxThreads)
     emb_bwd_fill_kernel(const EmbParams p, const BwdIndex ix, const long long total_pairs) {
   __shared__ unsigned int h_uid[kSmemSlots];
@@ -352,6 +354,7 @@ __global__ void __launch_bounds__(kIdxThreads)
         const int nnz = bucket_nnz(p, __ldg(&lk->hotness), __ldg(&lk->nnz_off), pi.src, pi.s);
         sc = 1.f / static_cast<float>(max(nnz, 1));
       }
+      if constexpr (WGT) sc *= key_weight(p, *lk, pi.src, pi.s, pi.h);
       ix.bucket_scale[pos] = sc;
     }
   }
@@ -798,7 +801,9 @@ extern "C" int hctr_emb_bwd_index(const EmbParams* p, const UniqueTable* ut, con
   scan_apply_kernel<<<nb, 1024, 0, st>>>(ix->count, ix->block_sums, ix->offsets, ut->counter,
                                          ut->max_unique);
   emb_bwd_classify_kernel<<<num_sms(), 1024, 0, st>>>(*ut, *ix);
-  emb_bwd_fill_kernel<<<blocks, kIdxThreads, 0, st>>>(*p, *ix, total_pairs);
+  with_weighted(*p, [&](auto wgt) {
+    emb_bwd_fill_kernel<decltype(wgt)::value><<<blocks, kIdxThreads, 0, st>>>(*p, *ix, total_pairs);
+  });
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

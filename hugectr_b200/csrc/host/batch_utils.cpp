@@ -7,8 +7,10 @@
 // receives the final layout.
 #include <stdint.h>
 
-extern "C" void hctr_csr_to_padded(const void* offs, int off_bytes, const long long* vals, int n, int H,
-                                   long long add, long long* out, long long row_stride, int32_t* nnz) {
+// T = long long (keys, + add) or float (the per-key weights of a weighted input, add unused)
+template <typename T>
+static void csr_to_padded(const void* offs, int off_bytes, const T* vals, int n, int H, T add, T* out,
+                          long long row_stride, int32_t* nnz) {
 #pragma omp parallel for schedule(static) if (n > 2048)
   for (int i = 0; i < n; ++i) {
     long long lo, hi;
@@ -22,10 +24,22 @@ extern "C" void hctr_csr_to_padded(const void* offs, int off_bytes, const long l
     long long c = hi - lo;
     if (c > H) c = H;
     if (c < 0) c = 0;
-    long long* o = out + static_cast<long long>(i) * row_stride;
+    T* o = out + static_cast<long long>(i) * row_stride;
     for (long long h = 0; h < c; ++h) o[h] = vals[lo + h] + add;
-    nnz[i] = static_cast<int32_t>(c);
+    if (nnz) nnz[i] = static_cast<int32_t>(c);
   }
+}
+
+extern "C" void hctr_csr_to_padded(const void* offs, int off_bytes, const long long* vals, int n, int H,
+                                   long long add, long long* out, long long row_stride, int32_t* nnz) {
+  csr_to_padded<long long>(offs, off_bytes, vals, n, H, add, out, row_stride, nnz);
+}
+
+// hctr_csr_to_padded_f32: the weight column of a weighted multi-hot slot into the [b, S, H] fp32 weight block, in
+// the positions hctr_csr_to_padded gives the keys (0 padding already in place)
+extern "C" void hctr_csr_to_padded_f32(const void* offs, int off_bytes, const float* vals, int n, int H, float* out,
+                                       long long row_stride) {
+  csr_to_padded<float>(offs, off_bytes, vals, n, H, 0.f, out, row_stride, nullptr);
 }
 
 // hctr_onehot_block: S one-hot (scalar) columns of a row-group slice -> the [b, S] key block of a batch in

@@ -5,6 +5,8 @@ Layout handed to the model (per rank, ``b`` = samples of this rank):
   keys   1-D, *feature-major*: for sparse param p (in Input order) a block [b, S_p * H_p]
          (slot_num x max nnz per slot), padded with -1 for variable-length slots
   nnz    optional 1-D int32: for param p a block [S_p, b] with the valid count per (slot, sample)
+  weights optional 1-D fp32 in the layout of keys: the weight of every key of a weighted input (1 for
+         the keys of unweighted inputs); None when no input is weighted
 All tensors are pinned so the H2D copies are asynchronous.
 """
 from __future__ import annotations
@@ -27,6 +29,7 @@ class HostBatch:
     raw: Optional[torch.Tensor] = None   # device-split readers: the batch's raw records (pinned uint8) ...
     raw_skew: int = 0                    # ... starting at this byte offset; label / dense / keys are None
     splitter: object = None              # RawSplit: knows how to turn ``raw`` into the three tensors on the device
+    weights: Optional[torch.Tensor] = None
 
     def mark_copied(self):
         """Called by the consumer right after it queued its asynchronous H2D copies: ring-buffer
@@ -44,7 +47,7 @@ class HostBatch:
 
     def pin(self):
         if torch.cuda.is_available():
-            for n in ("label", "dense", "keys", "nnz"):
+            for n in ("label", "dense", "keys", "nnz", "weights"):
                 t = getattr(self, n)
                 if t is not None and not t.is_pinned():
                     setattr(self, n, t.pin_memory())
@@ -53,7 +56,7 @@ class HostBatch:
     def h2d_bytes(self) -> int:
         if self.raw is not None:
             return int(self.splitter.batch * self.splitter.rec_bytes)
-        return sum(t.numel() * t.element_size() for t in (self.label, self.dense, self.keys, self.nnz)
+        return sum(t.numel() * t.element_size() for t in (self.label, self.dense, self.keys, self.nnz, self.weights)
                    if t is not None)
 
 

@@ -46,6 +46,23 @@ def _csr_to_padded(offs, vals, n, H, add, blk, s, nz):
                          blk.ctypes.data + 8 * s * Hb, S * Hb, nz.ctypes.data + 4 * s * nz.shape[1])
 
 
+def _csr_to_padded_f32(offs, vals, n, H, wblk, s):
+    """wblk[i, s, :min(len_i, H)] = vals[offs[i]:...]: the weights of a multi-hot slot where _csr_to_padded puts
+    its keys (native, OpenMP)"""
+    import ctypes as C
+    from .. import _native
+    L = _native.host_lib()
+    L.hctr_csr_to_padded_f32.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                         C.c_longlong]
+    offs = np.ascontiguousarray(offs)
+    if offs.dtype not in (np.int32, np.int64):
+        offs = offs.astype(np.int64)
+    vals = np.ascontiguousarray(vals, dtype=np.float32)
+    S, Hb = wblk.shape[1], wblk.shape[2]
+    L.hctr_csr_to_padded_f32(offs.ctypes.data, offs.dtype.itemsize, vals.ctypes.data, int(n), int(H),
+                             wblk.ctypes.data + 4 * s * Hb, S * Hb)
+
+
 def _onehot_block(cols, add, lo, nloc, b, blk, nz):
     """blk[i, s, 0] = cols[s][lo + i] + add[s] (i < nloc; -1 behind), nz[s, i] = 1 / 0 -- native, GIL released"""
     import ctypes as C
@@ -85,6 +102,10 @@ class ParquetReader(IDataReader):
         # `Solver.drop_incomplete_batch` is applied by Model._train_step, like for the Raw / Norm readers)
         self.drop_incomplete = False
         self._device = getattr(model, "device", None)
+        # per block: does the input carry weights (weight_index columns of its slots)
+        self.weighted = list(getattr(self.layout, "weighted", None) or [False] * len(self.layout.blocks))
+        if any(self.weighted):
+            self._columns(read_file_list(self.file_list))     # a weighted slot without a weight column raises here
 
     # -------------------------------------------------------------- producer
     def _columns(self, files):
@@ -92,18 +113,30 @@ class ParquetReader(IDataReader):
         meta_path = os.path.join(d, "_metadata.json")
         inp = self.inp
         nl, nd, ns = inp.label_dim, inp.dense_dim, self.layout.total_slots
+        wgt = [None] * ns
         if os.path.exists(meta_path):
             m = json.load(open(meta_path))
             lab = [c["index"] for c in m["labels"]][:nl]
             con = [c["index"] for c in m["conts"]][:nd]
             cat = [c["index"] for c in m["cats"]][:ns]
+            wgt = [c.get("weight_index") for c in m["cats"]][:ns]
         else:
             lab, con, cat = list(range(nl)), list(range(nl, nl + nd)), list(range(nl + nd, nl + nd + ns))
-        return lab, con, cat
+        # weight columns of the slots of weighted inputs only (an unweighted input ignores a weight_index)
+        si = 0
+        for (name, S, _, _), w in zip(self.layout.blocks, self.weighted):
+            for s in range(S):
+                if not w:
+                    wgt[si] = None
+                elif wgt[si] is None:
+                    raise ValueError(f"weighted input {name}: slot {s} (cats entry {si} of {meta_path}) has no "
+                                     "weight_index")
+                si += 1
+        return lab, con, (cat, wgt)
 
     def _decode_row_group(self, fp, rg, lab_i, con_i, cat_i):
-        """one row group -> (label [n, L], dense [n, D], per-slot (offsets|None, values), n); runs on the
-        row-group worker threads (reference RowGroupReadingThread, row_group_reading_thread.cpp)"""
+        """one row group -> (label [n, L], dense [n, D], per-slot (offsets|None, values, weights|None), n); runs
+        on the row-group worker threads (reference RowGroupReadingThread, row_group_reading_thread.cpp)"""
         import pyarrow as pa
         import pyarrow.parquet as pq
         from ..utils.diagnose import nvtx_range
@@ -119,12 +152,28 @@ class ParquetReader(IDataReader):
         den = np.stack([cols[i].to_numpy().astype("float32", copy=False) for i in con_i], 1) \
             if con_i else np.zeros((n, 0), "float32")
         cats = []
-        for i in cat_i:
+        is_list = lambda c: pa.types.is_list(c.type) or pa.types.is_large_list(c.type)
+        for i, wi in zip(*cat_i):
             c = cols[i].combine_chunks()
-            if pa.types.is_list(c.type) or pa.types.is_large_list(c.type):
-                cats.append((c.offsets.to_numpy(), c.values.to_numpy().astype("int64", copy=False)))
+            wv = None
+            if wi is not None:
+                w = cols[wi].combine_chunks()
+                same = is_list(w) == is_list(c) and (not is_list(c) or np.array_equal(
+                    np.diff(w.offsets.to_numpy()), np.diff(c.offsets.to_numpy())))
+                if not same:
+                    raise ValueError(f"{fp} row group {rg}: weight column {tbl.column_names[wi]} does not have the "
+                                     f"list lengths of key column {tbl.column_names[i]}")
+                if is_list(w):
+                    # indexed like the key values: both columns' offsets may start anywhere in their buffers
+                    ko, wo = c.offsets.to_numpy(), w.offsets.to_numpy()
+                    wv = np.zeros(len(c.values), dtype="float32")
+                    wv[ko[0]:ko[-1]] = w.values.to_numpy(zero_copy_only=False)[wo[0]:wo[-1]]
+                else:
+                    wv = w.to_numpy(zero_copy_only=False).astype("float32", copy=False)
+            if is_list(c):
+                cats.append((c.offsets.to_numpy(), c.values.to_numpy().astype("int64", copy=False), wv))
             else:
-                cats.append((None, c.to_numpy().astype("int64", copy=False)))
+                cats.append((None, c.to_numpy().astype("int64", copy=False), wv))
         return (lab, den, cats, n)
 
     def _row_groups(self, files):
@@ -188,18 +237,19 @@ class ParquetReader(IDataReader):
 
     @staticmethod
     def _slice_cat(cat, a, b):
-        offs, vals = cat
+        offs, vals, w = cat
         if offs is None:
-            return (None, vals[a:b])
+            return (None, vals[a:b], None if w is None else w[a:b])
         o = offs[a:b + 1]
-        return (o - o[0], vals[o[0]:o[-1]])
+        return (o - o[0], vals[o[0]:o[-1]], None if w is None else w[o[0]:o[-1]])
 
     @staticmethod
     def _cat_concat(c1, c2):
+        w = None if c1[2] is None else np.concatenate([c1[2], c2[2]])
         if c1[0] is None:
-            return (None, np.concatenate([c1[1], c2[1]]))
+            return (None, np.concatenate([c1[1], c2[1]]), w)
         o = np.concatenate([c1[0], c2[0][1:] + c1[0][-1]])
-        return (o, np.concatenate([c1[1], c2[1]]))
+        return (o, np.concatenate([c1[1], c2[1]]), w)
 
     def _emit(self, chunk, carry, gb):
         if carry is not None:
@@ -252,10 +302,22 @@ class ParquetReader(IDataReader):
         nelems = sum(S * b for (_, S, H, _) in blocks)
         keys = np.full(kelems, -1, dtype=kdt)
         nnz = np.zeros(nelems, dtype="int32")
+        # weights in the key layout: 1 for unweighted inputs, 0 at the padding of weighted ones
+        wts = np.ones(kelems, dtype="float32") if any(self.weighted) else None
         si = ko = no = 0
-        for (name, S, H, fixed) in blocks:
+        for (name, S, H, fixed), weighted in zip(blocks, self.weighted):
             blk = keys[ko:ko + b * S * H].reshape(b, S, H)
             nz = nnz[no:no + S * b].reshape(S, b)
+            if weighted:
+                wblk = wts[ko:ko + b * S * H].reshape(b, S, H)
+                wblk[...] = 0
+                for s in range(S):
+                    if nloc > 0:
+                        offs, _, wv = self._slice_cat(cats[si + s], lo, hi)
+                        if offs is None:
+                            wblk[:nloc, s, 0] = wv[:nloc]
+                        else:
+                            _csr_to_padded_f32(offs, wv, nloc, H, wblk, s)
             if H == 1 and all(cats[si + s][0] is None for s in range(S)):
                 # one-hot block: one strided store per slot, offsets added in the key dtype
                 _onehot_block([cats[si + s][1] for s in range(S)],
@@ -265,7 +327,7 @@ class ParquetReader(IDataReader):
             else:
                 tmp = blk if kdt == "int64" else np.full((b, S, H), -1, dtype="int64")
                 for s in range(S):
-                    offs, vals = self._slice_cat(cats[si], lo, hi) if nloc > 0 else (None, np.zeros(0, "int64"))
+                    offs, vals, _ = self._slice_cat(cats[si], lo, hi) if nloc > 0 else (None, np.zeros(0, "int64"), None)
                     off_add = 0 if self.slot_offsets is None else self.slot_offsets[si]
                     if offs is None:
                         tmp[:nloc, s, 0] = vals[:nloc] + off_add
@@ -278,7 +340,8 @@ class ParquetReader(IDataReader):
             ko += b * S * H
             no += S * b
         hb = HostBatch(torch.from_numpy(L), torch.from_numpy(D), torch.from_numpy(keys),
-                       torch.from_numpy(nnz) if blocks else None, nloc).pin()
+                       torch.from_numpy(nnz) if blocks else None, nloc,
+                       weights=None if wts is None else torch.from_numpy(wts)).pin()
         return (hb, nvalid_global)
 
     # -------------------------------------------------------------- consumer

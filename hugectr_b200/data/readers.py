@@ -113,7 +113,8 @@ class CachedEvalReader(IDataReader):
             kept = HostBatch(lab, den, keys, None, hb.num_valid)
         else:
             mv = lambda t: None if t is None else t.to(self.device, copy=True)
-            kept = HostBatch(mv(hb.label), mv(hb.dense), mv(hb.keys), mv(hb.nnz), hb.num_valid)
+            kept = HostBatch(mv(hb.label), mv(hb.dense), mv(hb.keys), mv(hb.nnz), hb.num_valid,
+                             weights=mv(hb.weights))
         hb.mark_copied()
         self.cache.append(kept)
         self.current_batchsize = self.inner.current_batchsize
@@ -132,6 +133,7 @@ class SparseLayout:
         self.blocks = []   # (name, slot_num, H, fixed)
         for p in self.params:
             self.blocks.append((p.top_name, p.slot_num, max(p.nnz_per_slot), p.is_fixed_length))
+        self.weighted = [bool(getattr(p, "weighted", False)) for p in self.params]
         self.total_slots = sum(b[1] for b in self.blocks)
         self.slot_sizes = list(slot_size_array or [])
 
@@ -155,6 +157,9 @@ class SparseLayout:
     def has_variable(self) -> bool:
         return any(not f for (_, _, _, f) in self.blocks)
 
+    def has_weights(self) -> bool:
+        return any(self.weighted)
+
 
 class SyntheticReader(IDataReader):
     """Pre-generates a pool of pinned batches (power-law or uniform keys) and cycles through it."""
@@ -168,6 +173,7 @@ class SyntheticReader(IDataReader):
         gen = torch.Generator()
         gen.manual_seed(seed * 1000003 + rank * 7919 + 17)
         b = batch_per_rank
+        wgen = None
         for _ in range(pool):
             label = (torch.rand(b, label_dim, generator=gen) < 0.3).float()
             dense = torch.rand(b, dense_dim, generator=gen)
@@ -194,7 +200,17 @@ class SyntheticReader(IDataReader):
                 blocks.append(torch.stack(cols, 1).reshape(-1))   # [b, S, H]
             keys = torch.cat(blocks).to(key_dtype) if blocks else torch.zeros(0, dtype=key_dtype)
             nnz = torch.cat(nnzs) if (nnzs and layout.has_variable()) else None
-            self.pool.append(HostBatch(label, dense, keys, nnz, b).pin())
+            weights = None
+            if layout.has_weights():
+                # a generator of their own: the key, label and dense streams stay as without weights
+                if wgen is None:
+                    wgen = torch.Generator()
+                    wgen.manual_seed(seed * 1000003 + rank * 7919 + 29)
+                wb = []
+                for (name, S, H, fixed), wt in zip(layout.blocks, layout.weighted):
+                    wb.append(torch.rand(b * S * H, generator=wgen) + 0.5 if wt else torch.ones(b * S * H))
+                weights = torch.cat(wb)
+            self.pool.append(HostBatch(label, dense, keys, nnz, b, weights=weights).pin())
         self.i = 0
         self.num_batches = num_batches
         self.served = 0

@@ -226,8 +226,12 @@ class EmbeddingCollection:
     def __init__(self, cfg: EmbeddingCollectionConfig, batch_per_gpu: int, hotness: Dict[str, int],
                  device, act_dtype, comm, default_opt: OptParamsPy, key_dtype=torch.int32,
                  scaler: float = 1.0, state_dtype=torch.float32, seed: int = 0,
-                 fused: Optional[bool] = None, is_train: bool = True):
+                 fused: Optional[bool] = None, is_train: bool = True, weighted=()):
+        """``weighted``: names of the sparse inputs whose keys carry an fp32 weight each (see
+        docs/embedding.md): every lookup of such an input pools ``sum_h w_h * T[key_h]`` (mean: divided
+        by ``sum_h w_h``, or by 1 when that is 0)."""
         self.cfg, self.b, self.device, self.act_dtype = cfg, batch_per_gpu, device, act_dtype
+        self.weighted_inputs = frozenset(weighted)
         # who am I / whom do I talk to: through the backend-neutral interface (core.py; reference core.hpp)
         from ..core import as_core
         self.core = as_core(comm)
@@ -268,6 +272,7 @@ class EmbeddingCollection:
         # index: a run is reproducible for a fixed sharding plan)
         self.sr_seed = int(seed) & 0xFFFFFFFF
         self._unique_tables = self._resolve_unique_tables()
+        self._check_weighted()
         self._kb = 8 if key_dtype == torch.int64 else 4
         self._abf = act_dtype == torch.bfloat16
         # clock of the evicting tables: ticked once per training step inside the step (not Model.step_t,
@@ -308,6 +313,25 @@ class EmbeddingCollection:
                             f"dynamic={t.dynamic}) stays on the Reduction exchange")
         return ok
 
+    def _check_weighted(self):
+        """Weighted inputs pool weighted sums or means; the lookups that cannot honour weights reject them."""
+        from ..enums import CompressionStrategy
+        unique = set()
+        for k, v in (self.cfg.compression_strategy or {}).items():
+            if k == CompressionStrategy.Unique or str(k).endswith("Unique"):
+                names = [t.name for t in self.tables]
+                unique |= {names[x] if isinstance(x, int) else str(x) for x in v}
+        for lk in self.cfg.lookups:
+            for t, bot, comb in zip(lk["tables"], lk["bottoms"], lk["combiners"]):
+                if bot not in self.weighted_inputs:
+                    continue
+                if comb not in ("sum", "mean", "average"):
+                    raise ValueError(f"weighted input {bot}: lookup {lk['top']} of table {t.name} uses the {comb!r} "
+                                     "combiner; weighted inputs pool with sum or mean")
+                if t.name in unique:
+                    raise ValueError(f"weighted input {bot}: table {t.name} is listed under CompressionStrategy.Unique, "
+                                     "which does not carry weights")
+
     def eval_clone(self, batch_per_gpu: int) -> "EmbeddingCollection":
         """Second plan (different batch, no grads) over the SAME tables -- the eval graph."""
         import copy
@@ -339,7 +363,8 @@ class EmbeddingCollection:
                 H = int(hotness[bot])
                 gl = {"table": t.name, "bottom": bot, "combiner": comb, "hotness": H,
                       "key_off": koff, "top": len(self.tops), "col": col, "ev": t.ev_size,
-                      "out_off": ooff + col, "out_stride": width}
+                      "out_off": ooff + col, "out_stride": width,
+                      "weighted": bot in getattr(self, "weighted_inputs", ())}
                 koff += b * H
                 col += t.ev_size * (H if comb == "concat" else 1)
                 ids.append(len(self.glookups))
@@ -349,6 +374,8 @@ class EmbeddingCollection:
             ooff += b * width
         self.user_key_elems = koff
         self.key_slab_elems = koff
+        # fp32 per-key weights in the layout of the user region of the key slab (weighted inputs only)
+        self.has_weights = any(gl["weighted"] for gl in self.glookups)
         self.nnz_slab_elems = 0
         self.top_slab_elems = ooff
         # partial blocks for row-sharded lookups (k > 1 on the mp side)
@@ -362,9 +389,11 @@ class EmbeddingCollection:
                 # no owner-side lookup descriptors, no per-shard partial blocks
                 gl["unique"], gl["unique_owners"] = True, list(pl.shard_gpus)
                 continue
-            # (not for evicting tables: their owners translate the raw keys of the whole bag)
+            # (not for evicting tables: their owners translate the raw keys of the whole bag; not for
+            # weighted lookups: their owners read each key's weight at the key's own position)
             if getattr(self, "shard_split", False) and pl.kind == "mp" and k > 1 and pl.col_factor == 1 \
-                    and gl["combiner"] == "sum" and self.tmap[gl["table"]].evict_strategy is None:
+                    and gl["combiner"] == "sum" and self.tmap[gl["table"]].evict_strategy is None \
+                    and not gl["weighted"]:
                 # Requester-side split: every rank rewrites its bag of a row-sharded table into k
                 # compacted per-shard lists of LOCAL ROW INDICES (key // k) plus their lengths, stored
                 # behind the user keys in the (symmetric) key slab.  A shard owner then reads only
@@ -477,7 +506,8 @@ class EmbeddingCollection:
                             combiner=1 if gl["combiner"] in ("mean", "average") else 0,
                             ev_size=sl["ev"], rows=sl["rows"],
                             nnz_off=(gl["split_nnz_off"] + sl["s"] * b)
-                            if (split and not sl["dynamic"]) else -1))
+                            if (split and not sl["dynamic"]) else -1,
+                            weighted=int(gl["weighted"])))
         self.groups = list(groups.values())
         dev = self.device
         gen = torch.Generator(device="cpu")
@@ -514,7 +544,7 @@ class EmbeddingCollection:
                 if grp.kind == "mp":
                     grp.indexed = dev.type == "cuda" and fused_backward_ok(grp)
                     grp.ws = E.UniqueWorkspace(max(pairs, 1), grp.pitch, dev, indexed=grp.indexed,
-                                               need_scale=any(l.combiner == 1 for l in grp.lookups))
+                                               need_scale=any(l.combiner == 1 or l.weighted for l in grp.lookups))
                 else:
                     n_pad = (n + 4 * self.world - 1) // (4 * self.world) * (4 * self.world)
                     if self.fused and self.world > 1 and not getattr(self.comm, "emulated", False):
@@ -557,6 +587,8 @@ class EmbeddingCollection:
         self.nnz_all = None
         self.key_slab = z(self.key_slab_elems, self.key_dtype)
         self.nnz_slab = z(self.nnz_slab_elems, torch.int32) if self.nnz_slab_elems else None
+        self.weight_slab = z(self.user_key_elems, torch.float32) if self.has_weights else None
+        self.weights_all = None
         if self.fused:
             # Inboxes in the peer-mapped heap, one slot per source rank, same layout as a key / grad
             # slab: requesters scatter their key blocks and gradient rows into them with posted peer
@@ -569,6 +601,10 @@ class EmbeddingCollection:
             if ns:
                 self.nnz_all = sa(W * ns, torch.int32).view(W, ns)
                 self.peer_nnz = self.comm.peer_ptrs(self.nnz_all)
+            if self.has_weights:
+                wn = max(self.user_key_elems, 1)
+                self.weights_all = sa(W * wn, torch.float32).view(W, wn)
+                self.peer_weights_all = self.comm.peer_ptrs(self.weights_all)
             self.out_slab = sa(max(self.out_slab_elems, 1), self.act_dtype)
             self.peer_out = self.comm.peer_ptrs(self.out_slab)
             self.grad_slab = z(self.grad_slab_elems, self.act_dtype) if self.is_train else None
@@ -582,6 +618,8 @@ class EmbeddingCollection:
             self.grad_slab = z(self.grad_slab_elems, self.act_dtype) if self.is_train else None
             if W > 1:
                 self.keys_all = torch.zeros(W, max(self.key_slab_elems, 1), dtype=self.key_dtype, device=dev)
+                if self.has_weights:
+                    self.weights_all = torch.zeros(W, max(self.user_key_elems, 1), dtype=torch.float32, device=dev)
                 if self.nnz_slab is not None:
                     self.nnz_all = torch.zeros(W, self.nnz_slab_elems, dtype=torch.int32, device=dev)
                 self.send_out = torch.zeros(W, max(self.out_slab_elems, 1), dtype=self.act_dtype, device=dev)
@@ -605,10 +643,13 @@ class EmbeddingCollection:
             from .unique_exchange import UniqueExchange
             self._uniq = UniqueExchange(self, uq)
         # named views
-        self.key_views = {}
+        self.key_views, self.weight_views = {}, {}
         for gl in self.glookups:
             self.key_views[gl["bottom"]] = self.key_slab[gl["key_off"]:gl["key_off"] + b * gl["hotness"]] \
                 .view(b, gl["hotness"])
+            if gl["weighted"]:
+                self.weight_views[gl["bottom"]] = self.weight_slab[gl["key_off"]:gl["key_off"] + b * gl["hotness"]] \
+                    .view(b, gl["hotness"])
         self.top_data, self.top_grad = {}, {}
         for tp in self.tops:
             w = tp["width"]
@@ -650,9 +691,22 @@ class EmbeddingCollection:
                                           row_elems=b * H, src_stride=b * H, dst_stride=b * H, dst_rank=g))
         self._key_routes = routes
         self._key_routes_dev = E.routes_to_device(routes, self.device)
+        # the weights of weighted lookups follow their keys' block routes into the weight inboxes
+        wn = max(self.user_key_elems, 1)
+        wroutes = []
+        for gl in self.glookups:
+            if not gl["weighted"]:
+                continue
+            n = b * gl["hotness"]
+            for g in sorted({o[0] for o in self._mp_owners(gl)}):
+                wroutes.append(E.Route(src_off=gl["key_off"], dst_off=me * wn + gl["key_off"], rows=1,
+                                       row_elems=n, src_stride=n, dst_stride=n, dst_rank=g))
+        self._weight_routes = wroutes
+        self._weight_routes_dev = E.routes_to_device(wroutes, self.device)
         # bytes this rank stores into peers per step (roofline accounting)
         kb = self._kb
-        self.dispatch_key_bytes = sum(r.rows * r.row_elems * kb for r in routes if r.dst_rank != me)
+        self.dispatch_key_bytes = sum(r.rows * r.row_elems * kb for r in routes if r.dst_rank != me) + \
+            sum(r.rows * r.row_elems * 4 for r in wroutes if r.dst_rank != me)
 
     def _build_grad_routes(self):
         """Backward push plan: the gradient columns of every model-parallel lookup go to each rank that
@@ -752,6 +806,9 @@ class EmbeddingCollection:
         self.packed = {
             "kn": kn, "kn_me": kn[self.rank], "key_me": kidx[self.rank].to(dev), "key_all": torch.cat(kidx).to(dev),
             "key_recv": torch.zeros(max(self.world * kn[self.rank], 1), dtype=self.key_dtype, device=dev),
+            # the weights of the same key blocks take the same exchange (weighted inputs only)
+            "wgt_recv": torch.zeros(max(self.world * kn[self.rank], 1), dtype=torch.float32, device=dev)
+            if self.has_weights else None,
             "n": n, "n_me": n[self.rank],
             "out_me": oidx[self.rank].to(dev), "out_all": torch.cat(oidx).to(dev),
             "grad_me": gidx[self.rank].to(dev), "grad_all": torch.cat(gidx).to(dev),
@@ -762,6 +819,18 @@ class EmbeddingCollection:
     def set_keys(self, feature_major_keys: torch.Tensor):
         """Copy a whole feature-major key batch into the key slab (H2D lands here directly)."""
         self.key_slab[:feature_major_keys.numel()].copy_(feature_major_keys.reshape(-1), non_blocking=True)
+
+    def set_weights(self, feature_major_weights: torch.Tensor):
+        """Copy the fp32 per-key weights of a batch, in the layout of ``set_keys``, into the weight slab."""
+        self.weight_slab[:feature_major_weights.numel()].copy_(feature_major_weights.reshape(-1), non_blocking=True)
+
+    def _wbufs(self, grp):
+        """per-source-rank weight buffers of a group's launches (None without weighted lookups)"""
+        if not self.has_weights:
+            return None
+        if self.world == 1 or grp.kind == "dp":
+            return [self.weight_slab]
+        return list(self.weights_all.unbind(0))
 
     def forward(self, is_train: bool = True):
         self.forward_begin()
@@ -787,6 +856,9 @@ class EmbeddingCollection:
                 # device barrier (also orders the previous step's readers of these inboxes)
                 E.dispatch(self.key_slab, self._key_routes, self._key_routes_dev, self.peer_keys_all,
                            self.peer_nnz, blocks_x=48)
+                if self._weight_routes:
+                    E.dispatch(self.weight_slab, self._weight_routes, self._weight_routes_dev,
+                               self.peer_weights_all, blocks_x=48)
                 self.comm.barrier_device()
             elif os.environ.get("SKIP_DATA_DISTRIBUTOR", "0") not in ("0", ""):
                 pass          # ablation (model_pipeline.cpp:118): owners keep the keys of an earlier step
@@ -794,6 +866,8 @@ class EmbeddingCollection:
                 self.comm.hier_all_gather(self.keys_all, self.key_slab)
                 if self.nnz_all is not None:
                     self.comm.hier_all_gather(self.nnz_all, self.nnz_slab)
+                if self.weights_all is not None:
+                    self.comm.hier_all_gather(self.weights_all, self.weight_slab)
             elif getattr(self, "packed", None) is not None and self.nnz_all is None:
                 pk = self.packed        # every owner receives only the key blocks of the lookups it serves
                 send = self.key_slab.index_select(0, pk["key_all"])
@@ -801,10 +875,18 @@ class EmbeddingCollection:
                 self.comm.all_to_all_v(recv, send, [pk["kn_me"]] * self.world, pk["kn"])
                 if pk["kn_me"]:
                     self.keys_all.index_copy_(1, pk["key_me"], recv.view(self.world, pk["kn_me"]))
+                if self.weights_all is not None:
+                    wsend = self.weight_slab.index_select(0, pk["key_all"])
+                    wrecv = pk["wgt_recv"][:self.world * pk["kn_me"]]
+                    self.comm.all_to_all_v(wrecv, wsend, [pk["kn_me"]] * self.world, pk["kn"])
+                    if pk["kn_me"]:
+                        self.weights_all.index_copy_(1, pk["key_me"], wrecv.view(self.world, pk["kn_me"]))
             else:
                 self.comm.all_gather(self.keys_all, self.key_slab)
                 if self.nnz_all is not None:
                     self.comm.all_gather(self.nnz_all, self.nnz_slab)
+                if self.weights_all is not None:
+                    self.comm.all_gather(self.weights_all, self.weight_slab)
         if self.has_dynamic:
             self._translate_dynamic_keys()
 
@@ -1023,23 +1105,24 @@ class EmbeddingCollection:
         if self.world == 1:
             for grp in self.groups:
                 E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, [self.key_slab],
-                          [self.out_slab], b, key_bytes=self._kb, act_bf16=self._abf)
+                          [self.out_slab], b, key_bytes=self._kb, act_bf16=self._abf, weight_bufs=self._wbufs(grp))
         elif self.fused:
             for grp in self.groups:
                 if grp.kind == "mp":
                     E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch,
                               list(self.keys_all.unbind(0)), self.peer_out, b, self.rank,
-                              nnz_bufs=self._nnz_bufs(grp), key_bytes=self._kb, act_bf16=self._abf)
+                              nnz_bufs=self._nnz_bufs(grp), key_bytes=self._kb, act_bf16=self._abf,
+                              weight_bufs=self._wbufs(grp))
                 else:
                     E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, [self.key_slab],
-                              [self.out_slab], b, key_bytes=self._kb, act_bf16=self._abf)
+                              [self.out_slab], b, key_bytes=self._kb, act_bf16=self._abf, weight_bufs=self._wbufs(grp))
         else:
             self.send_out.zero_()
             for grp in self.groups:
                 if grp.kind == "mp" and grp.lookups:
                     E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch,
                               list(self.keys_all.unbind(0)), list(self.send_out.unbind(0)), b, self.rank,
-                              nnz_bufs=self._nnz_bufs(grp))
+                              nnz_bufs=self._nnz_bufs(grp), weight_bufs=self._wbufs(grp))
 
     def forward_end(self):
         b = self.b
@@ -1064,7 +1147,7 @@ class EmbeddingCollection:
                 for grp in self.groups:
                     if grp.kind == "dp":
                         E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, [self.key_slab],
-                                  [self.out_slab], b)
+                                  [self.out_slab], b, weight_bufs=self._wbufs(grp))
         if getattr(self, "_uniq", None) is not None:
             self._uniq.forward()
         self._reduce_partials()
@@ -1074,14 +1157,21 @@ class EmbeddingCollection:
         """Mean-combined bags may be shorter than the maximum hotness (padding keys are -1): the lookup
         kernels divide by the maximum hotness, the requester -- who owns the keys -- rescales its
         pooled vectors (forward) / their gradients (backward) by hotness / (number of valid keys), i.e.
-        the mean is over the actual bag like the reference's bucket ranges."""
+        the mean is over the actual bag like the reference's bucket ranges.  A weighted bag takes
+        hotness / (sum of the valid keys' weights), with 1 for a sum of exactly 0; all-ones weights sum to
+        the count exactly, so they rescale as the unweighted bag does."""
         for gi, gl in enumerate(self.glookups):
-            if gl["combiner"] not in ("mean", "average") or gl["hotness"] <= 1:
+            if gl["combiner"] not in ("mean", "average") or (gl["hotness"] <= 1 and not gl["weighted"]):
                 continue
             tp = self.tops[gl["top"]]
             if forward:
                 keys = self.key_views[gl["bottom"]]
-                cnt = (keys >= 0).sum(1).clamp(min=1).to(torch.float32)
+                if gl["weighted"]:
+                    w = torch.where(keys >= 0, self.weight_views[gl["bottom"]], torch.zeros((), device=keys.device))
+                    sw = w.sum(1)
+                    cnt = torch.where(sw == 0, torch.ones_like(sw), sw)
+                else:
+                    cnt = (keys >= 0).sum(1).clamp(min=1).to(torch.float32)
                 self._mean_factor = getattr(self, "_mean_factor", {})
                 self._mean_factor[gi] = (float(gl["hotness"]) / cnt).unsqueeze(1)
                 t2d = self.top_data[tp["name"]].reshape(self.b, -1) if not tp.get("alias") \
@@ -1121,7 +1211,8 @@ class EmbeddingCollection:
             if grp.kind == "mp" and getattr(grp, "indexed", False) and grp.lookups:
                 kb, _ = self._bwd_bufs(grp)
                 E.bwd_index(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, kb, self.b, grp.ws,
-                            self.rank, nnz_bufs=self._nnz_bufs(grp), key_bytes=self._kb)
+                            self.rank, nnz_bufs=self._nnz_bufs(grp), key_bytes=self._kb,
+                            weight_bufs=self._wbufs(grp))
         self._index_done = True
 
     def backward(self, lr_t, step_t, dp_stream=None):
@@ -1199,13 +1290,14 @@ class EmbeddingCollection:
         elif grp.kind == "mp":
             E.backward_accum(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, key_bufs, grad_bufs,
                              self.b, grp.ws, 1.0, self.rank, nnz_bufs=self._nnz_bufs(grp),
-                             key_bytes=self._kb, act_bf16=self._abf)
+                             key_bytes=self._kb, act_bf16=self._abf, weight_bufs=self._wbufs(grp))
             E.update(o.optimizer_type, grp.table, grp.s0, grp.s1, grp.pitch, grp.ws, self._hp(o),
                      lr_t, step_t)
         else:
             from ..ops import dense as D
             E.backward_accum(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, key_bufs, grad_bufs,
-                             self.b, None, 1.0, self.rank, dense_wgrad=grp.dense_wgrad)
+                             self.b, None, 1.0, self.rank, dense_wgrad=grp.dense_wgrad,
+                             weight_bufs=self._wbufs(grp))
             if self.world > 1:
                 if grp.p2p_ar is not None:
                     grp.p2p_ar.run()

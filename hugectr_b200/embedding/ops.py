@@ -1,8 +1,9 @@
 """Embedding kernels: ctypes bindings for csrc/embedding.cu + PyTorch reference implementations.
 
 The reference implementations define the semantics (they are the CPU path and the test oracle):
-  forward   pooled[src, lookup, sample] = combiner( table[row_off + key // k] for owned keys )
-  backward  per unique arena row: g = sum of bucket gradients (scaled 1/nnz for mean);
+  forward   pooled[src, lookup, sample] = combiner( w * table[row_off + key // k] for owned keys ),
+            w the key's weight for a weighted lookup, else 1
+  backward  per unique arena row: g = sum of bucket gradients times w (scaled 1/nnz for mean);
             then the sparse optimizer of Appendix A.3 on that row.
 """
 from __future__ import annotations
@@ -27,7 +28,7 @@ class CEmbLookup(C.Structure):
                 ("nnz_off", C.c_longlong), ("out_off", C.c_longlong), ("grad_off", C.c_longlong),
                 ("hotness", C.c_int), ("key_stride", C.c_int), ("num_shards", C.c_int),
                 ("shard_idx", C.c_int), ("out_stride", C.c_int), ("grad_stride", C.c_int),
-                ("combiner", C.c_int), ("ev_size", C.c_int), ("rows", C.c_int), ("pad_", C.c_int),
+                ("combiner", C.c_int), ("ev_size", C.c_int), ("rows", C.c_int), ("weighted", C.c_int),
                 ("pair_off", C.c_longlong)]
 
 
@@ -36,7 +37,7 @@ class CEmbParams(C.Structure):
                 ("num_lookups", C.c_int), ("keys", C.c_void_p * MAX_RANKS),
                 ("nnz", C.c_void_p * MAX_RANKS), ("out", C.c_void_p * MAX_RANKS),
                 ("grad", C.c_void_p * MAX_RANKS), ("lookups", C.c_void_p), ("table", C.c_void_p),
-                ("ev_size", C.c_int)]
+                ("ev_size", C.c_int), ("weights", C.c_void_p * MAX_RANKS)]
 
 
 class CUniqueTable(C.Structure):
@@ -110,12 +111,13 @@ class LookupDesc:
     rows: int
     nnz_off: int = -1
     pair_off: int = 0
+    weighted: int = 0    # 1: every key has an fp32 weight at the same element offset of the weight buffers
 
     def to_c(self) -> CEmbLookup:
         return CEmbLookup(self.table_row_off, self.key_off, self.nnz_off, self.out_off,
                           self.grad_off, self.hotness, self.key_stride, self.num_shards,
                           self.shard_idx, self.out_stride, self.grad_stride, self.combiner,
-                          self.ev_size, self.rows, 0, self.pair_off)
+                          self.ev_size, self.rows, int(self.weighted), self.pair_off)
 
 
 def lookups_to_device(lookups: List[LookupDesc], device) -> torch.Tensor:
@@ -274,12 +276,33 @@ def dispatch(src: torch.Tensor, routes: List[Route], routes_dev, dst_bufs, nnz_b
 
 
 # ----------------------------------------------------------------------------- forward
+def _weight_ptrs(p, lookups, weight_bufs):
+    """per-source-rank weight pointers of a launch with a weighted lookup (left null otherwise: the
+    kernels' unweighted instantiations)"""
+    if weight_bufs is None or not any(l.weighted for l in lookups):
+        return
+    for r, w in enumerate(weight_bufs):
+        p.weights[r] = w if isinstance(w, int) else w.data_ptr()
+
+
+def _key_weights(lk, weight_bufs, src, batch, own):
+    """[batch, hotness] fp32 weights of the owned keys of lookup ``lk`` (1 for an unweighted lookup,
+    0 where a key is not owned, whatever the stored weight)"""
+    if not lk.weighted:
+        return own.float()
+    wbuf = weight_bufs[src].reshape(-1)
+    w = torch.as_strided(wbuf, (batch, lk.hotness), (lk.key_stride, 1), wbuf.storage_offset() + lk.key_off)
+    return torch.where(own, w.float(), torch.zeros((), device=w.device))
+
+
 def forward(lookups, lookups_dev, table, ev_pitch, key_bufs, out_bufs, batch, my_rank=0,
-            nnz_bufs=None, key_bytes=4, act_bf16=True):
-    """key_bufs / out_bufs: one entry per source rank (tensor, or int device pointer for peers)."""
+            nnz_bufs=None, key_bytes=4, act_bf16=True, weight_bufs=None):
+    """key_bufs / out_bufs (/ weight_bufs, fp32 per-key weights of weighted lookups): one entry per
+    source rank (tensor, or int device pointer for peers)."""
     R = len(key_bufs)
     if table.is_cuda:
         p = CEmbParams()
+        _weight_ptrs(p, lookups, weight_bufs)
         p.num_ranks, p.my_rank, p.batch, p.num_lookups = R, my_rank, batch, len(lookups)
         kb = key_bytes
         out_bf16 = int(act_bf16)
@@ -306,7 +329,7 @@ def forward(lookups, lookups_dev, table, ev_pitch, key_bufs, out_bufs, batch, my
             raise RuntimeError(f"hctr_emb_forward failed rc={rc}")
         D._count()
         return
-    forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs)
+    forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs, weight_bufs)
 
 
 def _owned(lk: LookupDesc, keys):
@@ -319,7 +342,7 @@ def _owned(lk: LookupDesc, keys):
     return own, lk.table_row_off + torch.where(own, r, torch.zeros_like(r))
 
 
-def forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs=None):
+def forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs=None, weight_bufs=None):
     tab = table.view(-1, ev_pitch)
     for src in range(len(key_bufs)):
         kbuf, obuf = key_bufs[src].reshape(-1), out_bufs[src].reshape(-1)
@@ -331,7 +354,7 @@ def forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_b
             if lk.nnz_off >= 0 and nnz_bufs is not None:
                 nnz = nnz_bufs[src].reshape(-1)[lk.nnz_off:lk.nnz_off + batch].long().clamp(max=lk.hotness)
                 own &= torch.arange(lk.hotness, device=keys.device).view(1, -1) < nnz.view(-1, 1)
-            v = tab[rows][..., :lk.ev_size].float() * own.unsqueeze(-1)
+            v = tab[rows][..., :lk.ev_size].float() * _key_weights(lk, weight_bufs, src, batch, own).unsqueeze(-1)
             pooled = v.sum(1)
             if lk.combiner == 1:
                 pooled = pooled / nnz.clamp(min=1).view(-1, 1).float()
@@ -432,11 +455,13 @@ def check_workspace_overflow(ws, what: str):
 
 
 def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch, ws, grad_scale=1.0,
-                   my_rank=0, nnz_bufs=None, dense_wgrad=None, key_bytes=4, act_bf16=True):
-    """Accumulate bucket gradients per unique row (or into a dense wgrad for DP tables)."""
+                   my_rank=0, nnz_bufs=None, dense_wgrad=None, key_bytes=4, act_bf16=True, weight_bufs=None):
+    """Accumulate bucket gradients (times the key's weight for weighted lookups) per unique row (or
+    into a dense wgrad for DP tables)."""
     R = len(key_bufs)
     if table.is_cuda:
         p = CEmbParams()
+        _weight_ptrs(p, lookups, weight_bufs)
         p.num_ranks, p.my_rank, p.batch, p.num_lookups = R, my_rank, batch, len(lookups)
         kb, gbf = key_bytes, int(act_bf16)
         for r in range(R):
@@ -484,7 +509,10 @@ def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, b
             g = g.float() * grad_scale
             if lk.combiner == 1:
                 g = g / nnz.clamp(min=1).view(-1, 1).float()
-            gg = g.unsqueeze(1).expand(batch, lk.hotness, lk.ev_size)[own]
+            gg = g.unsqueeze(1).expand(batch, lk.hotness, lk.ev_size)
+            if lk.weighted:
+                gg = gg * _key_weights(lk, weight_bufs, src, batch, own).unsqueeze(-1)
+            gg = gg[own]
             if lk.ev_size < ev_pitch:
                 gg = torch.nn.functional.pad(gg, (0, ev_pitch - lk.ev_size))
             rows_all.append(rows[own])
@@ -663,9 +691,10 @@ def gather_rows(table, ev_pitch, rows, out):
 
 
 def _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch, my_rank, nnz_bufs,
-                 key_bytes=4, act_bf16=True):
+                 key_bytes=4, act_bf16=True, weight_bufs=None):
     R = len(key_bufs)
     p = CEmbParams()
+    _weight_ptrs(p, lookups, weight_bufs)
     p.num_ranks, p.my_rank, p.batch, p.num_lookups = R, my_rank, batch, len(lookups)
     kb, gbf = key_bytes, int(act_bf16)
     for r in range(R):
@@ -688,14 +717,17 @@ def _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, bat
 
 
 def bwd_index(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, ws, my_rank=0, nnz_bufs=None,
-              key_bytes=4):
-    """Gradient-independent part of the backward: unique rows + per-row bucket lists."""
+              key_bytes=4, weight_bufs=None):
+    """Gradient-independent part of the backward: unique rows + per-row bucket lists (with the
+    per-entry scales: 1/nnz of mean bags, times the key's weight of weighted lookups)."""
     check_ev_size(ev_pitch)
     if not vec4_aligned(lookups, ev_pitch, [table], grad=True):
         raise ValueError("the fused backward needs 4-element aligned gradient rows and pitch "
                          "(see vec4_aligned); use backward_accum + update")
+    if any(l.weighted for l in lookups) and (weight_bufs is None or ws.bucket_scale is None):
+        raise ValueError("weighted lookups need their weight buffers and a workspace built with need_scale")
     p, kb, _ = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, None, batch, my_rank,
-                            nnz_bufs, key_bytes)
+                            nnz_bufs, key_bytes, weight_bufs=weight_bufs)
     total_pairs = len(key_bufs) * batch * sum(l.hotness for l in lookups)
     rc = lib().hctr_emb_bwd_index(C.byref(p), C.byref(ws.c), C.byref(ws.ix), total_pairs, kb,
                                   _st(table.device))

@@ -44,6 +44,10 @@ class InferenceModel:
                                   check_type=Check_t.Non)
         self.model = Model(solver, reader, OptParamsPy(), comm=Comm.single(dev))
         self.model.construct_from_json(model_config_path)
+        weighted = [p.top_name for p in self.model.input.data_reader_sparse_param_array if getattr(p, "weighted", False)]
+        if weighted:
+            # predict() takes keys only: the weights of these inputs would be dropped
+            raise ValueError(f"weighted input {weighted[0]}: the inference session does not take per-key weights")
         self.model.compile()
         if params.dense_model_file:
             self.model.load_dense_weights(params.dense_model_file)

@@ -175,9 +175,26 @@ class Model:
         out.shard_matrix, out._layout_applied = rows, True
         return out
 
+    def _check_weighted_inputs(self):
+        """Weighted sparse inputs need a reader that delivers weights and embeddings that pool them."""
+        from .enums import DataReaderType_t
+        weighted = [p.top_name for p in self.input.data_reader_sparse_param_array if getattr(p, "weighted", False)]
+        if not weighted:
+            return
+        t = self.reader_params.data_reader_type
+        if t in (DataReaderType_t.Norm, DataReaderType_t.Raw, DataReaderType_t.RawAsync):
+            raise ValueError(f"weighted input {weighted[0]}: the {t.name} data format has no weights")
+        for se in self.sparse_embeddings:
+            if se.bottom_name in weighted:
+                raise ValueError(f"weighted input {se.bottom_name}: the legacy SparseEmbedding "
+                                 f"{getattr(se, 'sparse_embedding_name', '')} cannot pool weights "
+                                 "(use an EmbeddingCollection lookup)")
+
     def _build_embeddings(self):
         s = self.solver
+        self._check_weighted_inputs()
         hot = {p.top_name: max(p.nnz_per_slot) for p in self.input.data_reader_sparse_param_array}
+        weighted = {p.top_name for p in self.input.data_reader_sparse_param_array if getattr(p, "weighted", False)}
         self.ebcs_train, self.ebcs_eval = [], []
         state_dtype = torch.float32
         if os.environ.get("HCTR_EMB_STATE_BF16", "0") == "1":
@@ -195,7 +212,7 @@ class Model:
                                     self.opt_params, self.key_dtype,
                                     scaler=s.scaler if self.mixed else 1.0, state_dtype=state_dtype,
                                     seed=s.seed,
-                                    fused=None if s.fused_embedding_comm else False)
+                                    fused=None if s.fused_embedding_comm else False, weighted=weighted)
             self.ebcs_train.append(e)
             self.ebcs_eval.append(e.eval_clone(self.b_eval))
         self.legacy_train, self.legacy_eval = [], []
@@ -347,6 +364,8 @@ class Model:
         legs = self.legacy_train if is_train else self.legacy_eval
         if len(ebcs) == 1 and not legs:
             ebcs[0].set_keys(hb.keys)
+            if ebcs[0].has_weights:
+                ebcs[0].set_weights(hb.weights)
         else:
             b = self.b_train if is_train else self.b_eval
             offs, _ = self.layout.key_block_offsets(b)
@@ -355,6 +374,9 @@ class Model:
                     o = offs[gl["bottom"]]
                     e.key_views[gl["bottom"]].copy_(
                         hb.keys[o:o + b * gl["hotness"]].view(b, gl["hotness"]), non_blocking=nb)
+                    if gl["weighted"]:
+                        e.weight_views[gl["bottom"]].copy_(
+                            hb.weights[o:o + b * gl["hotness"]].view(b, gl["hotness"]), non_blocking=nb)
             for rt in legs:
                 rt.set_keys(hb, offs, self.layout.nnz_block_offsets(b)[0])
         hb.mark_copied()
@@ -674,6 +696,8 @@ class Model:
             self._stg = {"label": torch.empty_like(self.net_train.tensors[self.input.label_name].data),
                          "dense": torch.empty_like(self.net_train.tensors[self.input.dense_name].data),
                          "keys": torch.empty_like(self.ebcs_train[0].key_slab)}
+            if self.ebcs_train[0].has_weights:
+                self._stg["weights"] = torch.empty_like(self.ebcs_train[0].weight_slab)
             self._stg_free = torch.cuda.Event()
             self._stg_free.record()
         cs = self._copy_stream
@@ -692,6 +716,8 @@ class Model:
             if self.input.dense_dim > 0:
                 self._stg["dense"].copy_(hb.dense, non_blocking=True)
             self._stg["keys"][:hb.keys.numel()].copy_(hb.keys, non_blocking=True)
+            if "weights" in self._stg:
+                self._stg["weights"][:hb.weights.numel()].copy_(hb.weights, non_blocking=True)
             hb.mark_copied()
         self._staged = hb
 
@@ -703,6 +729,8 @@ class Model:
         if self.input.dense_dim > 0:
             net.tensors[self.input.dense_name].data.copy_(self._stg["dense"], non_blocking=True)
         self.ebcs_train[0].key_slab.copy_(self._stg["keys"], non_blocking=True)
+        if "weights" in self._stg:
+            self.ebcs_train[0].weight_slab.copy_(self._stg["weights"], non_blocking=True)
         self._stg_free.record(main)
         self._staged = None
 

@@ -310,6 +310,9 @@ def convert(onnx_model_path: str, graph_config: str, dense_model: str, convert_e
     dense = torch.zeros(batch_size, data["dense"]["dense_dim"])
     extras = []
     sp = {s["top"]: s for s in data.get("sparse", [])}
+    for s in sp.values():
+        if s.get("weighted"):
+            raise ValueError(f"weighted input {s['top']}: the ONNX export does not carry per-key weights")
     for l in g.emb_layers:
         s = sp[l["bottom"]]
         nnz = s["nnz_per_slot"]

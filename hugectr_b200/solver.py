@@ -189,8 +189,11 @@ def CreateOptimizer(optimizer_type=Optimizer_t.Adam, update_type=Update_t.Global
 # --------------------------------------------------------------------------- data reader params
 class DataReaderSparseParam:
     def __init__(self, top_name: str, nnz_per_slot: Union[int, Sequence[int]],
-                 is_fixed_length: bool, slot_num: int):
+                 is_fixed_length: bool, slot_num: int, weighted: bool = False):
+        """``weighted``: the reader delivers an fp32 weight with every key of this input, and every
+        embedding lookup of it pools weighted (see docs/embedding.md)."""
         self.top_name = top_name
+        self.weighted = bool(weighted)
         if isinstance(nnz_per_slot, int):
             self.nnz_per_slot = [nnz_per_slot] * slot_num
         else:
@@ -206,7 +209,8 @@ class DataReaderSparseParam:
         return {"top": self.top_name, "type": "DistributedSlot",
                 "nnz_per_slot": self.nnz_per_slot if len(set(self.nnz_per_slot)) > 1
                 else self.nnz_per_slot[0],
-                "is_fixed_length": self.is_fixed_length, "slot_num": self.slot_num}
+                "is_fixed_length": self.is_fixed_length, "slot_num": self.slot_num,
+                **({"weighted": True} if self.weighted else {})}
 
 
 @dataclass
