@@ -538,48 +538,6 @@ extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, i
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
-// Requester-side split of a row-sharded bag: one warp per sample compacts, for every shard j, the
-// local row indices (key / k) of the keys with key % k == j (original order), pads with -1 and
-// writes the list length.  out: [k, batch, hotness], nnz: [k, batch].
-template <typename KeyT>
-__global__ void __launch_bounds__(256)
-    emb_shard_split_kernel(const KeyT* __restrict__ keys, KeyT* __restrict__ out, int* __restrict__ nnz,
-                           const int batch, const int hotness, const int k) {
-  const int lane = threadIdx.x & 31;
-  const int warps = (gridDim.x * blockDim.x) >> 5;
-  for (int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; s < batch; s += warps) {
-    const KeyT* kb = keys + static_cast<long long>(s) * hotness;
-    for (int j = 0; j < k; ++j) {
-      KeyT* ob = out + (static_cast<long long>(j) * batch + s) * hotness;
-      int pos = 0;
-      for (int h0 = 0; h0 < hotness; h0 += 32) {
-        const int h = h0 + lane;
-        long long key = -1;
-        if (h < hotness) key = static_cast<long long>(kb[h]);
-        const bool match = key >= 0 && (key % k) == j;
-        const unsigned bal = __ballot_sync(0xffffffffu, match);
-        if (match) ob[pos + __popc(bal & ((1u << lane) - 1u))] = static_cast<KeyT>(key / k);
-        pos += __popc(bal);
-      }
-      for (int h = pos + lane; h < hotness; h += 32) ob[h] = static_cast<KeyT>(-1);
-      if (lane == 0) nnz[j * batch + s] = pos;
-    }
-  }
-}
-
-extern "C" int hctr_emb_shard_split(const void* keys, void* out, int* nnz, int batch, int hotness,
-                                    int k, int key_bytes, void* stream_) {
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
-  if (batch <= 0 || hotness <= 0 || k <= 1) return 0;
-  const int blocks = (batch * 32 + 255) / 256;
-  with_key(key_bytes, [&](auto kt) {
-    using KeyT = type_of<decltype(kt)>;
-    emb_shard_split_kernel<KeyT><<<blocks, 256, 0, st>>>(
-        reinterpret_cast<const KeyT*>(keys), reinterpret_cast<KeyT*>(out), nnz, batch, hotness, k);
-  });
-  return cudaGetLastError() == cudaSuccess ? 0 : -1;
-}
-
 extern "C" int hctr_emb_backward_accum(const EmbParams* p, const UniqueTable* ut,
                                        float* wgrad_unique, float grad_scale, int max_ev,
                                        int key_bytes, int grad_bf16, int dp_ev4, void* stream_) {

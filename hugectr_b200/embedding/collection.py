@@ -11,8 +11,8 @@ keys / EBC outputs / EBC top-grads in *slabs* with identical layout on all ranks
 the slabs live in a peer-mapped symmetric heap and the owner-side kernels read the requesters' keys
 and write their outputs (and read their gradients) directly over NVLink, so no NCCL all-to-all runs
 on the forward or backward path.  In ``collective`` mode (CPU/gloo tests and the NCCL baseline the
-fused path is measured against) the same local kernels run on all-gathered keys and the pooled
-vectors travel through ``all_to_all_single``.
+fused path is measured against) the same local kernels run on the key blocks each owner received and
+the pooled vectors travel through variable-size all-to-alls.
 """
 from __future__ import annotations
 
@@ -213,6 +213,31 @@ class _Group:
         return 1 if self.rowwise else self.pitch
 
 
+@dataclass
+class _KeyChannel:
+    """One key-side buffer (the keys, or the fp32 weights of weighted lookups) and its exchange: the
+    owners read row r of ``all`` as rank r's copy of ``slab``."""
+    slab: torch.Tensor
+    all: Optional[torch.Tensor] = None         # [world, n]
+    peers: Optional[list] = None               # peer-memory path: every rank's ``all`` (the inboxes)
+    routes: Optional[list] = None              # peer-memory path: this rank's dispatch plan
+    routes_dev: Optional[torch.Tensor] = None
+    nnz_all: Optional[torch.Tensor] = None     # keys on the peer-memory path: [world, nnz_slab_elems]
+    nnz_peers: Optional[list] = None           # split lengths, written by the key dispatch
+    recv: Optional[torch.Tensor] = None        # packed collective exchange: blocks from every rank
+
+
+@dataclass
+class _SourceBufs:
+    """What a group's kernels read and write, one entry per source rank whose batch they serve (this
+    rank alone for data-parallel groups and single-GPU jobs)."""
+    keys: list
+    out: list
+    grads: Optional[list]
+    nnz: Optional[list]
+    weights: Optional[list]
+
+
 def fused_backward_ok(grp: _Group) -> bool:
     """Whether a model-parallel group may use the fused index + reduce/update backward: it locates
     gradient rows in 4-element units, so every lookup's gradient columns must be 4-aligned (a top
@@ -252,11 +277,8 @@ class EmbeddingCollection:
         self.native = device.type == "cuda"
         self.has_dynamic = any(t.dynamic for t in self.tables)
         self.fused = (self.native and self.world > 1 and comm.p2p_available) if fused is None else fused
-        # requester-side split of row-sharded bags (see _build_layout): part of the key dispatch on the
-        # fused path (default on there, HCTR_SHARD_SPLIT=0 disables); opt-in on the collective path
-        import os as _os
-        ss = _os.environ.get("HCTR_SHARD_SPLIT", "")
-        self.shard_split = self.world > 1 and (ss == "1" or (ss != "0" and bool(self.fused)))
+        # requester-side split of row-sharded bags (see _build_layout): part of the fused key dispatch
+        self.shard_split = self.world > 1 and bool(self.fused)
         # dynamic tables translate keys with a device hash table and flag overflow on the device: the
         # step has no host sync (graph capturable); check_overflow() reads the flags on demand
         self.dynamic_graph_safe = True
@@ -583,51 +605,64 @@ class EmbeddingCollection:
     def _alloc_buffers(self):
         dev, b, W = self.device, self.b, self.world
         z = lambda n, dt: torch.zeros(max(int(n), 1), dtype=dt, device=dev)
-        self.peer_nnz = None
-        self.nnz_all = None
         self.key_slab = z(self.key_slab_elems, self.key_dtype)
-        self.nnz_slab = z(self.nnz_slab_elems, torch.int32) if self.nnz_slab_elems else None
         self.weight_slab = z(self.user_key_elems, torch.float32) if self.has_weights else None
-        self.weights_all = None
+        # the key-side channels: the keys (whose peer-memory dispatch also writes the split lengths), then
+        # the weights of weighted lookups, which follow their keys' blocks
+        self.key_chans = [_KeyChannel(self.key_slab)]
+        if self.has_weights:
+            self.key_chans.append(_KeyChannel(self.weight_slab))
+        self.grads_all = None
         if self.fused:
             # Inboxes in the peer-mapped heap, one slot per source rank, same layout as a key / grad
             # slab: requesters scatter their key blocks and gradient rows into them with posted peer
             # stores (csrc/emb_dispatch.cu); owners write pooled vectors into the requesters' out slabs.
             # Every owner-side kernel then reads LOCAL memory only.
             sa = self.comm.symm_alloc
-            ks, ns, gs = max(self.key_slab_elems, 1), self.nnz_slab_elems, max(self.grad_slab_elems, 1)
-            self.keys_all = sa(W * ks, self.key_dtype).view(W, ks)
-            self.peer_keys_all = self.comm.peer_ptrs(self.keys_all)
-            if ns:
-                self.nnz_all = sa(W * ns, torch.int32).view(W, ns)
-                self.peer_nnz = self.comm.peer_ptrs(self.nnz_all)
-            if self.has_weights:
-                wn = max(self.user_key_elems, 1)
-                self.weights_all = sa(W * wn, torch.float32).view(W, wn)
-                self.peer_weights_all = self.comm.peer_ptrs(self.weights_all)
+            for ch in self.key_chans:
+                n = ch.slab.numel()
+                ch.all = sa(W * n, ch.slab.dtype).view(W, n)
+                ch.peers = self.comm.peer_ptrs(ch.all)
+            if self.nnz_slab_elems:
+                ns, kc = self.nnz_slab_elems, self.key_chans[0]
+                kc.nnz_all = sa(W * ns, torch.int32).view(W, ns)
+                kc.nnz_peers = self.comm.peer_ptrs(kc.nnz_all)
             self.out_slab = sa(max(self.out_slab_elems, 1), self.act_dtype)
             self.peer_out = self.comm.peer_ptrs(self.out_slab)
             self.grad_slab = z(self.grad_slab_elems, self.act_dtype) if self.is_train else None
             if self.is_train:
+                gs = max(self.grad_slab_elems, 1)
                 self.grads_all = sa(W * gs, self.act_dtype).view(W, gs)
                 self.peer_grads_all = self.comm.peer_ptrs(self.grads_all)
-            self._build_key_routes()
+            for ch, routes in zip(self.key_chans, self._build_key_routes(self.rank)):
+                ch.routes, ch.routes_dev = routes, E.routes_to_device(routes, dev)
+            # bytes this rank stores into peers per step (roofline accounting)
+            self.dispatch_key_bytes = sum(r.rows * r.row_elems * ch.slab.element_size()
+                                          for ch in self.key_chans for r in ch.routes if r.dst_rank != self.rank)
             self._grad_routes = None
         else:
             self.out_slab = z(self.out_slab_elems, self.act_dtype)
             self.grad_slab = z(self.grad_slab_elems, self.act_dtype) if self.is_train else None
             if W > 1:
-                self.keys_all = torch.zeros(W, max(self.key_slab_elems, 1), dtype=self.key_dtype, device=dev)
-                if self.has_weights:
-                    self.weights_all = torch.zeros(W, max(self.user_key_elems, 1), dtype=torch.float32, device=dev)
-                if self.nnz_slab is not None:
-                    self.nnz_all = torch.zeros(W, self.nnz_slab_elems, dtype=torch.int32, device=dev)
+                for ch in self.key_chans:
+                    ch.all = torch.zeros(W, ch.slab.numel(), dtype=ch.slab.dtype, device=dev)
                 self.send_out = torch.zeros(W, max(self.out_slab_elems, 1), dtype=self.act_dtype, device=dev)
-                self.recv_out = torch.zeros_like(self.send_out)
                 if self.is_train:
                     self.grads_all = torch.zeros(W, max(self.grad_slab_elems, 1), dtype=self.act_dtype,
                                                  device=dev)
-                self._build_packed_exchange()
+                if not self.hier:
+                    self._build_packed_exchange()
+        rows = lambda t: None if t is None else list(t.unbind(0))
+        for grp in self.groups:
+            if W == 1 or grp.kind == "dp":
+                grp.src = _SourceBufs([self.key_slab], [self.out_slab],
+                                      None if self.grad_slab is None else [self.grad_slab], None,
+                                      None if self.weight_slab is None else [self.weight_slab])
+            else:
+                kc = self.key_chans[0]
+                grp.src = _SourceBufs(rows(kc.all), self.peer_out if self.fused else rows(self.send_out),
+                                      rows(self.grads_all), rows(kc.nnz_all),
+                                      rows(self.key_chans[1].all) if self.has_weights else None)
         # evicting tables: the ways admitted by one step (at most one per key position), re-initialised
         # after the table's last insert
         self._evict_adm = {}
@@ -666,47 +701,28 @@ class EmbeddingCollection:
         kk = len(pl.shard_gpus) // pl.col_factor
         return [(g, idx // kk, kk, idx % kk) for idx, g in enumerate(pl.shard_gpus)]
 
-    def _build_key_routes(self):
-        """Forward dispatch plan of THIS rank's batch: per model-parallel lookup one route per owner --
-        the whole key block, or (row-sharded, split on) the owner's compacted shard list + lengths."""
-        b, me = self.b, self.rank
-        ks, ns = max(self.key_slab_elems, 1), self.nnz_slab_elems
-        routes = []
+    def _build_key_routes(self, me):
+        """Forward dispatch plan of rank ``me``'s batch, one route list per key-side channel: per
+        model-parallel lookup one route per owner -- the whole block of keys (and of their weights), or
+        (row-sharded, peer-memory path) the owner's compacted shard list + lengths."""
+        b = self.b
+        ks, ns, wn = max(self.key_slab_elems, 1), self.nnz_slab_elems, max(self.user_key_elems, 1)
+        keys, weights = [], []
         for gl in self.glookups:
-            H = gl["hotness"]
-            seen = set()
-            for (g, cpart, kk, s_) in self._mp_owners(gl):
-                if "split_off" in gl:
-                    if (g, s_) in seen:
-                        continue
-                    seen.add((g, s_))
-                    routes.append(E.Route(src_off=gl["key_off"], dst_off=me * ks + gl["split_off"] + s_ * b * H,
-                                          rows=b, row_elems=H, src_stride=H, dst_stride=H, dst_rank=g, kind=1,
-                                          k=kk, shard=s_, nnz_off=me * ns + gl["split_nnz_off"] + s_ * b))
-                else:
-                    if g in seen:
-                        continue
-                    seen.add(g)
-                    routes.append(E.Route(src_off=gl["key_off"], dst_off=me * ks + gl["key_off"], rows=1,
-                                          row_elems=b * H, src_stride=b * H, dst_stride=b * H, dst_rank=g))
-        self._key_routes = routes
-        self._key_routes_dev = E.routes_to_device(routes, self.device)
-        # the weights of weighted lookups follow their keys' block routes into the weight inboxes
-        wn = max(self.user_key_elems, 1)
-        wroutes = []
-        for gl in self.glookups:
-            if not gl["weighted"]:
+            H, n, off = gl["hotness"], b * gl["hotness"], gl["key_off"]
+            if "split_off" in gl:
+                for (g, _, kk, s_) in self._mp_owners(gl):
+                    keys.append(E.Route(src_off=off, dst_off=me * ks + gl["split_off"] + s_ * b * H, rows=b,
+                                        row_elems=H, src_stride=H, dst_stride=H, dst_rank=g, kind=1, k=kk,
+                                        shard=s_, nnz_off=me * ns + gl["split_nnz_off"] + s_ * b))
                 continue
-            n = b * gl["hotness"]
             for g in sorted({o[0] for o in self._mp_owners(gl)}):
-                wroutes.append(E.Route(src_off=gl["key_off"], dst_off=me * wn + gl["key_off"], rows=1,
-                                       row_elems=n, src_stride=n, dst_stride=n, dst_rank=g))
-        self._weight_routes = wroutes
-        self._weight_routes_dev = E.routes_to_device(wroutes, self.device)
-        # bytes this rank stores into peers per step (roofline accounting)
-        kb = self._kb
-        self.dispatch_key_bytes = sum(r.rows * r.row_elems * kb for r in routes if r.dst_rank != me) + \
-            sum(r.rows * r.row_elems * 4 for r in wroutes if r.dst_rank != me)
+                keys.append(E.Route(src_off=off, dst_off=me * ks + off, rows=1, row_elems=n, src_stride=n,
+                                    dst_stride=n, dst_rank=g))
+                if gl["weighted"]:
+                    weights.append(E.Route(src_off=off, dst_off=me * wn + off, rows=1, row_elems=n,
+                                           src_stride=n, dst_stride=n, dst_rank=g))
+        return [keys, weights] if self.has_weights else [keys]
 
     def _build_grad_routes(self):
         """Backward push plan: the gradient columns of every model-parallel lookup go to each rank that
@@ -737,7 +753,7 @@ class EmbeddingCollection:
         if not getattr(self, "alias_reserve", 0) or name not in self.alias_out_off:
             return None
         if self.world > 1 and not self.fused:
-            return None                       # the collective path ships whole slabs
+            return None                       # the collective exchanges are planned over the slab layout
         tp = [t for t in self.tops if t["name"] == name][0]
         w, b = tp["width"], self.b
         esz = 2 if self.act_dtype == torch.bfloat16 else 4
@@ -772,15 +788,12 @@ class EmbeddingCollection:
                 for tp in self.tops}
 
     def _build_packed_exchange(self):
-        """Collective (NCCL / gloo) path: every element of a requester's output slab is produced by
-        exactly one owner, and an owner needs only the gradient columns of its own lookups.  Instead
-        of shipping whole slabs (all-to-all of ``world`` full slabs forward, all-gather of full gradient
-        slabs backward -- ``world`` times the useful bytes) the owners' regions are packed: rank o sends
-        requester r the ``n_o`` elements it owns, r returns the ``n_o`` matching gradient elements.
-        The region lists are exchanged once here; ``HCTR_PACKED_EXCHANGE=0`` keeps the full-slab path."""
-        self.packed = None
-        if os.environ.get("HCTR_PACKED_EXCHANGE", "1") == "0" or self.hier:
-            return
+        """Flat collective (NCCL / gloo) path: every element of a requester's output slab is produced by
+        exactly one owner, and an owner needs only the key blocks and gradient columns of its own
+        lookups.  So nothing travels as a whole slab (``world`` times the useful bytes): every requester
+        sends owner o the key (and weight) blocks o serves, o sends requester r the ``n_o`` output
+        elements it owns, r returns the ``n_o`` matching gradient elements.  The region lists are
+        exchanged once here."""
         mine = [(int(d.out_off), int(d.out_stride), int(d.grad_off), int(d.grad_stride), int(d.ev_size))
                 for grp in self.groups if grp.kind == "mp" for d in grp.lookups]
         # key blocks [key_off, key_off + b * hotness) of the lookups this rank serves
@@ -803,12 +816,10 @@ class EmbeddingCollection:
         kidx = [torch.cat([torch.arange(o, o + ln, dtype=torch.int64) for (o, ln) in regs]) if regs
                 else torch.zeros(0, dtype=torch.int64) for regs in kregions]
         kn = [int(x.numel()) for x in kidx]
+        for ch in self.key_chans:
+            ch.recv = torch.zeros(max(self.world * kn[self.rank], 1), dtype=ch.slab.dtype, device=dev)
         self.packed = {
             "kn": kn, "kn_me": kn[self.rank], "key_me": kidx[self.rank].to(dev), "key_all": torch.cat(kidx).to(dev),
-            "key_recv": torch.zeros(max(self.world * kn[self.rank], 1), dtype=self.key_dtype, device=dev),
-            # the weights of the same key blocks take the same exchange (weighted inputs only)
-            "wgt_recv": torch.zeros(max(self.world * kn[self.rank], 1), dtype=torch.float32, device=dev)
-            if self.has_weights else None,
             "n": n, "n_me": n[self.rank],
             "out_me": oidx[self.rank].to(dev), "out_all": torch.cat(oidx).to(dev),
             "grad_me": gidx[self.rank].to(dev), "grad_all": torch.cat(gidx).to(dev),
@@ -824,69 +835,32 @@ class EmbeddingCollection:
         """Copy the fp32 per-key weights of a batch, in the layout of ``set_keys``, into the weight slab."""
         self.weight_slab[:feature_major_weights.numel()].copy_(feature_major_weights.reshape(-1), non_blocking=True)
 
-    def _wbufs(self, grp):
-        """per-source-rank weight buffers of a group's launches (None without weighted lookups)"""
-        if not self.has_weights:
-            return None
-        if self.world == 1 or grp.kind == "dp":
-            return [self.weight_slab]
-        return list(self.weights_all.unbind(0))
-
     def forward(self, is_train: bool = True):
         self.forward_begin()
         self.forward_compute()
         self.forward_end()
 
-    def _nnz_bufs(self, grp):
-        """per-source-rank bag-length buffers of the split lists (None when the split is off)"""
-        if self.nnz_all is None or grp.kind != "mp":
-            return None
-        return list(self.nnz_all.unbind(0))
-
     def forward_begin(self):
-        """every rank's keys are in place (fused mode: device-side barrier; collective: all-gather)"""
-        if self.nnz_slab is not None and not self.fused:
-            for gl in self.glookups:
-                if "split_off" in gl:
-                    E.shard_split(self.key_slab, gl["key_off"], self.b, gl["hotness"], gl["k"],
-                                  gl["split_off"], self.nnz_slab, gl["split_nnz_off"])
+        """every rank's keys are in place (fused mode: device-side barrier; collective: all-to-all)"""
         if self.world > 1:
             if self.fused:
                 # forward all-to-all of keys: posted peer stores into the owners' inboxes, then ONE
                 # device barrier (also orders the previous step's readers of these inboxes)
-                E.dispatch(self.key_slab, self._key_routes, self._key_routes_dev, self.peer_keys_all,
-                           self.peer_nnz, blocks_x=48)
-                if self._weight_routes:
-                    E.dispatch(self.weight_slab, self._weight_routes, self._weight_routes_dev,
-                               self.peer_weights_all, blocks_x=48)
+                for ch in self.key_chans:
+                    E.dispatch(ch.slab, ch.routes, ch.routes_dev, ch.peers, ch.nnz_peers, blocks_x=48)
                 self.comm.barrier_device()
             elif os.environ.get("SKIP_DATA_DISTRIBUTOR", "0") not in ("0", ""):
                 pass          # ablation (model_pipeline.cpp:118): owners keep the keys of an earlier step
             elif self.hier:
-                self.comm.hier_all_gather(self.keys_all, self.key_slab)
-                if self.nnz_all is not None:
-                    self.comm.hier_all_gather(self.nnz_all, self.nnz_slab)
-                if self.weights_all is not None:
-                    self.comm.hier_all_gather(self.weights_all, self.weight_slab)
-            elif getattr(self, "packed", None) is not None and self.nnz_all is None:
-                pk = self.packed        # every owner receives only the key blocks of the lookups it serves
-                send = self.key_slab.index_select(0, pk["key_all"])
-                recv = pk["key_recv"][:self.world * pk["kn_me"]]
-                self.comm.all_to_all_v(recv, send, [pk["kn_me"]] * self.world, pk["kn"])
-                if pk["kn_me"]:
-                    self.keys_all.index_copy_(1, pk["key_me"], recv.view(self.world, pk["kn_me"]))
-                if self.weights_all is not None:
-                    wsend = self.weight_slab.index_select(0, pk["key_all"])
-                    wrecv = pk["wgt_recv"][:self.world * pk["kn_me"]]
-                    self.comm.all_to_all_v(wrecv, wsend, [pk["kn_me"]] * self.world, pk["kn"])
-                    if pk["kn_me"]:
-                        self.weights_all.index_copy_(1, pk["key_me"], wrecv.view(self.world, pk["kn_me"]))
+                for ch in self.key_chans:
+                    self.comm.hier_all_gather(ch.all, ch.slab)
             else:
-                self.comm.all_gather(self.keys_all, self.key_slab)
-                if self.nnz_all is not None:
-                    self.comm.all_gather(self.nnz_all, self.nnz_slab)
-                if self.weights_all is not None:
-                    self.comm.all_gather(self.weights_all, self.weight_slab)
+                pk, W = self.packed, self.world   # every owner receives only the blocks of the lookups it serves
+                for ch in self.key_chans:
+                    recv = ch.recv[:W * pk["kn_me"]]
+                    self.comm.all_to_all_v(recv, ch.slab.index_select(0, pk["key_all"]), [pk["kn_me"]] * W, pk["kn"])
+                    if pk["kn_me"]:
+                        ch.all.index_copy_(1, pk["key_me"], recv.view(W, pk["kn_me"]))
         if self.has_dynamic:
             self._translate_dynamic_keys()
 
@@ -983,7 +957,7 @@ class EmbeddingCollection:
         keys get the next free row while training, unknown keys read as empty (-1) in evaluation; keys
         owned by another shard become -1.  The lookup kernels then run exactly as for static tables."""
         b = self.b
-        buf = self.key_slab.view(1, -1) if self.world == 1 else self.keys_all
+        buf = self.key_slab.view(1, -1) if self.world == 1 else self.key_chans[0].all
         for gl in self.glookups:
             t = self.tmap[gl["table"]]
             if not t.dynamic or t.evict_strategy is not None:
@@ -1100,32 +1074,21 @@ class EmbeddingCollection:
                 d.table_row_off, d.rows = sl["row_off"], sl["rows"]
             grp.lookups_dev = E.lookups_to_device(grp.lookups, self.device)
 
+    def _lookup(self, grp):
+        s = grp.src
+        E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, s.keys, s.out, self.b, self.rank,
+                  nnz_bufs=s.nnz, key_bytes=self._kb, act_bf16=self._abf, weight_bufs=s.weights)
+
     def forward_compute(self):
-        b = self.b
-        if self.world == 1:
-            for grp in self.groups:
-                E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, [self.key_slab],
-                          [self.out_slab], b, key_bytes=self._kb, act_bf16=self._abf, weight_bufs=self._wbufs(grp))
-        elif self.fused:
-            for grp in self.groups:
-                if grp.kind == "mp":
-                    E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch,
-                              list(self.keys_all.unbind(0)), self.peer_out, b, self.rank,
-                              nnz_bufs=self._nnz_bufs(grp), key_bytes=self._kb, act_bf16=self._abf,
-                              weight_bufs=self._wbufs(grp))
-                else:
-                    E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, [self.key_slab],
-                              [self.out_slab], b, key_bytes=self._kb, act_bf16=self._abf, weight_bufs=self._wbufs(grp))
-        else:
+        collective = self.world > 1 and not self.fused
+        if collective:
             self.send_out.zero_()
-            for grp in self.groups:
-                if grp.kind == "mp" and grp.lookups:
-                    E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch,
-                              list(self.keys_all.unbind(0)), list(self.send_out.unbind(0)), b, self.rank,
-                              nnz_bufs=self._nnz_bufs(grp), weight_bufs=self._wbufs(grp))
+        for grp in self.groups:
+            # (collective path: data-parallel lookups run in forward_end, after the exchange wrote the out slab)
+            if grp.lookups and not (collective and grp.kind == "dp"):
+                self._lookup(grp)
 
     def forward_end(self):
-        b = self.b
         if self.world > 1:
             if self.fused:
                 self.comm.barrier_device()       # every owner finished writing my outputs
@@ -1134,20 +1097,15 @@ class EmbeddingCollection:
             else:
                 if self.hier:
                     self.out_slab.copy_(self.comm.hier_all_to_all_sum(self.send_out))
-                elif self.packed is not None:
+                else:
                     pk = self.packed
                     send = self.send_out.index_select(1, pk["out_me"]).reshape(-1)        # [world * n_me]
                     recv = pk["fwd_recv"][:sum(pk["n"])]
                     self.comm.all_to_all_v(recv, send, pk["n"], [pk["n_me"]] * self.world)
                     self.out_slab.index_copy_(0, pk["out_all"], recv)
-                else:
-                    self.comm.all_to_all(self.recv_out, self.send_out)
-                    # each (rank, lookup) region of my slab is written by exactly one owner
-                    self.out_slab.copy_(self.recv_out.sum(0))
                 for grp in self.groups:
                     if grp.kind == "dp":
-                        E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, [self.key_slab],
-                                  [self.out_slab], b, weight_bufs=self._wbufs(grp))
+                        self._lookup(grp)
         if getattr(self, "_uniq", None) is not None:
             self._uniq.forward()
         self._reduce_partials()
@@ -1199,20 +1157,13 @@ class EmbeddingCollection:
                 from ..ops import dense as D
                 D.partial_sum(part, full, gl["col"], gl["k"], w)
 
-    def _bwd_bufs(self, grp):
-        if self.world == 1 or grp.kind == "dp":
-            return [self.key_slab], [self.grad_slab]
-        return list(self.keys_all.unbind(0)), list(self.grads_all.unbind(0))
-
     def backward_index(self):
         """gradient-independent part of the backward (unique rows + bucket lists); may run on a
         side stream concurrently with the dense network once the keys are in place."""
         for grp in self.groups:
             if grp.kind == "mp" and getattr(grp, "indexed", False) and grp.lookups:
-                kb, _ = self._bwd_bufs(grp)
-                E.bwd_index(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, kb, self.b, grp.ws,
-                            self.rank, nnz_bufs=self._nnz_bufs(grp), key_bytes=self._kb,
-                            weight_bufs=self._wbufs(grp))
+                E.bwd_index(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, grp.src.keys, self.b, grp.ws,
+                            self.rank, nnz_bufs=grp.src.nnz, key_bytes=self._kb, weight_bufs=grp.src.weights)
         self._index_done = True
 
     def backward(self, lr_t, step_t, dp_stream=None):
@@ -1233,7 +1184,7 @@ class EmbeddingCollection:
             dp_stream.wait_stream(cur)
             with torch.cuda.stream(dp_stream):
                 for grp in dp_groups:
-                    self._accum_update(grp, [self.key_slab], [self.grad_slab], lr_t, step_t)
+                    self._accum_update(grp, lr_t, step_t)
         if self.world > 1:
             if self.fused:
                 # backward all-to-all of gradients: every rank pushes the gradient columns of each
@@ -1248,25 +1199,22 @@ class EmbeddingCollection:
                 pass
             elif self.hier:
                 self.comm.hier_all_gather(self.grads_all, self.grad_slab)
-            elif getattr(self, "packed", None) is not None:
+            else:
                 pk = self.packed
                 send = self.grad_slab.index_select(0, pk["grad_all"])                    # chunks per owner
                 recv = pk["bwd_recv"][:self.world * pk["n_me"]]
                 self.comm.all_to_all_v(recv, send, [pk["n_me"]] * self.world, pk["n"])
                 if pk["n_me"]:
                     self.grads_all.index_copy_(1, pk["grad_me"], recv.view(self.world, pk["n_me"]))
-            else:
-                self.comm.all_gather(self.grads_all, self.grad_slab)
         for grp in mp_groups:
-            kb, gb = self._bwd_bufs(grp)
-            self._accum_update(grp, kb, gb, lr_t, step_t)
+            self._accum_update(grp, lr_t, step_t)
         if getattr(self, "_uniq", None) is not None:
             self._uniq.backward(lr_t, step_t)
         if side:
             torch.cuda.current_stream().wait_stream(dp_stream)
         else:
             for grp in dp_groups:
-                self._accum_update(grp, [self.key_slab], [self.grad_slab], lr_t, step_t)
+                self._accum_update(grp, lr_t, step_t)
         sched = os.environ.get("HCTR_STEP_SCHEDULE", "")
         end_default = "0" if (sched == "aggressive" or (sched != "safe" and self.world <= 4)) else "1"
         if self.world > 1 and self.fused and os.environ.get("HCTR_EMB_END_BARRIER", end_default) == "1":
@@ -1278,26 +1226,26 @@ class EmbeddingCollection:
     def _hp(self, o: OptParamsPy):
         return opt_hp(o, self.scaler, self.sr_seed)
 
-    def _accum_update(self, grp, key_bufs, grad_bufs, lr_t, step_t):
-        o = grp.opt
+    def _accum_update(self, grp, lr_t, step_t):
+        o, s = grp.opt, grp.src
         if not grp.lookups:
             return            # (every lookup of this group travels through the Unique exchange)
         if grp.kind == "mp" and getattr(grp, "indexed", False):
             E.bwd_reduce_update(o.optimizer_type, grp.lookups, grp.lookups_dev, grp.table, grp.s0,
-                                grp.s1, grp.pitch, key_bufs, grad_bufs, self.b, grp.ws, self._hp(o),
-                                lr_t, step_t, 1.0, self.rank, nnz_bufs=self._nnz_bufs(grp),
-                                key_bytes=self._kb, act_bf16=self._abf)
+                                grp.s1, grp.pitch, s.keys, s.grads, self.b, grp.ws, self._hp(o),
+                                lr_t, step_t, 1.0, self.rank, nnz_bufs=s.nnz, key_bytes=self._kb,
+                                act_bf16=self._abf)
         elif grp.kind == "mp":
-            E.backward_accum(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, key_bufs, grad_bufs,
-                             self.b, grp.ws, 1.0, self.rank, nnz_bufs=self._nnz_bufs(grp),
-                             key_bytes=self._kb, act_bf16=self._abf, weight_bufs=self._wbufs(grp))
+            E.backward_accum(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, s.keys, s.grads,
+                             self.b, grp.ws, 1.0, self.rank, nnz_bufs=s.nnz, key_bytes=self._kb,
+                             act_bf16=self._abf, weight_bufs=s.weights)
             E.update(o.optimizer_type, grp.table, grp.s0, grp.s1, grp.pitch, grp.ws, self._hp(o),
                      lr_t, step_t)
         else:
             from ..ops import dense as D
-            E.backward_accum(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, key_bufs, grad_bufs,
+            E.backward_accum(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, s.keys, s.grads,
                              self.b, None, 1.0, self.rank, dense_wgrad=grp.dense_wgrad,
-                             weight_bufs=self._wbufs(grp))
+                             weight_bufs=s.weights)
             if self.world > 1:
                 if grp.p2p_ar is not None:
                     grp.p2p_ar.run()

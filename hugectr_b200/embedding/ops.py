@@ -162,41 +162,6 @@ def vec4_aligned(lookups, ev_pitch, bufs=(), grad: bool = True) -> bool:
     return all(ptr(b) % 16 == 0 for b in bufs if b is not None)
 
 
-# ----------------------------------------------------------------------------- shard split
-def shard_split(key_slab, key_off, batch, hotness, k, split_off, nnz_slab, nnz_off):
-    """Rewrite the bag ``key_slab[key_off : key_off + batch*hotness]`` ([batch, hotness], -1 = empty) of
-    a table that is row-sharded k ways into k compacted lists of local row indices (key // k for the
-    keys with key % k == j, original order, -1 padded) at ``split_off + j*batch*hotness`` and their
-    lengths at ``nnz_slab[nnz_off + j*batch : ...]``."""
-    if key_slab.is_cuda:
-        l = lib()
-        if not hasattr(l, "_split_ready"):
-            l.hctr_emb_shard_split.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
-                                               C.c_int, C.c_int, C.c_void_p]
-            l.hctr_emb_shard_split.restype = C.c_int
-            l._split_ready = True
-        esz = key_slab.element_size()
-        rc = l.hctr_emb_shard_split(key_slab.data_ptr() + key_off * esz,
-                                    key_slab.data_ptr() + split_off * esz,
-                                    nnz_slab.data_ptr() + nnz_off * 4, batch, hotness, k, esz,
-                                    _st(key_slab.device))
-        if rc:
-            raise RuntimeError("hctr_emb_shard_split failed")
-        D._count()
-        return
-    keys = key_slab[key_off:key_off + batch * hotness].view(batch, hotness).long()
-    out = key_slab[split_off:split_off + k * batch * hotness].view(k, batch, hotness)
-    cnts = nnz_slab[nnz_off:nnz_off + k * batch].view(k, batch)
-    pos = torch.arange(hotness).view(1, -1)
-    for j in range(k):
-        m = (keys >= 0) & (keys % k == j)
-        order = torch.argsort((~m).to(torch.int8), dim=1, stable=True)
-        rows = torch.div(keys, k, rounding_mode="floor").gather(1, order)
-        cnt = m.sum(1)
-        out[j].copy_(torch.where(pos < cnt.view(-1, 1), rows, torch.full_like(rows, -1)).to(out.dtype))
-        cnts[j].copy_(cnt.to(torch.int32))
-
-
 # ----------------------------------------------------------------------------- dispatch (peer stores)
 class CDispatchRoute(C.Structure):
     _fields_ = [("src_off", C.c_longlong), ("dst_off", C.c_longlong), ("nnz_off", C.c_longlong),
@@ -276,13 +241,35 @@ def dispatch(src: torch.Tensor, routes: List[Route], routes_dev, dst_bufs, nnz_b
 
 
 # ----------------------------------------------------------------------------- forward
-def _weight_ptrs(p, lookups, weight_bufs):
-    """per-source-rank weight pointers of a launch with a weighted lookup (left null otherwise: the
-    kernels' unweighted instantiations)"""
-    if weight_bufs is None or not any(l.weighted for l in lookups):
-        return
-    for r, w in enumerate(weight_bufs):
-        p.weights[r] = w if isinstance(w, int) else w.data_ptr()
+def _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes, act_bf16,
+            nnz_bufs=None, weight_bufs=None, out_bufs=None, grad_bufs=None):
+    """CEmbParams of a launch over one source rank per entry of ``key_bufs`` (tensors, or int device
+    pointers for peers), with the key width and whether the outputs / gradients are bf16: read from the
+    buffers that are tensors, ``key_bytes`` / ``act_bf16`` where every one is a pointer.  The weight
+    pointers stay null without a weighted lookup (the kernels' unweighted instantiations)."""
+    def ptr(x):
+        return x if isinstance(x, int) else x.data_ptr()
+    p = CEmbParams()
+    p.num_ranks, p.my_rank, p.batch, p.num_lookups = len(key_bufs), my_rank, batch, len(lookups)
+    kb, abf = key_bytes, int(act_bf16)
+    weighted = weight_bufs is not None and any(l.weighted for l in lookups)
+    for r, k in enumerate(key_bufs):
+        p.keys[r] = ptr(k)
+        if not isinstance(k, int):
+            kb = k.element_size()
+        if nnz_bufs is not None:
+            p.nnz[r] = ptr(nnz_bufs[r])
+        if weighted:
+            p.weights[r] = ptr(weight_bufs[r])
+        for dst, bufs in ((p.out, out_bufs), (p.grad, grad_bufs)):
+            if bufs is not None:
+                dst[r] = ptr(bufs[r])
+                if not isinstance(bufs[r], int):
+                    abf = int(bufs[r].dtype == torch.bfloat16)
+    p.lookups = lookups_dev.data_ptr()
+    p.table = table.data_ptr()
+    p.ev_size = ev_pitch
+    return p, kb, abf
 
 
 def _key_weights(lk, weight_bufs, src, batch, own):
@@ -299,27 +286,9 @@ def forward(lookups, lookups_dev, table, ev_pitch, key_bufs, out_bufs, batch, my
             nnz_bufs=None, key_bytes=4, act_bf16=True, weight_bufs=None):
     """key_bufs / out_bufs (/ weight_bufs, fp32 per-key weights of weighted lookups): one entry per
     source rank (tensor, or int device pointer for peers)."""
-    R = len(key_bufs)
     if table.is_cuda:
-        p = CEmbParams()
-        _weight_ptrs(p, lookups, weight_bufs)
-        p.num_ranks, p.my_rank, p.batch, p.num_lookups = R, my_rank, batch, len(lookups)
-        kb = key_bytes
-        out_bf16 = int(act_bf16)
-        for r in range(R):
-            k, o = key_bufs[r], out_bufs[r]
-            p.keys[r] = k if isinstance(k, int) else k.data_ptr()
-            p.out[r] = o if isinstance(o, int) else o.data_ptr()
-            if nnz_bufs is not None:
-                n = nnz_bufs[r]
-                p.nnz[r] = n if isinstance(n, int) else n.data_ptr()
-            if not isinstance(k, int):
-                kb = k.element_size()
-            if not isinstance(o, int):
-                out_bf16 = int(o.dtype == torch.bfloat16)
-        p.lookups = lookups_dev.data_ptr()
-        p.table = table.data_ptr()
-        p.ev_size = ev_pitch
+        p, kb, out_bf16 = _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes,
+                                  act_bf16, nnz_bufs, weight_bufs, out_bufs=out_bufs)
         max_ev = max((l.ev_size for l in lookups), default=ev_pitch)
         check_ev_size(max_ev)
         al4 = int(vec4_aligned(lookups, ev_pitch, [table, *out_bufs], grad=False))
@@ -332,28 +301,30 @@ def forward(lookups, lookups_dev, table, ev_pitch, key_bufs, out_bufs, batch, my
     forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs, weight_bufs)
 
 
-def _owned(lk: LookupDesc, keys):
-    keys = keys.long()
+def _bag(lk: LookupDesc, key_bufs, nnz_bufs, src, batch):
+    """(owned [batch, hotness], arena rows, bag lengths [batch]) of lookup ``lk`` over source rank
+    ``src``'s keys: a key is owned when valid, of this shard, inside the table and -- for a split list
+    -- inside its bag length"""
+    kbuf = key_bufs[src].reshape(-1)
+    keys = torch.as_strided(kbuf, (batch, lk.hotness), (lk.key_stride, 1), kbuf.storage_offset() + lk.key_off).long()
     own = keys >= 0
     if lk.num_shards > 1:
         own &= (keys % lk.num_shards) == lk.shard_idx
     r = torch.div(keys, lk.num_shards, rounding_mode="floor")
     own &= r < lk.rows
-    return own, lk.table_row_off + torch.where(own, r, torch.zeros_like(r))
+    nnz = torch.full((batch,), lk.hotness, device=keys.device)
+    if lk.nnz_off >= 0 and nnz_bufs is not None:
+        nnz = nnz_bufs[src].reshape(-1)[lk.nnz_off:lk.nnz_off + batch].long().clamp(max=lk.hotness)
+        own &= torch.arange(lk.hotness, device=keys.device).view(1, -1) < nnz.view(-1, 1)
+    return own, lk.table_row_off + torch.where(own, r, torch.zeros_like(r)), nnz
 
 
 def forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs=None, weight_bufs=None):
     tab = table.view(-1, ev_pitch)
     for src in range(len(key_bufs)):
-        kbuf, obuf = key_bufs[src].reshape(-1), out_bufs[src].reshape(-1)
+        obuf = out_bufs[src].reshape(-1)
         for lk in lookups:
-            keys = torch.as_strided(kbuf, (batch, lk.hotness), (lk.key_stride, 1),
-                                    kbuf.storage_offset() + lk.key_off)
-            own, rows = _owned(lk, keys)
-            nnz = torch.full((batch,), lk.hotness, device=keys.device)
-            if lk.nnz_off >= 0 and nnz_bufs is not None:
-                nnz = nnz_bufs[src].reshape(-1)[lk.nnz_off:lk.nnz_off + batch].long().clamp(max=lk.hotness)
-                own &= torch.arange(lk.hotness, device=keys.device).view(1, -1) < nnz.view(-1, 1)
+            own, rows, nnz = _bag(lk, key_bufs, nnz_bufs, src, batch)
             v = tab[rows][..., :lk.ev_size].float() * _key_weights(lk, weight_bufs, src, batch, own).unsqueeze(-1)
             pooled = v.sum(1)
             if lk.combiner == 1:
@@ -458,26 +429,9 @@ def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, b
                    my_rank=0, nnz_bufs=None, dense_wgrad=None, key_bytes=4, act_bf16=True, weight_bufs=None):
     """Accumulate bucket gradients (times the key's weight for weighted lookups) per unique row (or
     into a dense wgrad for DP tables)."""
-    R = len(key_bufs)
     if table.is_cuda:
-        p = CEmbParams()
-        _weight_ptrs(p, lookups, weight_bufs)
-        p.num_ranks, p.my_rank, p.batch, p.num_lookups = R, my_rank, batch, len(lookups)
-        kb, gbf = key_bytes, int(act_bf16)
-        for r in range(R):
-            k, g = key_bufs[r], grad_bufs[r]
-            p.keys[r] = k if isinstance(k, int) else k.data_ptr()
-            p.grad[r] = g if isinstance(g, int) else g.data_ptr()
-            if nnz_bufs is not None:
-                n = nnz_bufs[r]
-                p.nnz[r] = n if isinstance(n, int) else n.data_ptr()
-            if not isinstance(k, int):
-                kb = k.element_size()
-            if not isinstance(g, int):
-                gbf = int(g.dtype == torch.bfloat16)
-        p.lookups = lookups_dev.data_ptr()
-        p.table = table.data_ptr()
-        p.ev_size = ev_pitch
+        p, kb, gbf = _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes, act_bf16,
+                             nnz_bufs, weight_bufs, grad_bufs=grad_bufs)
         max_ev = max((l.ev_size for l in lookups), default=ev_pitch)
         if dense_wgrad is not None:
             ut = CUniqueTable(0, 0, 0, 0, 0, 0, 0xFFFFFFFF)
@@ -494,16 +448,10 @@ def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, b
         D._count()
         return
     rows_all, grads_all = [], []
-    for src in range(R):
-        kbuf, gbuf = key_bufs[src].reshape(-1), grad_bufs[src].reshape(-1)
+    for src in range(len(key_bufs)):
+        gbuf = grad_bufs[src].reshape(-1)
         for lk in lookups:
-            keys = torch.as_strided(kbuf, (batch, lk.hotness), (lk.key_stride, 1),
-                                    kbuf.storage_offset() + lk.key_off)
-            own, rows = _owned(lk, keys)
-            nnz = torch.full((batch,), lk.hotness, device=keys.device)
-            if lk.nnz_off >= 0 and nnz_bufs is not None:
-                nnz = nnz_bufs[src].reshape(-1)[lk.nnz_off:lk.nnz_off + batch].long().clamp(max=lk.hotness)
-                own &= torch.arange(lk.hotness, device=keys.device).view(1, -1) < nnz.view(-1, 1)
+            own, rows, nnz = _bag(lk, key_bufs, nnz_bufs, src, batch)
             g = torch.as_strided(gbuf, (batch, lk.ev_size), (lk.grad_stride, 1),
                                  gbuf.storage_offset() + lk.grad_off)
             g = g.float() * grad_scale
@@ -690,32 +638,6 @@ def gather_rows(table, ev_pitch, rows, out):
     out.copy_(v.to(out.dtype))
 
 
-def _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch, my_rank, nnz_bufs,
-                 key_bytes=4, act_bf16=True, weight_bufs=None):
-    R = len(key_bufs)
-    p = CEmbParams()
-    _weight_ptrs(p, lookups, weight_bufs)
-    p.num_ranks, p.my_rank, p.batch, p.num_lookups = R, my_rank, batch, len(lookups)
-    kb, gbf = key_bytes, int(act_bf16)
-    for r in range(R):
-        k = key_bufs[r]
-        p.keys[r] = k if isinstance(k, int) else k.data_ptr()
-        if not isinstance(k, int):
-            kb = k.element_size()
-        if grad_bufs is not None:
-            g = grad_bufs[r]
-            p.grad[r] = g if isinstance(g, int) else g.data_ptr()
-            if not isinstance(g, int):
-                gbf = int(g.dtype == torch.bfloat16)
-        if nnz_bufs is not None:
-            n = nnz_bufs[r]
-            p.nnz[r] = n if isinstance(n, int) else n.data_ptr()
-    p.lookups = lookups_dev.data_ptr()
-    p.table = table.data_ptr()
-    p.ev_size = ev_pitch
-    return p, kb, gbf
-
-
 def bwd_index(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, ws, my_rank=0, nnz_bufs=None,
               key_bytes=4, weight_bufs=None):
     """Gradient-independent part of the backward: unique rows + per-row bucket lists (with the
@@ -726,8 +648,8 @@ def bwd_index(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, ws, my_ran
                          "(see vec4_aligned); use backward_accum + update")
     if any(l.weighted for l in lookups) and (weight_bufs is None or ws.bucket_scale is None):
         raise ValueError("weighted lookups need their weight buffers and a workspace built with need_scale")
-    p, kb, _ = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, None, batch, my_rank,
-                            nnz_bufs, key_bytes, weight_bufs=weight_bufs)
+    p, kb, _ = _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes, True,
+                       nnz_bufs, weight_bufs)
     total_pairs = len(key_bufs) * batch * sum(l.hotness for l in lookups)
     rc = lib().hctr_emb_bwd_index(C.byref(p), C.byref(ws.c), C.byref(ws.ix), total_pairs, kb,
                                   _st(table.device))
@@ -744,8 +666,8 @@ def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_
     if not vec4_aligned(lookups, ev_pitch, [table, *grad_bufs], grad=True):
         raise ValueError("the fused backward needs 4-element aligned gradient rows and pitch "
                          "(see vec4_aligned); use backward_accum + update")
-    p, kb, gbf = _fill_params(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, batch,
-                              my_rank, nnz_bufs, key_bytes, act_bf16)
+    p, kb, gbf = _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes, act_bf16,
+                         nnz_bufs, grad_bufs=grad_bufs)
     h = opt_hyper(hp, lr_t, step_t)
     sbf = int(s0 is not None and s0.dtype == torch.bfloat16)
     rc = lib().hctr_emb_bwd_reduce_update(C.byref(p), C.byref(ws.c), C.byref(ws.ix),

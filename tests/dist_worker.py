@@ -658,8 +658,6 @@ def run_equiv(optimizer="sgd", gpus_per_node=0, comm=None):
         assert m.ebcs_train[0]._uniq is not None and not m._graph_safe()
     if gpus_per_node:
         assert m.ebcs_train[0].hier and comm.num_nodes == world // gpus_per_node
-    if os.environ.get("HCTR_SHARD_SPLIT", "0") == "1":
-        assert m.ebcs_train[0].nnz_slab is not None, "requester-side shard split is not active"
     single = Comm.single(comm.device)
     ref = build_dlrm_dcnv2(batchsize=b * world, num_gpus=1, comm=single, **kw)
     ref.compile()

@@ -134,26 +134,6 @@ def test_hierarchical_exchange_gloo():
 
 
 @pytest.mark.dist
-@pytest.mark.parametrize("nproc,extra", [(2, []), (4, ["2"])])
-def test_requester_side_shard_split_gloo(nproc, extra):
-    """HCTR_SHARD_SPLIT=1: row-sharded bags are pre-split into per-shard row lists by the requester;
-    training must still equal the single-process run (flat and hierarchical exchange)"""
-    out = _run(nproc, ["equiv", "sgd"] + extra, 29711, env={"CUDA_VISIBLE_DEVICES": "", "HCTR_SHARD_SPLIT": "1"})
-    assert "EQUIV_OK" in out
-
-
-@pytest.mark.gpu
-def test_requester_side_shard_split_multi_gpu():
-    n = torch.cuda.device_count()
-    if n < 2:
-        pytest.skip("needs >= 2 GPUs")
-    if os.environ.get("HCTR_TEST_EXPERIMENTAL", "0") != "1":
-        pytest.skip("experimental CUDA path (validated on CPU/gloo only so far): set HCTR_TEST_EXPERIMENTAL=1")
-    out = _run(min(n, 8), ["equiv", "sgd"], 29721, env={"HCTR_SHARD_SPLIT": "1"})
-    assert "EQUIV_OK" in out
-
-
-@pytest.mark.dist
 def test_checkpoint_resharding_gloo(world2):
     """2-rank checkpoint (dense + embedding collection) loads into a single-process model"""
     assert "CKPT_OK" in world2 and _done(world2, "ckpt;")
@@ -234,13 +214,6 @@ def test_embedding_collection_benchmark_script_gloo():
 def test_symmetric_heap_failure_is_agreed_on_by_all_ranks_gloo():
     out = _run(3, ["symmfail"], 29791, env={"CUDA_VISIBLE_DEVICES": ""})
     assert "SYMMFAIL_OK" in out, out[-2000:]
-
-
-@pytest.mark.dist
-def test_full_slab_exchange_still_selectable_gloo():
-    """HCTR_PACKED_EXCHANGE=0: whole-slab all-to-all / all-gather instead of the packed owner regions"""
-    out = _run(2, ["fuzz", "301,302,303"], 29795, env={"CUDA_VISIBLE_DEVICES": "", "HCTR_PACKED_EXCHANGE": "0"})
-    assert out.count("FUZZ_OK") == 3, out[-2000:]
 
 
 @pytest.mark.dist

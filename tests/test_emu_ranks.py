@@ -33,33 +33,12 @@ def test_emu_fuzz_cpu():
         run_ranks(2, lambda c: W.run_fuzz(seed, comm=c), device=CPU)
 
 
-@pytest.fixture
-def shard_split_env():
-    old = os.environ.get("HCTR_SHARD_SPLIT")
-    os.environ["HCTR_SHARD_SPLIT"] = "1"
-    yield
-    if old is None:
-        os.environ.pop("HCTR_SHARD_SPLIT", None)
-    else:
-        os.environ["HCTR_SHARD_SPLIT"] = old
-
-
-def test_emu_shard_split_cpu(shard_split_env):
-    run_ranks(2, lambda c: W.run_ebc("mixed", False, comm=c), device=CPU)
-    run_ranks(2, lambda c: W.run_equiv("sgd", comm=c), device=CPU)
-
-
 # ----------------------------------------------------------------------------- GPU: fused peer kernels
 @pytest.mark.gpu
 @pytest.mark.parametrize("world", [2, 4])
 @pytest.mark.parametrize("plan", ["mixed", "column"])
 def test_emu_ebc_fused_gpu(plan, world):
     run_ranks(world, lambda c: W.run_ebc(plan, True, comm=c))
-
-
-@pytest.mark.gpu
-def test_emu_ebc_fused_shard_split_gpu(shard_split_env):
-    run_ranks(4, lambda c: W.run_ebc("mixed", True, comm=c))
 
 
 @pytest.mark.gpu
@@ -77,11 +56,6 @@ def test_emu_p2p_allreduce_gpu():
 @pytest.mark.parametrize("opt", ["sgd", "adagrad"])
 def test_emu_model_equals_single_gpu(opt):
     run_ranks(4, lambda c: W.run_equiv(opt, comm=c))
-
-
-@pytest.mark.gpu
-def test_emu_model_equals_single_shard_split_gpu(shard_split_env):
-    run_ranks(4, lambda c: W.run_equiv("adagrad", comm=c))
 
 
 @pytest.mark.gpu

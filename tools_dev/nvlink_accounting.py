@@ -30,7 +30,6 @@ def collection(world, rank):
     e.placement = resolve_placement(cfg, world)
     e.shard_split, e._kb, e._abf = world > 1, 4, True
     e._build_layout({f"d{i}": CRITEO_TB_MULTI_HOT[i] for i in range(n)})
-    e._build_key_routes()
     e._build_grad_routes()
     return e
 
@@ -42,7 +41,7 @@ for W in (2, 4, 8):
     kmax = omax = gmax = 0
     for r in range(W):
         e = collection(W, r)
-        kmax = max(kmax, e.dispatch_key_bytes)
+        kmax = max(kmax, sum(x.rows * x.row_elems * e._kb for x in e._build_key_routes(r)[0] if x.dst_rank != r))
         gmax = max(gmax, e.push_grad_bytes)
         out = 0
         for gl in e.glookups:                     # vectors this rank (as owner) stores into the other requesters
