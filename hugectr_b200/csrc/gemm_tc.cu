@@ -177,8 +177,9 @@ __global__ void __launch_bounds__(kNumThreads, 1)
   using L = SmemLayout<BN, TMA_EPI>;
   constexpr int kStages = L::kStages;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
+  // aligned by an offset from smem_raw, so that the compiler keeps every derived pointer in the shared window: the
+  // TMA epilogue then reads and writes its boxes with 32-bit LDS / STS addresses instead of 64-bit generic ones
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * L::kABytes;
   uint8_t* epi = smem + kStages * L::kStageBytes;

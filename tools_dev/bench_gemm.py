@@ -10,7 +10,8 @@ kept with its M, N, K, operand layouts, epilogue flags, splits, the operands pre
 call is then replayed on fresh random operands of the same shapes and strides; the three arms run
 alternately, `iters` launches per timed block, and the median over `rounds` blocks is reported with the
 achieved TFLOP/s and GB/s and the floor max(FLOP / 989 TFLOP/s, bytes / 3.35 TB/s) from the H100 SXM data
-sheet.  Bytes are one pass over every operand and epilogue tensor (fp32 accumulating outputs twice).
+sheet.  Bytes are one pass over every operand and epilogue tensor (fp32 accumulating outputs twice).  `block_n` is
+the tile the autotuner picked for ours (gemm_bf16's block_n code).
 
 --tree DIR imports hugectr_b200 from another checkout (built in place), so that two builds can be timed one
 process per run in one session.  Without a CUDA device the tool exits with an error and measures nothing.
@@ -232,13 +233,22 @@ def main(argv):
             G.gemm_bf16(ts["a"], ts["b"], ts["out"], **kw)
             G.IMPL = "tc"
 
-        arms = {"ours": ours, "mm": lambda: torch.mm(A, B), "library": library}
-        ms = time_arms(arms, a.iters, a.rounds)
+        picks, tuned = [], G._tuned_block_n
+
+        def spy_tuned(*args):
+            picks.append(tuned(*args))
+            return picks[-1]
+
+        G._tuned_block_n = spy_tuned
+        try:
+            ms = time_arms({"ours": ours, "mm": lambda: torch.mm(A, B), "library": library}, a.iters, a.rounds)
+        finally:
+            G._tuned_block_n = tuned
         G.IMPL = "tc"
         flop, byt = 2.0 * M * N * K, nbytes(c)
         floor_ms = max(flop / PEAK_FLOPS, byt / PEAK_BW) * 1e3
         r = {"call": i, "M": M, "N": N, "K": K, "a_mn": c["a_mn"], "b_mn": c["b_mn"], "flags": c["flags"],
-             "splits": c["splits"], "operands": [k for k in TENSORS[3:] if k in c],
+             "splits": c["splits"], "operands": [k for k in TENSORS[3:] if k in c], "block_n": picks[-1],
              "floor_ms": round(floor_ms, 5),
              "floor_bound": "compute" if flop / PEAK_FLOPS >= byt / PEAK_BW else "memory"}
         for k, t in ms.items():
