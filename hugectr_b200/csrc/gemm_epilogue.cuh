@@ -1,4 +1,5 @@
-// Shared declarations + the fused epilogue of the wgmma GEMM kernels (gemm_tc.cu, gemm_mxfp8.cu).
+// Shared declarations, the tensor-map encoder, the pipeline-ring position and the fused epilogue of the wgmma GEMM
+// kernels (gemm_tc.cu, gemm_mxfp8.cu).
 #pragma once
 #include "ptx.cuh"
 
@@ -8,11 +9,10 @@ enum EpiFlags : int {
   EPI_RELU = 1,
   EPI_OUT_F32 = 2,
   EPI_ATOMIC = 4,   // fp32 red.add into out (split-K / beta=1)
-  EPI_ACCUM = 8,    // out(fp32) += acc, non atomic
   EPI_CROSS = 16,   // out = x0 * (acc + bias) + xl ; aux (optional) = acc + bias
   EPI_MASK = 32,    // out = acc * (mask > 0)
   EPI_SIGMOID = 64, // out = sigmoid(acc + bias)
-  EPI_ADD = 128,    // out = acc + xl (bf16) [+ addf (fp32)]   (residual / gradient accumulation)
+  EPI_ADD = 128,    // out = acc + xl (bf16)   (residual / gradient accumulation)
 };
 
 struct GemmParams {
@@ -30,8 +30,48 @@ struct GemmParams {
   long long ldx;
   float alpha;
   int flags;
-  const float* addf;
-  long long ldaddf;
+  // Unused.  Keeps the struct at its earlier size: without these 16 bytes nvcc 12.9 duplicates the TMA epilogue
+  // loop of gemm_tc_kernel, and its bf16-output GEMMs ran 10-17% slower on an H100 80GB HBM3 (700 W).
+  long long reserved[2];
+};
+
+// cuTensorMapEncodeTiled, looked up once through the runtime's driver entry point (nullptr if the driver lacks it)
+typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
+                                    const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+
+inline PFN_encodeTiled get_encode() {
+  static PFN_encodeTiled fn = nullptr;
+  if (fn == nullptr) {
+    void* ptr = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) !=
+            cudaSuccess ||
+        ptr == nullptr)
+      return nullptr;
+    fn = reinterpret_cast<PFN_encodeTiled>(ptr);
+  }
+  return fn;
+}
+
+// The dynamic shared-memory base rounded up to 1024 bytes (SWIZZLE_128B tiles).  It is an offset from `smem_raw`
+// rather than an integer cast, so that the compiler keeps every derived pointer in the shared window and addresses
+// it with 32-bit LDS / STS instead of 64-bit generic loads and stores.
+HCTR_DEVICE uint8_t* smem_align1024(uint8_t* smem_raw) {
+  return smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+}
+
+// Position in a ring of mbarrier-guarded slots: the slot, and the parity of the current pass over the ring.
+struct RingPos {
+  int slot = 0;
+  uint32_t phase = 0;
+  HCTR_DEVICE void advance(const int slots) {
+    if (++slot == slots) {
+      slot = 0;
+      phase ^= 1;
+    }
+  }
 };
 
 
@@ -108,21 +148,10 @@ HCTR_DEVICE void epilogue_chunk(const GemmParams& p, const int flags, const int 
           v[8 * j + 2 * q + 1] += bf16_hi(bw[q]);
         }
       }
-      if (p.addf != nullptr) {
-        const float* pf = p.addf + static_cast<long long>(m) * p.ldaddf + n0;
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          const float4 f = __ldg(reinterpret_cast<const float4*>(pf + j));
-          v[j] += f.x; v[j + 1] += f.y; v[j + 2] += f.z; v[j + 3] += f.w;
-        }
-      }
     } else {
 #pragma unroll
       for (int j = 0; j < 32; ++j)
-        if (j < nvalid) {
-          v[j] += __bfloat162float(pxl[j]);
-          if (p.addf != nullptr) v[j] += p.addf[static_cast<long long>(m) * p.ldaddf + n0 + j];
-        }
+        if (j < nvalid) v[j] += __bfloat162float(pxl[j]);
     }
   }
   if (flags & EPI_MASK) {
@@ -152,7 +181,7 @@ HCTR_DEVICE void epilogue_chunk(const GemmParams& p, const int flags, const int 
 #pragma unroll
     for (int j = 0; j < 32; ++j) v[j] = 1.f / (1.f + __expf(-v[j]));
   }
-  if (flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)) {
+  if (flags & (EPI_OUT_F32 | EPI_ATOMIC)) {
     float* po = reinterpret_cast<float*>(p.out) + static_cast<long long>(m) * p.ldo + n0;
     if (flags & EPI_ATOMIC) {
       if (nvalid == 32) {
@@ -164,8 +193,6 @@ HCTR_DEVICE void epilogue_chunk(const GemmParams& p, const int flags, const int 
       } else {
         _Pragma("unroll") for (int j = 0; j < 32; ++j) if (j < nvalid) atomicAdd(po + j, v[j]);
       }
-    } else if (flags & EPI_ACCUM) {
-      _Pragma("unroll") for (int j = 0; j < 32; ++j) if (j < nvalid) po[j] += v[j];
     } else if (nvalid == 32) {
 #pragma unroll
       for (int j = 0; j < 32; j += 4)

@@ -37,7 +37,7 @@ __global__ void __launch_bounds__(MX_THREADS, 1)
     gemm_mxfp8_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const uint8_t* __restrict__ sfa, const uint8_t* __restrict__ sfb, const GemmParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~static_cast<uintptr_t>(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + MX_STAGES * MX_TILE_BYTES;
   uint8_t* smem_sfa = smem + 2 * MX_STAGES * MX_TILE_BYTES;
@@ -66,21 +66,17 @@ __global__ void __launch_bounds__(MX_THREADS, 1)
   if (wg == 0) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp_idx == 0 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos s;
       for (int kb = 0; kb < k_blocks; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        mbar_arrive_expect_tx(&full_bar[stage], 2 * MX_TILE_BYTES + 2 * MX_SF_BYTES);
-        tma_load_2d(smem_a + stage * MX_TILE_BYTES, &tmA, &full_bar[stage], kb * MX_BK, m_blk * MX_BM);
-        tma_load_2d(smem_b + stage * MX_TILE_BYTES, &tmB, &full_bar[stage], kb * MX_BK, n_blk * MX_BN);
-        bulk_load_1d(smem_sfa + stage * MX_SF_BYTES,
-                     sfa + (static_cast<long long>(m_blk) * k_blocks + kb) * MX_SF_BYTES, MX_SF_BYTES, &full_bar[stage]);
-        bulk_load_1d(smem_sfb + stage * MX_SF_BYTES,
-                     sfb + (static_cast<long long>(n_blk) * k_blocks + kb) * MX_SF_BYTES, MX_SF_BYTES, &full_bar[stage]);
-        if (++stage == MX_STAGES) {
-          stage = 0;
-          phase ^= 1;
-        }
+        mbar_wait(&empty_bar[s.slot], s.phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[s.slot], 2 * MX_TILE_BYTES + 2 * MX_SF_BYTES);
+        tma_load_2d(smem_a + s.slot * MX_TILE_BYTES, &tmA, &full_bar[s.slot], kb * MX_BK, m_blk * MX_BM);
+        tma_load_2d(smem_b + s.slot * MX_TILE_BYTES, &tmB, &full_bar[s.slot], kb * MX_BK, n_blk * MX_BN);
+        bulk_load_1d(smem_sfa + s.slot * MX_SF_BYTES,
+                     sfa + (static_cast<long long>(m_blk) * k_blocks + kb) * MX_SF_BYTES, MX_SF_BYTES, &full_bar[s.slot]);
+        bulk_load_1d(smem_sfb + s.slot * MX_SF_BYTES,
+                     sfb + (static_cast<long long>(n_blk) * k_blocks + kb) * MX_SF_BYTES, MX_SF_BYTES, &full_bar[s.slot]);
+        s.advance(MX_STAGES);
       }
     }
   } else {
@@ -91,14 +87,13 @@ __global__ void __launch_bounds__(MX_THREADS, 1)
     float acc[64], part[64];
 #pragma unroll
     for (int i = 0; i < 64; ++i) acc[i] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
+    RingPos s;
     for (int kb = 0; kb < k_blocks; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
-      const uint64_t a_desc = make_smem_desc_sw128(smem_u32(smem_a + stage * MX_TILE_BYTES) + cw * (64 * 128), 16, 1024);
-      const uint64_t b_desc = make_smem_desc_sw128(smem_u32(smem_b + stage * MX_TILE_BYTES), 16, 1024);
-      const uint8_t* sa = smem_sfa + stage * MX_SF_BYTES;
-      const uint8_t* sb = smem_sfb + stage * MX_SF_BYTES;
+      mbar_wait(&full_bar[s.slot], s.phase);
+      const uint64_t a_desc = make_smem_desc_sw128(smem_u32(smem_a + s.slot * MX_TILE_BYTES) + cw * (64 * 128), 16, 1024);
+      const uint64_t b_desc = make_smem_desc_sw128(smem_u32(smem_b + s.slot * MX_TILE_BYTES), 16, 1024);
+      const uint8_t* sa = smem_sfa + s.slot * MX_SF_BYTES;
+      const uint8_t* sb = smem_sfb + s.slot * MX_SF_BYTES;
 #pragma unroll
       for (int k = 0; k < MX_BK / 32; ++k) {
         wgmma_fence_regs(part);
@@ -121,11 +116,8 @@ __global__ void __launch_bounds__(MX_THREADS, 1)
         }
       }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
-      if (++stage == MX_STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+      if (lane == 0) mbar_arrive(&empty_bar[s.slot]);
+      s.advance(MX_STAGES);
     }
     epilogue_tile_wg<MX_BN>(p, p.flags, acc, epi + cw * (kEpiSlabBytes / 4), m_blk * MX_BM + cw * 64,
                             n_blk * MX_BN, cw);
@@ -186,17 +178,9 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-typedef CUresult (*PFN_encodeTiledMx)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                      const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                      CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static int make_tmap_u8(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer, uint64_t ld_bytes) {
-  static PFN_encodeTiledMx enc = nullptr;
-  if (enc == nullptr) {
-    void* fp = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &qres) != cudaSuccess || !fp) return -1;
-    enc = reinterpret_cast<PFN_encodeTiledMx>(fp);
-  }
+  PFN_encodeTiled enc = get_encode();
+  if (enc == nullptr) return -1;
   cuuint64_t dims[2] = {inner, outer};
   cuuint64_t strides[1] = {ld_bytes};
   cuuint32_t box[2] = {128, 128};

@@ -17,9 +17,9 @@
 //    tile's main loop runs.  The consumers combine them with the accumulators in place, at the wgmma fragment
 //    positions, and one thread TMA-stores the bf16 box (and aux) asynchronously; the slot is handed back to the
 //    producer once the store has read it, which for a tile's last group happens in the next tile's main loop.
-//  * Slab epilogue (fp32 / atomic / accumulating outputs, addf, tensors TMA cannot address): the accumulators
-//    leave the registers through a per-warpgroup [64 x 64] fp32 staging slab, so the fused epilogue works on
-//    one row x 32 columns per thread with vectorised global accesses.
+//  * Slab epilogue (fp32 / atomic outputs, tensors TMA cannot address): the accumulators leave the registers
+//    through a per-warpgroup [64 x 64] fp32 staging slab, so the fused epilogue works on one row x 32 columns per
+//    thread with vectorised global accesses.
 #include <cstdio>
 #include <cstring>
 
@@ -61,14 +61,14 @@ struct SmemLayout {
 };
 
 // TMA epilogue of one warpgroup's m64 x BN accumulator tile (rows m_base.., columns n_base..).  `ring` holds the
-// warpgroup's kEpiBoxes boxes; slot / phase walk it in step with the producer (full / empty barriers, used only
-// when the flags read tensors), and `pending` is the slot whose TMA store has not been confirmed to have read it.
-// Every element goes through the same fp32 expressions, in the same order, as epilogue_chunk.
+// warpgroup's kEpiBoxes boxes; `pos` walks it in step with the producer (full / empty barriers, used only when the
+// flags read tensors), and `pending` is the slot whose TMA store has not been confirmed to have read it.  Every
+// element goes through the same fp32 expressions, in the same order, as epilogue_chunk.
 template <int BN>
 HCTR_DEVICE void epilogue_tile_tma(const GemmParams& p, const int flags, const float (&acc)[BN / 2],
                                    uint8_t* ring, uint64_t* full, uint64_t* empty, const CUtensorMap* tm_out,
                                    const CUtensorMap* tm_aux, const int m_base, const int n_base, const int wg,
-                                   int& slot, uint32_t& phase, int& pending) {
+                                   RingPos& pos, int& pending) {
   const int n_in = epi_in_boxes(flags);
   const int nbox = n_in > 0 ? n_in : 1;
   const int slots = kEpiBoxes / nbox;
@@ -85,7 +85,7 @@ HCTR_DEVICE void epilogue_tile_tma(const GemmParams& p, const int flags, const f
   for (int g = 0; g < BN / 64; ++g) {
     const int n0 = n_base + g * 64;
     if (n0 >= p.N) break;
-    uint8_t* box = ring + slot * nbox * kEpiBoxBytes;
+    uint8_t* box = ring + pos.slot * nbox * kEpiBoxBytes;
     float2 bv[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
@@ -96,7 +96,7 @@ HCTR_DEVICE void epilogue_tile_tma(const GemmParams& p, const int flags, const f
         else if (n < p.N) bv[j].x = __ldg(p.bias + n);
       }
     }
-    if (n_in > 0) mbar_wait(&full[slot], phase);
+    if (n_in > 0) mbar_wait(&full[pos.slot], pos.phase);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
 #pragma unroll
@@ -149,11 +149,8 @@ HCTR_DEVICE void epilogue_tile_tma(const GemmParams& p, const int flags, const f
       if (aux) tma_store_2d(tm_aux, box + kEpiBoxBytes, n0, m_base);
       bulk_commit();
     }
-    pending = slot;
-    if (++slot == slots) {
-      slot = 0;
-      phase ^= 1;
-    }
+    pending = pos.slot;
+    pos.advance(slots);
   }
 }
 
@@ -162,6 +159,27 @@ HCTR_DEVICE void wgmma_tile(float (&acc)[BN / 2], uint64_t a, uint64_t b, uint32
   if constexpr (BN == 64) wgmma_bf16_n64<TA, TB>(acc, a, b, accumulate);
   else if constexpr (BN == 128) wgmma_bf16_n128<TA, TB>(acc, a, b, accumulate);
   else wgmma_bf16_n256<TA, TB>(acc, a, b, accumulate);
+}
+
+// Work item t of the persistent walk is (m-group of MC tiles, n tile, k split), n fastest; the CTAs of a cluster take
+// the MC consecutive m tiles of one item.  Both producers and the consumers walk the items through this one mapping:
+// if they disagreed, they would wait on each other's barrier phases forever.
+struct TileWork {
+  int m_blk, n_blk, kb0, kb1;  // k blocks [kb0, kb1)
+};
+template <int MC>
+HCTR_DEVICE TileWork tile_work(const GemmParams& p, const int t, const int m_groups, const int cta_rank) {
+  const int split = t / (p.n_tiles * m_groups);
+  const int kb0 = split * p.kb_per_split;
+  return {((t / p.n_tiles) % m_groups) * MC + cta_rank, t % p.n_tiles, kb0, min(p.k_blocks, kb0 + p.kb_per_split)};
+}
+
+// hands an operand stage back to the producer of every CTA of the cluster (each of them multicast into it)
+template <int MC>
+HCTR_DEVICE void release_stage(uint64_t* empty) {
+  if constexpr (MC == 1) mbar_arrive(empty);
+  else
+    for (int r = 0; r < MC; ++r) mbar_arrive_cluster(empty, r);
 }
 
 // MC == 2: thread-block cluster of two CTAs stacked along M that share the B tile -- each CTA loads
@@ -177,9 +195,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
   using L = SmemLayout<BN, TMA_EPI>;
   constexpr int kStages = L::kStages;
   extern __shared__ uint8_t smem_raw[];
-  // aligned by an offset from smem_raw, so that the compiler keeps every derived pointer in the shared window: the
-  // TMA epilogue then reads and writes its boxes with 32-bit LDS / STS addresses instead of 64-bit generic ones
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_align1024(smem_raw);
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + kStages * L::kABytes;
   uint8_t* epi = smem + kStages * L::kStageBytes;
@@ -192,8 +208,6 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 
   const int wg = threadIdx.x >> 7;
   const int warp_idx = threadIdx.x >> 5;
-  // work items are (m-group of MC tiles, n tile, k split); the CTAs of a cluster take the MC
-  // consecutive m tiles of one item
   const int m_groups = (p.m_tiles + MC - 1) / MC;
   const int total_tiles = m_groups * p.n_tiles * p.splits;
   const int cta_rank = (MC > 1) ? static_cast<int>(cluster_ctarank()) : 0;
@@ -225,35 +239,30 @@ __global__ void __launch_bounds__(kNumThreads, 1)
     // ===================== TMA producer =====================
     asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
     if (warp_idx == 0 && elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
+      RingPos s;
       for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-        const int n_blk = t % p.n_tiles;
-        const int m_blk = ((t / p.n_tiles) % m_groups) * MC + cta_rank;
-        const int split = t / (p.n_tiles * m_groups);
-        const int kb0 = split * p.kb_per_split;
-        const int kb1 = min(p.k_blocks, kb0 + p.kb_per_split);
-        const int m0 = m_blk * BLOCK_M, n0 = n_blk * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          mbar_arrive_expect_tx(&full_bar[stage], L::kStageBytes);
-          uint8_t* sa = smem_a + stage * L::kABytes;
-          uint8_t* sb = smem_b + stage * L::kBBytes;
+        const TileWork w = tile_work<MC>(p, t, m_groups, cta_rank);
+        const int m0 = w.m_blk * BLOCK_M, n0 = w.n_blk * BN;
+        for (int kb = w.kb0; kb < w.kb1; ++kb) {
+          mbar_wait(&empty_bar[s.slot], s.phase ^ 1);
+          mbar_arrive_expect_tx(&full_bar[s.slot], L::kStageBytes);
+          uint8_t* sa = smem_a + s.slot * L::kABytes;
+          uint8_t* sb = smem_b + s.slot * L::kBBytes;
           const int k0 = kb * BLOCK_K;
           if constexpr (A_MN) {
 #pragma unroll
             for (int c = 0; c < BLOCK_M / 64; ++c)
-              tma_load_2d(sa + c * (BLOCK_K * 128), &tmA, &full_bar[stage], m0 + c * 64, k0);
+              tma_load_2d(sa + c * (BLOCK_K * 128), &tmA, &full_bar[s.slot], m0 + c * 64, k0);
           } else {
-            tma_load_2d(sa, &tmA, &full_bar[stage], k0, m0);
+            tma_load_2d(sa, &tmA, &full_bar[s.slot], k0, m0);
           }
           if constexpr (MC == 1) {
             if constexpr (B_MN) {
 #pragma unroll
               for (int c = 0; c < BN / 64; ++c)
-                tma_load_2d(sb + c * (BLOCK_K * 128), &tmB, &full_bar[stage], n0 + c * 64, k0);
+                tma_load_2d(sb + c * (BLOCK_K * 128), &tmB, &full_bar[s.slot], n0 + c * 64, k0);
             } else {
-              tma_load_2d(sb, &tmB, &full_bar[stage], k0, n0);
+              tma_load_2d(sb, &tmB, &full_bar[s.slot], k0, n0);
             }
           } else {
             // this CTA fetches its 1/MC share of the B tile and multicasts it to the whole cluster
@@ -264,21 +273,18 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 #pragma unroll
                 for (int c = 0; c < kChunks; ++c) {
                   const int cc = cta_rank * kChunks + c;
-                  tma_load_2d_mc(sb + cc * (BLOCK_K * 128), &tmB, &full_bar[stage], n0 + cc * 64, k0, kMask);
+                  tma_load_2d_mc(sb + cc * (BLOCK_K * 128), &tmB, &full_bar[s.slot], n0 + cc * 64, k0, kMask);
                 }
               } else if (cta_rank == 0) {  // BN == 64: one chunk, fetched by the first CTA
-                tma_load_2d_mc(sb, &tmB, &full_bar[stage], n0, k0, kMask);
+                tma_load_2d_mc(sb, &tmB, &full_bar[s.slot], n0, k0, kMask);
               }
             } else {
               constexpr int kRowsPer = BN / MC;
-              tma_load_2d_mc(sb + cta_rank * (kRowsPer * 128), &tmB, &full_bar[stage], k0,
+              tma_load_2d_mc(sb + cta_rank * (kRowsPer * 128), &tmB, &full_bar[s.slot], k0,
                              n0 + cta_rank * kRowsPer, kMask);
             }
           }
-          if (++stage == kStages) {
-            stage = 0;
-            phase ^= 1;
-          }
+          s.advance(kStages);
         }
       }
     } else if (TMA_EPI && warp_idx == 1 && epi_in_boxes(p.flags) > 0 && elect_one()) {
@@ -290,22 +296,20 @@ __global__ void __launch_bounds__(kNumThreads, 1)
       if (flags & EPI_CROSS) tma_prefetch_desc(&tmX0);
       if (flags & (EPI_CROSS | EPI_ADD)) tma_prefetch_desc(&tmXl);
       if (flags & EPI_MASK) tma_prefetch_desc(&tmMask);
-      int slot[2] = {0, 0};
-      uint32_t phase[2] = {0, 0};
+      RingPos pos[2];  // one ring per consumer warpgroup
       for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-        const int n_blk = t % p.n_tiles;
-        const int m_blk = ((t / p.n_tiles) % m_groups) * MC + cta_rank;
+        const TileWork w = tile_work<MC>(p, t, m_groups, cta_rank);
         for (int g = 0; g < BN / 64; ++g) {
-          const int n0 = n_blk * BN + g * 64;
+          const int n0 = w.n_blk * BN + g * 64;
           if (n0 >= p.N) break;
 #pragma unroll
           for (int cw = 0; cw < 2; ++cw) {
-            const int m0 = m_blk * BLOCK_M + cw * 64;
+            const int m0 = w.m_blk * BLOCK_M + cw * 64;
             if (m0 >= p.M) continue;
-            const int s = cw * kEpiBoxes + slot[cw];
-            mbar_wait(&epi_empty[s], phase[cw] ^ 1);
+            const int s = cw * kEpiBoxes + pos[cw].slot;
+            mbar_wait(&epi_empty[s], pos[cw].phase ^ 1);
             mbar_arrive_expect_tx(&epi_full[s], n_in * kEpiBoxBytes);
-            uint8_t* box = epi + (cw * kEpiBoxes + slot[cw] * n_in) * kEpiBoxBytes;
+            uint8_t* box = epi + (cw * kEpiBoxes + pos[cw].slot * n_in) * kEpiBoxBytes;
             if (flags & EPI_CROSS) {
               tma_load_2d(box, &tmX0, &epi_full[s], n0, m0);
               tma_load_2d(box + kEpiBoxBytes, &tmXl, &epi_full[s], n0, m0);
@@ -313,10 +317,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
               tma_load_2d(box, &tmXl, &epi_full[s], n0, m0);
             }
             if (flags & EPI_MASK) tma_load_2d(box + (n_in - 1) * kEpiBoxBytes, &tmMask, &epi_full[s], n0, m0);
-            if (++slot[cw] == slots) {
-              slot[cw] = 0;
-              phase[cw] ^= 1;
-            }
+            pos[cw].advance(slots);
           }
         }
       }
@@ -329,22 +330,16 @@ __global__ void __launch_bounds__(kNumThreads, 1)
     uint32_t* slab = reinterpret_cast<uint32_t*>(epi + cw * kEpiSlabBytes);
     uint8_t* ring = epi + cw * kEpiBoxes * kEpiBoxBytes;
     const int flags = p.flags;
-    int stage = 0;
-    uint32_t phase = 0;
-    int epi_slot = 0, epi_pending = -1;
-    uint32_t epi_phase = 0;
+    RingPos s, epi_pos;
+    int epi_pending = -1;
     float acc[BN / 2];
     for (int t = cluster_id; t < total_tiles; t += num_clusters) {
-      const int n_blk = t % p.n_tiles;
-      const int m_blk = ((t / p.n_tiles) % m_groups) * MC + cta_rank;
-      const int split = t / (p.n_tiles * m_groups);
-      const int kb0 = split * p.kb_per_split;
-      const int kb1 = min(p.k_blocks, kb0 + p.kb_per_split);
+      const TileWork w = tile_work<MC>(p, t, m_groups, cta_rank);
       int prev = -1;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t a_addr = smem_u32(smem_a + stage * L::kABytes) + cw * (64 * 128);
-        const uint32_t b_addr = smem_u32(smem_b + stage * L::kBBytes);
+      for (int kb = w.kb0; kb < w.kb1; ++kb) {
+        mbar_wait(&full_bar[s.slot], s.phase);
+        const uint32_t a_addr = smem_u32(smem_a + s.slot * L::kABytes) + cw * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem_b + s.slot * L::kBBytes);
         // K-major SW128 : 8-row atoms of 1024 B ; MN-major SW128: 64-wide chunks BLOCK_K*128 B
         // apart (LBO), 8-k-row groups 1024 B apart (SBO)
         const uint64_t a_desc = A_MN ? make_smem_desc_sw128(a_addr, BLOCK_K * 128, 1024)
@@ -359,7 +354,7 @@ __global__ void __launch_bounds__(kNumThreads, 1)
         for (int k = 0; k < BLOCK_K / WG_K; ++k)
           wgmma_tile<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, a_desc + static_cast<uint64_t>(k * a_step),
                                                       b_desc + static_cast<uint64_t>(k * b_step),
-                                                      (kb > kb0 || k > 0) ? 1u : 0u);
+                                                      (kb > w.kb0 || k > 0) ? 1u : 0u);
         wgmma_commit();
         wgmma_fence_regs(acc);
         if (TMA_EPI && epi_pending >= 0) {
@@ -372,32 +367,21 @@ __global__ void __launch_bounds__(kNumThreads, 1)
         }
         if (prev >= 0) {
           wgmma_wait<1>();  // the previous k block's wgmma has finished reading its slot
-          if (lane == 0) {
-            if constexpr (MC == 1) mbar_arrive(&empty_bar[prev]);
-            else
-              for (int r = 0; r < MC; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
-          }
+          if (lane == 0) release_stage<MC>(&empty_bar[prev]);
         }
-        prev = stage;
-        if (++stage == kStages) {
-          stage = 0;
-          phase ^= 1;
-        }
+        prev = s.slot;
+        s.advance(kStages);
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      if (prev >= 0 && lane == 0) {
-        if constexpr (MC == 1) mbar_arrive(&empty_bar[prev]);
-        else
-          for (int r = 0; r < MC; ++r) mbar_arrive_cluster(&empty_bar[prev], r);
-      }
+      if (prev >= 0 && lane == 0) release_stage<MC>(&empty_bar[prev]);
+      const int m_base = w.m_blk * BLOCK_M + cw * 64;
       if constexpr (TMA_EPI) {
-        if (m_blk * BLOCK_M + cw * 64 < p.M)
+        if (m_base < p.M)
           epilogue_tile_tma<BN>(p, flags, acc, ring, epi_full + cw * kEpiBoxes, epi_empty + cw * kEpiBoxes,
-                                &tmOut, &tmAux, m_blk * BLOCK_M + cw * 64, n_blk * BN, cw, epi_slot, epi_phase,
-                                epi_pending);
+                                &tmOut, &tmAux, m_base, w.n_blk * BN, cw, epi_pos, epi_pending);
       } else {
-        epilogue_tile_wg<BN>(p, flags, acc, slab, m_blk * BLOCK_M + cw * 64, n_blk * BN, cw);
+        epilogue_tile_wg<BN>(p, flags, acc, slab, m_base, w.n_blk * BN, cw);
       }
     }
     if (TMA_EPI && (threadIdx.x & 127) == 0) bulk_wait<0>();  // the stores are complete before the CTA exits
@@ -408,25 +392,6 @@ __global__ void __launch_bounds__(kNumThreads, 1)
 }
 
 // ------------------------------------------------------------------ host side
-typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                    const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                    const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static PFN_encodeTiled get_encode() {
-  static PFN_encodeTiled fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) !=
-            cudaSuccess ||
-        ptr == nullptr)
-      return nullptr;
-    fn = reinterpret_cast<PFN_encodeTiled>(ptr);
-  }
-  return fn;
-}
-
 // 2-D bf16 row-major tensor [outer, inner] with leading dimension ld (elements)
 static int make_tmap_bf16(CUtensorMap* m, const void* ptr, uint64_t inner, uint64_t outer,
                           uint64_t ld, uint32_t box_inner, uint32_t box_outer) {
@@ -447,17 +412,22 @@ struct EpiMaps {
   CUtensorMap out, aux, x0, xl, mask;
 };
 
-template <int BN, bool A_MN, bool B_MN, int MC, bool TMA_EPI>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& em, const GemmParams& p,
-                  cudaStream_t stream) {
+// one launcher per (BN, MC, TMA_EPI) over the four operand layouts (A_MN, B_MN)
+template <int BN, int MC, bool TMA_EPI>
+static int launch(const int a_mn, const int b_mn, const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& em,
+                  const GemmParams& p, cudaStream_t stream) {
   using L = SmemLayout<BN, TMA_EPI>;
-  static bool attr_set = false;
-  auto kern = gemm_tc_kernel<BN, A_MN, B_MN, MC, TMA_EPI>;
-  if (!attr_set) {
+  decltype(&gemm_tc_kernel<BN, false, false, MC, TMA_EPI>) const kernels[4] = {
+      gemm_tc_kernel<BN, false, false, MC, TMA_EPI>, gemm_tc_kernel<BN, false, true, MC, TMA_EPI>,
+      gemm_tc_kernel<BN, true, false, MC, TMA_EPI>, gemm_tc_kernel<BN, true, true, MC, TMA_EPI>};
+  const int layout = 2 * (a_mn != 0) + (b_mn != 0);
+  static bool attr_set[4] = {};
+  auto kern = kernels[layout];
+  if (!attr_set[layout]) {
     if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, L::kTotal) !=
         cudaSuccess)
       return -3;
-    attr_set = true;
+    attr_set[layout] = true;
   }
   const int m_groups = (p.m_tiles + MC - 1) / MC;
   const int total = m_groups * p.n_tiles * p.splits;       // cluster work items
@@ -483,32 +453,23 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const EpiMaps& e
 template <bool TMA_EPI>
 static int dispatch(int BN, int mc, int a_mn, int b_mn, const CUtensorMap& ta, const CUtensorMap& tb,
                     const EpiMaps& em, const GemmParams& p, cudaStream_t stream) {
-#define HCTR_DISPATCH(BNV, MCV)                                                             \
-  if (a_mn) {                                                                               \
-    if (b_mn) return launch<BNV, true, true, MCV, TMA_EPI>(ta, tb, em, p, stream);          \
-    return launch<BNV, true, false, MCV, TMA_EPI>(ta, tb, em, p, stream);                   \
-  } else {                                                                                  \
-    if (b_mn) return launch<BNV, false, true, MCV, TMA_EPI>(ta, tb, em, p, stream);         \
-    return launch<BNV, false, false, MCV, TMA_EPI>(ta, tb, em, p, stream);                  \
-  }
   if (mc == 2) {
-    if (BN == 256) { HCTR_DISPATCH(256, 2) }
-    if (BN == 64) { HCTR_DISPATCH(64, 2) }
-    HCTR_DISPATCH(128, 2)
+    if (BN == 256) return launch<256, 2, TMA_EPI>(a_mn, b_mn, ta, tb, em, p, stream);
+    if (BN == 64) return launch<64, 2, TMA_EPI>(a_mn, b_mn, ta, tb, em, p, stream);
+    return launch<128, 2, TMA_EPI>(a_mn, b_mn, ta, tb, em, p, stream);
   }
-  if (BN == 256) { HCTR_DISPATCH(256, 1) }
-  if (BN == 64) { HCTR_DISPATCH(64, 1) }
-  HCTR_DISPATCH(128, 1)
-#undef HCTR_DISPATCH
+  if (BN == 256) return launch<256, 1, TMA_EPI>(a_mn, b_mn, ta, tb, em, p, stream);
+  if (BN == 64) return launch<64, 1, TMA_EPI>(a_mn, b_mn, ta, tb, em, p, stream);
+  return launch<128, 1, TMA_EPI>(a_mn, b_mn, ta, tb, em, p, stream);
 }
 
-// The TMA epilogue takes bf16 outputs without addf whose slot holds at most two boxes, and whose epilogue tensors
-// TMA can address (16-byte bases and pitches) and bias, if any, is 8-byte aligned (float2 loads); it encodes
-// their maps into em.  Everything else runs the slab epilogue.
+// The TMA epilogue takes bf16 outputs whose slot holds at most two boxes, and whose epilogue tensors TMA can address
+// (16-byte bases and pitches) and bias, if any, is 8-byte aligned (float2 loads); it encodes their maps into em.
+// Everything else runs the slab epilogue.
 static bool tma_epilogue_maps(EpiMaps* em, int M, int N, int flags, const void* out, long long ldo, const void* aux,
                               long long ldaux, const void* x0, const void* xl, long long ldx, const void* mask,
-                              long long ldmask, const float* bias, const float* addf) {
-  if ((flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)) || addf != nullptr || epi_in_boxes(flags) > 2) return false;
+                              long long ldmask, const float* bias) {
+  if ((flags & (EPI_OUT_F32 | EPI_ATOMIC)) || epi_in_boxes(flags) > 2) return false;
   if (bias != nullptr && reinterpret_cast<uintptr_t>(bias) % 8) return false;
   auto map = [&](CUtensorMap* m, const void* ptr, long long ld) {
     return ptr != nullptr && reinterpret_cast<uintptr_t>(ptr) % 16 == 0 && ld >= N &&
@@ -529,7 +490,7 @@ using namespace hctr;
 
 // A: a_mn ? [K, M] row-major (lda) : [M, K] row-major (lda)
 // B: b_mn ? [K, N] row-major (ldb) : [N, K] row-major (ldb)
-// out: [M, N] row-major (ldo) bf16 (default) or fp32 (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)
+// out: [M, N] row-major (ldo) bf16 (default) or fp32 (EPI_OUT_F32 | EPI_ATOMIC)
 // block_n: BN in {64, 128, 256} (one CTA per tile) or 1000 + BN (2-CTA cluster sharing the B tile); other codes
 // >= 1000 are rejected (rc -11)
 extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, int N, int K,
@@ -537,7 +498,7 @@ extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, in
                               const float* bias, const void* mask, long long ldmask,
                               const void* x0, const void* xl, long long ldx, void* aux,
                               long long ldaux, float alpha, int flags, int splits, int block_n,
-                              const float* addf, long long ldaddf, void* stream_) {
+                              void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   if (M <= 0 || N <= 0 || K <= 0) return 0;
   if (block_n >= 2000) return -11;
@@ -558,7 +519,7 @@ extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, in
   p.mask = reinterpret_cast<const __nv_bfloat16*>(mask); p.ldmask = ldmask;
   p.x0 = reinterpret_cast<const __nv_bfloat16*>(x0);
   p.xl = reinterpret_cast<const __nv_bfloat16*>(xl); p.ldx = ldx;
-  p.alpha = alpha; p.flags = flags; p.addf = addf; p.ldaddf = ldaddf;
+  p.alpha = alpha; p.flags = flags;
 
   CUtensorMap ta, tb;
   int rc;
@@ -570,7 +531,7 @@ extern "C" int hctr_gemm_bf16(const void* A, const void* B, void* out, int M, in
   if (rc) return rc - 10;
 
   EpiMaps em;
-  if (tma_epilogue_maps(&em, M, N, flags, out, ldo, aux, ldaux, x0, xl, ldx, mask, ldmask, bias, addf))
+  if (tma_epilogue_maps(&em, M, N, flags, out, ldo, aux, ldaux, x0, xl, ldx, mask, ldmask, bias))
     return dispatch<true>(BN, mc, a_mn, b_mn, ta, tb, em, p, stream);
   return dispatch<false>(BN, mc, a_mn, b_mn, ta, tb, em, p, stream);
 }

@@ -16,7 +16,6 @@ from .. import _native
 EPI_RELU = 1
 EPI_OUT_F32 = 2
 EPI_ATOMIC = 4
-EPI_ACCUM = 8
 EPI_CROSS = 16
 EPI_MASK = 32
 EPI_SIGMOID = 64
@@ -35,8 +34,7 @@ def _lib():
             _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_int, _c.c_int, _c.c_int,
             _c.c_longlong, _c.c_longlong, _c.c_longlong, _c.c_int, _c.c_int,
             _c.c_void_p, _c.c_void_p, _c.c_longlong, _c.c_void_p, _c.c_void_p, _c.c_longlong,
-            _c.c_void_p, _c.c_longlong, _c.c_float, _c.c_int, _c.c_int, _c.c_int, _c.c_void_p,
-            _c.c_longlong, _c.c_void_p]
+            _c.c_void_p, _c.c_longlong, _c.c_float, _c.c_int, _c.c_int, _c.c_int, _c.c_void_p]
         _sig_set = True
     return lib
 
@@ -55,11 +53,11 @@ def tc_eligible(a: torch.Tensor, b: torch.Tensor, a_mn: bool, b_mn: bool) -> boo
     return True
 
 
-def epi_eligible(M: int, N: int, out, bias=None, mask=None, x0=None, xl=None, aux=None, addf=None) -> bool:
+def epi_eligible(M: int, N: int, out, bias=None, mask=None, x0=None, xl=None, aux=None) -> bool:
     """The kernel's epilogue reads and writes its tensors row-major with unit column stride, and from N >= 32 on in
     16-byte vectors or TMA boxes at every 32-column chunk of a row: 16-byte bases and row pitches.  x0 and xl
     share one pitch."""
-    for t in (out, mask, x0, xl, aux, addf):
+    for t in (out, mask, x0, xl, aux):
         if t is None:
             continue
         if t.dim() != 2 or t.stride(1) != 1:
@@ -74,7 +72,7 @@ def epi_eligible(M: int, N: int, out, bias=None, mask=None, x0=None, xl=None, au
 
 
 def gemm_reference(a, b, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, xl=None,
-                   alpha=1.0, flags=0, out=None, aux=None, addf=None):
+                   alpha=1.0, flags=0, out=None, aux=None):
     """fp32 PyTorch oracle with the same epilogue semantics as the kernel."""
     A = a.float().t() if a_mn else a.float()          # [M, K]
     B = b.float() if b_mn else b.float().t()          # [K, N]
@@ -87,15 +85,13 @@ def gemm_reference(a, b, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, 
         v = x0.float() * v + xl.float()
     if flags & EPI_ADD:
         v = v + xl.float()
-        if addf is not None:
-            v = v + addf.float()
     if flags & EPI_MASK:
         v = v * (mask.float() > 0)
     if flags & EPI_RELU:
         v = torch.relu(v)
     if flags & EPI_SIGMOID:
         v = torch.sigmoid(v)
-    if flags & (EPI_ATOMIC | EPI_ACCUM):
+    if flags & EPI_ATOMIC:
         out.add_(v.to(out.dtype))
         return out
     odt = torch.float32 if (flags & EPI_OUT_F32) else a.dtype
@@ -120,12 +116,12 @@ def set_impl(name: str):
 
 
 def gemm_library(a, b, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, xl=None,
-                 alpha=1.0, flags=0, out=None, aux=None, addf=None):
+                 alpha=1.0, flags=0, out=None, aux=None):
     """Same contract as ``gemm_reference`` with the matmul in the operands' dtype on the vendor
     library (what a cuBLASLt-based framework runs): bias through addmm, the rest eager."""
     A = a.t() if a_mn else a
     B = b if b_mn else b.t()
-    f32 = bool(flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM))
+    f32 = bool(flags & (EPI_OUT_F32 | EPI_ATOMIC))
     if f32:
         v = torch.mm(A, B).float()
         if alpha != 1.0:
@@ -146,15 +142,13 @@ def gemm_library(a, b, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, xl
         v = torch.addcmul(xl.to(v.dtype), x0.to(v.dtype), v)
     if flags & EPI_ADD:
         v = v + xl.to(v.dtype)
-        if addf is not None:
-            v = v + addf.to(v.dtype)
     if flags & EPI_MASK:
         v = v * (mask > 0).to(v.dtype)
     if flags & EPI_RELU:
         v = torch.relu(v)
     if flags & EPI_SIGMOID:
         v = torch.sigmoid(v)
-    if flags & (EPI_ATOMIC | EPI_ACCUM):
+    if flags & EPI_ATOMIC:
         out.add_(v.to(out.dtype))
         return out
     if out is None:
@@ -186,7 +180,7 @@ def _pick_block_n(M, N, K, splits):
 
 
 def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x0=None, xl=None,
-              aux=None, alpha=1.0, flags=0, splits=1, block_n=0, addf=None, colsum=None):
+              aux=None, alpha=1.0, flags=0, splits=1, block_n=0, colsum=None):
     """out[M,N] = epilogue(alpha * op(a) @ op(b)).
 
     ``colsum`` (fp32 [N], optional): += column sums of the bf16 output, i.e. the bias gradient of the
@@ -197,16 +191,16 @@ def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x
     M = a.shape[1] if a_mn else a.shape[0]
     K = a.shape[0] if a_mn else a.shape[1]
     N = b.shape[1] if b_mn else b.shape[0]
-    f32_out = bool(flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM))
+    f32_out = bool(flags & (EPI_OUT_F32 | EPI_ATOMIC))
     if out is None:
         out = torch.empty(M, N, device=a.device, dtype=torch.float32 if f32_out else a.dtype)
     if IMPL == "library" and a.is_cuda:
-        r = gemm_library(a, b, a_mn, b_mn, bias, mask, x0, xl, alpha, flags, out, aux, addf)
+        r = gemm_library(a, b, a_mn, b_mn, bias, mask, x0, xl, alpha, flags, out, aux)
         if colsum is not None:
             colsum.add_(out.float().sum(0))
         return r
     operands_ok = tc_eligible(a, b, a_mn, b_mn)
-    if not operands_ok or not epi_eligible(M, N, out, bias, mask, x0, xl, aux, addf):
+    if not operands_ok or not epi_eligible(M, N, out, bias, mask, x0, xl, aux):
         if a.is_cuda:
             # never silent: a misaligned / non-bf16 operand or epilogue tensor moves this GEMM off the wgmma kernel
             sig = (M, N, K, str(a.dtype), tuple(a.stride()), tuple(b.stride()), a.data_ptr() % 16,
@@ -214,34 +208,32 @@ def gemm_bf16(a, b, out=None, *, a_mn=False, b_mn=False, bias=None, mask=None, x
             if sig not in _fallback_logged:
                 _fallback_logged.add(sig)
                 from ..utils import logger
-                what = (f"an epilogue tensor (out / bias / mask / x0 / xl / aux / addf, flags={flags})" if operands_ok
+                what = (f"an epilogue tensor (out / bias / mask / x0 / xl / aux, flags={flags})" if operands_ok
                         else f"dtype={a.dtype} strides a={tuple(a.stride())} b={tuple(b.stride())}")
                 logger.warning(f"gemm_bf16: M={M} N={N} K={K} {what} is not TMA-addressable (16-byte base / pitch, "
                                "bf16): running the library matmul instead of the wgmma kernel")
-        r = gemm_reference(a, b, a_mn, b_mn, bias, mask, x0, xl, alpha, flags, out, aux, addf)
+        r = gemm_reference(a, b, a_mn, b_mn, bias, mask, x0, xl, alpha, flags, out, aux)
         if colsum is not None:
             colsum.add_(out.float().sum(0))
         return r
     if splits > 1:
         flags |= EPI_ATOMIC
     if block_n == 0:
-        block_n = _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags,
-                                 splits, addf)
-    _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, block_n, addf)
+        block_n = _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits)
+    _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, block_n)
     if colsum is not None:
         from . import dense as _D
         _D.colsum_accum(out, colsum)
     return out
 
 
-def _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, block_n, addf):
+def _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, block_n):
     stream = torch.cuda.current_stream(a.device).cuda_stream
     args = [a.data_ptr(), b.data_ptr(), out.data_ptr(), M, N, K, a.stride(0), b.stride(0),
             out.stride(0), int(a_mn), int(b_mn), _ptr(bias), _ptr(mask),
             0 if mask is None else mask.stride(0), _ptr(x0), _ptr(xl),
             0 if xl is None else xl.stride(0), _ptr(aux), 0 if aux is None else aux.stride(0),
-            float(alpha), int(flags), int(splits), int(block_n), _ptr(addf),
-            0 if addf is None else addf.stride(0), stream]
+            float(alpha), int(flags), int(splits), int(block_n), stream]
     rc = _lib().hctr_gemm_bf16(*args)
     if rc != 0:
         raise RuntimeError(f"hctr_gemm_bf16 failed rc={rc} M={M} N={N} K={K}")
@@ -257,7 +249,7 @@ def _launch(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flag
 _TUNE_CACHE = {}
 
 
-def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits, addf):
+def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alpha, flags, splits):
     import os
     heur = _pick_block_n(M, N, K, splits)
     if heur < 1000 or os.environ.get("HCTR_GEMM_AUTOTUNE", "1") == "0" or os.environ.get("HCTR_GEMM_BN"):
@@ -270,20 +262,20 @@ def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alph
     if torch.cuda.is_current_stream_capturing():
         return heur
     cands = [1128, 1256] if N >= 256 else [1128]
-    if not (flags & (EPI_OUT_F32 | EPI_ATOMIC | EPI_ACCUM)):
+    if not (flags & (EPI_OUT_F32 | EPI_ATOMIC)):
         # with the TMA epilogue, memory-bound bf16-output calls can win on more, narrower tiles
         cands = [1064] + cands + [64, 128, 256]
     if len(cands) == 1:
         _TUNE_CACHE[key] = cands[0]
         return cands[0]
     so = torch.empty_strided(out.size(), out.stride(), dtype=out.dtype, device=out.device)
-    if flags & (EPI_ATOMIC | EPI_ACCUM):
+    if flags & EPI_ATOMIC:
         so.zero_()
     sa = (torch.empty_strided(aux.size(), aux.stride(), dtype=aux.dtype, device=aux.device)
           if aux is not None else None)
     for bn in cands:
         for _ in range(2):
-            _launch(a, b, so, M, N, K, a_mn, b_mn, bias, mask, x0, xl, sa, alpha, flags, splits, bn, addf)
+            _launch(a, b, so, M, N, K, a_mn, b_mn, bias, mask, x0, xl, sa, alpha, flags, splits, bn)
     # candidates alternate over the rounds so that a slow spell of a shared GPU does not decide the pick
     times = {bn: [] for bn in cands}
     for _ in range(3):
@@ -291,7 +283,7 @@ def _tuned_block_n(a, b, out, M, N, K, a_mn, b_mn, bias, mask, x0, xl, aux, alph
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
             for _ in range(5):
-                _launch(a, b, so, M, N, K, a_mn, b_mn, bias, mask, x0, xl, sa, alpha, flags, splits, bn, addf)
+                _launch(a, b, so, M, N, K, a_mn, b_mn, bias, mask, x0, xl, sa, alpha, flags, splits, bn)
             e1.record()
             e1.synchronize()
             times[bn].append(e0.elapsed_time(e1))

@@ -13,7 +13,7 @@ def _bf(*shape):
 def test_aligned_epilogue_tensors_are_eligible():
     M, N = 64, 96
     assert G.epi_eligible(M, N, _bf(M, N), bias=torch.zeros(N), mask=_bf(M, N), x0=_bf(M, N), xl=_bf(M, N),
-                          aux=_bf(M, N), addf=torch.zeros(M, N))
+                          aux=_bf(M, N))
 
 
 def test_misaligned_base_or_pitch_is_not_eligible():
@@ -24,7 +24,6 @@ def test_misaligned_base_or_pitch_is_not_eligible():
     assert not G.epi_eligible(M, N, _bf(M, N), mask=_bf(M, N + 4)[:, :N])
     assert not G.epi_eligible(M, N, _bf(M, N), aux=big[:, 1:N + 1])
     assert not G.epi_eligible(M, N, _bf(M, N), bias=torch.zeros(N + 1)[1:])
-    assert not G.epi_eligible(M, N, _bf(M, N), addf=torch.zeros(M, N + 1)[:, :N])
     assert not G.epi_eligible(M, N, _bf(N, M).t())                       # column stride != 1
     assert not G.epi_eligible(M, N, _bf(M, N), x0=_bf(M, N + 8)[:, :N], xl=_bf(M, N))   # x0 / xl pitches differ
 

@@ -17,7 +17,7 @@ the tile the autotuner picked for ours (gemm_bf16's block_n code).
 process per run in one session.  Without a CUDA device the tool exits with an error and measures nothing.
 
 --check-bits OTHER_TREE times nothing: it replays every recorded call that does not accumulate into its output
-(no EPI_ATOMIC / EPI_ACCUM, no split K) on the same seeded operands under this tree and under OTHER_TREE, one
+(no EPI_ATOMIC, no split K) on the same seeded operands under this tree and under OTHER_TREE, one
 process each, and reports per call whether `out` and `aux` are equal bit for bit.  The K order of the
 accumulation does not depend on the tile, so two builds that tune to different tiles still agree.
 """
@@ -32,7 +32,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PEAK_FLOPS, PEAK_BW = 989e12, 3.35e12
-TENSORS = ("a", "b", "out", "bias", "mask", "x0", "xl", "aux", "addf", "colsum")
+TENSORS = ("a", "b", "out", "bias", "mask", "x0", "xl", "aux", "colsum")
 
 
 def card():
@@ -110,7 +110,7 @@ def nbytes(c):
             for s in shape:
                 n *= s
             total += n * torch.empty(0, dtype=getattr(torch, dt)).element_size()
-    if c["flags"] & 12 or c["splits"] > 1:          # EPI_ATOMIC / EPI_ACCUM read the output as well
+    if c["flags"] & 4 or c["splits"] > 1:           # EPI_ATOMIC reads the output as well
         shape, _, _ = c["out"]
         total += shape[0] * shape[1] * 4
     return total
@@ -142,7 +142,7 @@ def output_digests(batch):
     res = []
     for i, c in enumerate(calls):
         ts = make_operands(c, gen)
-        if c["flags"] & (G.EPI_ATOMIC | G.EPI_ACCUM) or c["splits"] > 1:
+        if c["flags"] & G.EPI_ATOMIC or c["splits"] > 1:
             continue
         kw = dict(a_mn=c["a_mn"], b_mn=c["b_mn"], flags=c["flags"], splits=c["splits"], alpha=c["alpha"])
         kw.update({k: ts[k] for k in TENSORS[3:] if k in ts and k != "colsum"})
