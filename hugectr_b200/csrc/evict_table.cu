@@ -4,11 +4,13 @@
 //
 // One training lookup of a table is two passes over its key regions, every region of the table through
 // the first pass before any region goes through the second:
-//   touch   a present key stamps its way with the collection clock and counts the occurrence;
+//   touch   a present key stamps its way with the collection clock and counts the occurrence (an admitting
+//           table counts a missing key's occurrence in its admission sketch instead, admit_sketch.cuh);
 //   insert  every key gets its row, written in place over the key (the lookup kernels then run as for a
 //           static table); a missing key takes, under its set's lock, an empty way or else the unprotected
 //           way with the smallest (stamp, key) (LRU) or (count, stamp, key) (LFU).  A way stamped with the
 //           current clock is protected, so every key of the running step keeps its row for the whole step.
+//           An admitting table first rejects a missing key whose sketch count is below its threshold.
 // Then the re-initialisation kernel gives every admitted row fresh weights and optimizer state.
 // Evaluation uses the get kernel only.  Everything reads the clock from device memory: no host input,
 // so the whole step is captured in one CUDA graph.
@@ -16,6 +18,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "admit_sketch.cuh"
 #include "embedding.cuh"
 #include "set_assoc.cuh"
 
@@ -63,8 +66,9 @@ HCTR_DEVICE long long evict_set_base(const EvictTableView& t, long long key) {
   return static_cast<long long>(set) * kEvictWays;
 }
 
-template <typename KT>
-__global__ void __launch_bounds__(256) evict_touch_kernel(EvictTableView t, KeyRegion r) {
+// kAdmit (admit_threshold > 1): an occurrence of a missing key is counted in the admission sketch
+template <typename KT, bool kAdmit>
+__global__ void __launch_bounds__(256) evict_touch_kernel(EvictTableView t, KeyRegion r, AdmitSketch s) {
   const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= r.n * r.ranks) return;
@@ -72,6 +76,12 @@ __global__ void __launch_bounds__(256) evict_touch_kernel(EvictTableView t, KeyR
   if (!owned(r, key)) return;
   const long long base = evict_set_base(t, key);
   const int slot = warp_find(t.keys + base, kEvictWays, key, lane);
+  if constexpr (kAdmit) {
+    if (slot < 0 && lane == 0) {
+      sketch_count(s, key);
+      atomicAdd(&s.stats[0], 1ull);
+    }
+  }
   if (slot < 0 || lane != 0) return;
   const long long g = base + slot;
   // a hot key is touched by many warps: store the stamp once, count with one atomic each
@@ -81,10 +91,11 @@ __global__ void __launch_bounds__(256) evict_touch_kernel(EvictTableView t, KeyR
 }
 
 // kEvict = false (checkpoint load): only empty ways are taken, a full set drops the key.
+// kAdmit: a missing key below the admission threshold is rejected before its set lock (row -1, counted).
 // adm (optional): the admitted ways are appended to adm[0 .. *adm_n) for the re-initialisation.
-template <typename KT, bool kEvict>
-__global__ void __launch_bounds__(256)
-    evict_insert_kernel(EvictTableView t, KeyRegion r, long long* __restrict__ adm, int* __restrict__ adm_n) {
+template <typename KT, bool kEvict, bool kAdmit>
+__global__ void __launch_bounds__(256) evict_insert_kernel(EvictTableView t, KeyRegion r, long long* __restrict__ adm,
+                                                           int* __restrict__ adm_n, AdmitSketch s) {
   const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= r.n * r.ranks) return;
@@ -98,7 +109,14 @@ __global__ void __launch_bounds__(256)
   const long long base = evict_set_base(t, key);
   // A key of the running step found here stays: it was touched (protected) or inserted this step.
   int slot = warp_find(t.keys + base, kEvictWays, key, lane);
-  if (slot < 0) {
+  bool admit = true;
+  if constexpr (kAdmit) {
+    if (slot < 0 && !sketch_admits(s, key)) {
+      admit = false;
+      if (lane == 0) atomicAdd(&s.stats[1], 1ull);
+    }
+  }
+  if (slot < 0 && admit) {
     const int set = static_cast<int>(base / kEvictWays);
     lock_set(t.locks, set, lane);
     volatile long long* vk = t.keys + base;
@@ -245,20 +263,26 @@ int launch_by_key(const KeyRegion& r, cudaStream_t st, A... a) {
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 
+// s: the shard's admission sketch, or nullptr (no admission: today's instantiations)
 template <typename KT>
 struct TouchL {
-  static void launch(unsigned g, cudaStream_t st, const KeyRegion& r, const EvictTableView& t) {
-    evict_touch_kernel<KT><<<g, 256, 0, st>>>(t, r);
+  static void launch(unsigned g, cudaStream_t st, const KeyRegion& r, const EvictTableView& t, const AdmitSketch* s) {
+    if (s)
+      evict_touch_kernel<KT, true><<<g, 256, 0, st>>>(t, r, *s);
+    else
+      evict_touch_kernel<KT, false><<<g, 256, 0, st>>>(t, r, AdmitSketch{});
   }
 };
 template <typename KT>
 struct InsertL {
   static void launch(unsigned g, cudaStream_t st, const KeyRegion& r, const EvictTableView& t, long long* adm,
-                     int* adm_n, int evict) {
-    if (evict)
-      evict_insert_kernel<KT, true><<<g, 256, 0, st>>>(t, r, adm, adm_n);
+                     int* adm_n, int evict, const AdmitSketch* s) {
+    if (s && evict)
+      evict_insert_kernel<KT, true, true><<<g, 256, 0, st>>>(t, r, adm, adm_n, *s);
+    else if (evict)
+      evict_insert_kernel<KT, true, false><<<g, 256, 0, st>>>(t, r, adm, adm_n, AdmitSketch{});
     else
-      evict_insert_kernel<KT, false><<<g, 256, 0, st>>>(t, r, adm, adm_n);
+      evict_insert_kernel<KT, false, false><<<g, 256, 0, st>>>(t, r, adm, adm_n, AdmitSketch{});
   }
 };
 template <typename KT>
@@ -272,13 +296,14 @@ struct GetL {
 
 using namespace hctr;
 
-extern "C" int hctr_evict_touch(const EvictTableView* t, const KeyRegion* r, void* stream) {
-  return launch_by_key<TouchL>(*r, (cudaStream_t)stream, *t);
+// s (optional): the admission sketch of an admitting shard; the insert applies it only when evicting
+extern "C" int hctr_evict_touch(const EvictTableView* t, const KeyRegion* r, const AdmitSketch* s, void* stream) {
+  return launch_by_key<TouchL>(*r, (cudaStream_t)stream, *t, s);
 }
 
 extern "C" int hctr_evict_insert(const EvictTableView* t, const KeyRegion* r, long long* adm, int* adm_n,
-                                 int evict, void* stream) {
-  return launch_by_key<InsertL>(*r, (cudaStream_t)stream, *t, adm, adm_n, evict);
+                                 int evict, const AdmitSketch* s, void* stream) {
+  return launch_by_key<InsertL>(*r, (cudaStream_t)stream, *t, adm, adm_n, evict, s);
 }
 
 extern "C" int hctr_evict_get(const EvictTableView* t, const KeyRegion* r, void* stream) {

@@ -6,6 +6,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "admit_sketch.cuh"
 #include "embedding.cuh"
 
 namespace hctr {
@@ -137,6 +138,43 @@ __global__ void ht_translate_kernel(HashTableView t, const long long* __restrict
   out[i] = -1;
 }
 
+// ---- admission of a growing dynamic table (admit_threshold > 1, admit_sketch.cuh).  A training lookup runs
+// the count kernel over every key region of the table, then the filter kernel and the get-insert per region.
+
+// whether `key` has a slot (read-only probe; no insert of the table runs concurrently)
+HCTR_DEVICE bool ht_has(const HashTableView& t, unsigned long long k) {
+  unsigned long long h = hash64(k) & t.capacity_mask;
+  for (unsigned long long probes = 0; probes <= t.capacity_mask; ++probes) {
+    const unsigned long long prev = t.keys[h];
+    if (prev == k) return true;
+    if (prev == kEmptyKey) return false;
+    h = (h + 1) & t.capacity_mask;
+  }
+  return false;
+}
+
+// keys >= 0 (the owned ones) without a slot count one occurrence each
+__global__ void __launch_bounds__(256) ht_admit_count_kernel(HashTableView t, const long long* __restrict__ keys,
+                                                             long long n, AdmitSketch s) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long key = i < n ? keys[i] : -1;
+  const bool miss = key >= 0 && !ht_has(t, static_cast<unsigned long long>(key));
+  if (miss) sketch_count(s, key);
+  const unsigned m = __ballot_sync(0xffffffffu, miss);
+  if ((threadIdx.x & 31) == 0 && m) atomicAdd(&s.stats[0], static_cast<unsigned long long>(__popc(m)));
+}
+
+// keys >= 0 without a slot whose count is below the threshold become -1 (rejected, counted), in place
+__global__ void __launch_bounds__(256) ht_admit_filter_kernel(HashTableView t, long long* __restrict__ keys,
+                                                              long long n, AdmitSketch s) {
+  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  const long long key = i < n ? keys[i] : -1;
+  const bool rej = key >= 0 && !ht_has(t, static_cast<unsigned long long>(key)) && !sketch_admits(s, key);
+  if (rej) keys[i] = -1;
+  const unsigned m = __ballot_sync(0xffffffffu, rej);
+  if ((threadIdx.x & 31) == 0 && m) atomicAdd(&s.stats[1], static_cast<unsigned long long>(__popc(m)));
+}
+
 __global__ void ht_set_kernel(HashTableView t, const long long* __restrict__ keys,
                               const long long* __restrict__ vals, long long n) {
   const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
@@ -209,5 +247,18 @@ extern "C" int hctr_ht_dump(void* keys_tab, void* vals_tab, unsigned long long c
   HashTableView t{(unsigned long long*)keys_tab, (long long*)vals_tab, nullptr, capacity - 1, 0};
   ht_dump_kernel<<<(unsigned)((capacity + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
       t, out_keys, out_vals, (unsigned long long*)out_count, capacity);
+  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+// filter = 0: count the missing keys of `keys`; 1: reject the missing keys below the threshold (in place)
+extern "C" int hctr_ht_admit(void* keys_tab, unsigned long long capacity, long long* keys, long long n,
+                             const AdmitSketch* sketch, int filter, void* stream) {
+  if (n == 0) return 0;
+  HashTableView t{(unsigned long long*)keys_tab, nullptr, nullptr, capacity - 1, 0};
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  if (filter)
+    ht_admit_filter_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(t, keys, n, *sketch);
+  else
+    ht_admit_count_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(t, keys, n, *sketch);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -17,6 +17,7 @@ the pooled vectors travel through variable-size all-to-alls.
 from __future__ import annotations
 
 import math
+import numbers
 import os
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
@@ -81,6 +82,22 @@ class EmbeddingTableConfig:
                 raise ValueError(f"table {self.name}: evict_strategy needs a dynamic table (max_vocabulary_size=-1)")
             if self.max_capacity <= 0:
                 raise ValueError(f"table {self.name}: evict_strategy needs max_capacity > 0 (rows per shard)")
+        # admission (see docs/embedding.md): a dynamic table gives a missing key a row only once a count-min
+        # sketch of its shard counted admit_threshold occurrences of it (1: every key, no sketch);
+        # admit_decay_steps = P > 0 halves the counts every P training steps (0: never)
+        self.admit_threshold = kw.get("admit_threshold", 1)
+        self.admit_decay_steps = kw.get("admit_decay_steps", 0)
+        from .hashtable import SKETCH_MAX
+        for opt, lo in (("admit_threshold", 1), ("admit_decay_steps", 0)):
+            v = getattr(self, opt)
+            if isinstance(v, bool) or not isinstance(v, numbers.Integral) or not lo <= v <= SKETCH_MAX:
+                raise ValueError(f"table {self.name}: {opt} must be an int in [{lo}, {SKETCH_MAX}], not {v!r}")
+            if opt in kw and not self.dynamic:
+                raise ValueError(f"table {self.name}: {opt} needs a dynamic table (max_vocabulary_size=-1)")
+            setattr(self, opt, int(v))
+        if self.admit_decay_steps > 0 and self.admit_threshold == 1:
+            raise ValueError(f"table {self.name}: admit_decay_steps needs admit_threshold > 1 (a threshold of 1 "
+                             "keeps no counts)")
 
 
 class EmbeddingCollectionConfig:
@@ -274,6 +291,9 @@ class EmbeddingCollection:
             if t.evict_strategy is not None and (pl.kind != "mp" or pl.col_factor > 1):
                 raise ValueError(f"table {t.name}: an evicting table is model parallel, table-wise or row-wise "
                                  f"(placement {pl.kind!r}, column factor {pl.col_factor})")
+            if t.admit_threshold > 1 and (pl.kind != "mp" or pl.col_factor > 1):
+                raise ValueError(f"table {t.name}: an admitting table (admit_threshold > 1) is model parallel, "
+                                 f"table-wise or row-wise (placement {pl.kind!r}, column factor {pl.col_factor})")
         self.native = device.type == "cuda"
         self.has_dynamic = any(t.dynamic for t in self.tables)
         self.fused = (self.native and self.world > 1 and comm.p2p_available) if fused is None else fused
@@ -299,7 +319,9 @@ class EmbeddingCollection:
         self._abf = act_dtype == torch.bfloat16
         # clock of the evicting tables: ticked once per training step inside the step (not Model.step_t,
         # which a learning-rate scheduler reset zeroes and Adam's bias correction reads)
+        # and of the admitting tables' sketch decay
         self.evict_clock = torch.zeros(1, dtype=torch.int64, device=device)
+        self.ticks_clock = any(t.evict_strategy is not None or t.admit_threshold > 1 for t in self.tables)
         self._build_layout(hotness)
         self._build_storage(seed)
         self._alloc_buffers()
@@ -411,10 +433,11 @@ class EmbeddingCollection:
                 # no owner-side lookup descriptors, no per-shard partial blocks
                 gl["unique"], gl["unique_owners"] = True, list(pl.shard_gpus)
                 continue
-            # (not for evicting tables: their owners translate the raw keys of the whole bag; not for
-            # weighted lookups: their owners read each key's weight at the key's own position)
+            # (not for evicting or admitting tables: their owners translate the raw keys of the whole bag;
+            # not for weighted lookups: their owners read each key's weight at the key's own position)
+            tc = self.tmap[gl["table"]]
             if getattr(self, "shard_split", False) and pl.kind == "mp" and k > 1 and pl.col_factor == 1 \
-                    and gl["combiner"] == "sum" and self.tmap[gl["table"]].evict_strategy is None \
+                    and gl["combiner"] == "sum" and tc.evict_strategy is None and tc.admit_threshold == 1 \
                     and not gl["weighted"]:
                 # Requester-side split: every rank rewrites its bag of a row-sharded table into k
                 # compacted per-shard lists of LOCAL ROW INDICES (key // k) plus their lengths, stored
@@ -559,8 +582,8 @@ class EmbeddingCollection:
                 po += R * self.b * l.hotness
             grp.lookups_dev = E.lookups_to_device(grp.lookups, dev)
             for sl in grp.table_slices:
-                if sl["evict"]:
-                    self._dyn_hash(sl["table"], sl)
+                if sl["evict"] or (sl["dynamic"] and self.tmap[sl["table"]].admit_threshold > 1):
+                    self._dyn_hash(sl["table"], sl)         # (an admitting shard's sketch: allocated here, once)
             pairs = po
             if self.is_train:
                 if grp.kind == "mp":
@@ -871,12 +894,22 @@ class EmbeddingCollection:
             owner._dyn_tables = {}
         key = (name, sl["cpart"], sl["s"])
         if key not in owner._dyn_tables:
+            from .hashtable import AdmitSketch
+            t = self.tmap[name]
+            sketch = None
+            if t.admit_threshold > 1:
+                # sized by the shard's rows at construction (an evicting shard's capacity, a growing shard's
+                # initial rows), never resized
+                sketch = AdmitSketch(sl["rows"], t.admit_threshold, t.admit_decay_steps, owner.evict_clock,
+                                     self.device)
             if sl.get("evict"):
                 from .hashtable import SetAssocTable
-                owner._dyn_tables[key] = SetAssocTable(sl["rows"], sl["evict"], owner.evict_clock, self.device)
+                owner._dyn_tables[key] = SetAssocTable(sl["rows"], sl["evict"], owner.evict_clock, self.device,
+                                                       sketch=sketch)
             else:
                 from .hashtable import HashTable
                 owner._dyn_tables[key] = HashTable(sl["rows"], self.device)
+                owner._dyn_tables[key].sketch = sketch
         return owner._dyn_tables[key]
 
     def _evicting_lookups(self):
@@ -912,13 +945,11 @@ class EmbeddingCollection:
         return E.evict_init_key(self.seed, _stable_seed("evict_init", name))
 
     def _translate_evicting(self, buf):
-        """Evicting tables (see csrc/evict_table.cu): a training lookup ticks the clock, touches every key
-        region of a table, then inserts into every region (rows in place over the keys), then re-initialises
-        the admitted rows; an evaluation lookup only reads.  No host synchronisation."""
+        """Evicting tables (see csrc/evict_table.cu): a training lookup touches every key region of a table
+        (counting the missing keys of an admitting table), then inserts into every region (rows in place over
+        the keys), then re-initialises the admitted rows; an evaluation lookup only reads.  No host
+        synchronisation."""
         b = self.b
-        owner = getattr(self, "_shared", self)
-        if self.is_train:
-            owner.evict_clock.add_(1)
         for name, gls in self._evicting_lookups().items():
             regs = [(gl["key_off"], b * gl["hotness"]) for gl in gls]
             loc = self._evict_local(name)
@@ -952,19 +983,45 @@ class EmbeddingCollection:
         return {(name, s_): dict(zip(("live", "admitted", "evicted", "dropped"), (int(x) for x in v)))
                 for ((name, _, s_), _), v in zip(items, vals)}
 
+    def _admit_sketches(self):
+        """the admission sketches of the dynamic shards held here"""
+        owner = getattr(self, "_shared", self)
+        return [ht.sketch for ht in getattr(owner, "_dyn_tables", {}).values() if getattr(ht, "sketch", None) is not None]
+
+    def admission_stats(self):
+        """{(table, shard): {counted, rejected}} of the admitting tables held here: cumulative device counters of
+        the counted occurrences and the rejected key positions, read with one host synchronisation (call it
+        outside the step)"""
+        owner = getattr(self, "_shared", self)
+        items = [(k, ht.sketch) for k, ht in getattr(owner, "_dyn_tables", {}).items()
+                 if getattr(ht, "sketch", None) is not None]
+        if not items:
+            return {}
+        vals = torch.stack([sk.stats for _, sk in items]).cpu().tolist()
+        return {(name, s_): dict(zip(("counted", "rejected"), (int(x) for x in v)))
+                for ((name, _, s_), _), v in zip(items, vals)}
+
     def _translate_dynamic_keys(self):
         """Dynamic tables: overwrite the (gathered) keys of their lookups with local row indices -- new
         keys get the next free row while training, unknown keys read as empty (-1) in evaluation; keys
-        owned by another shard become -1.  The lookup kernels then run exactly as for static tables."""
+        owned by another shard become -1.  The lookup kernels then run exactly as for static tables.
+        A training step first ticks the clock of the evicting and admitting tables and decays the sketches
+        that are due; an admitting table counts its missing keys in every region before any insert, then
+        rejects the keys below its threshold (-1) ahead of each insert."""
         b = self.b
         buf = self.key_slab.view(1, -1) if self.world == 1 else self.key_chans[0].all
+        if self.is_train and self.ticks_clock:
+            getattr(self, "_shared", self).evict_clock.add_(1)
+            for sk in self._admit_sketches():
+                sk.decay()
+        growing = []
         for gl in self.glookups:
             t = self.tmap[gl["table"]]
             if not t.dynamic or t.evict_strategy is not None:
                 continue
             region = buf[:, gl["key_off"]:gl["key_off"] + b * gl["hotness"]]
             keys = region.to(torch.int64)
-            out = torch.full_like(keys, -1)
+            parts = []
             for grp in self.groups:
                 for sl in grp.table_slices:
                     if sl["table"] != t.name or sl["cpart"] != 0:
@@ -972,10 +1029,19 @@ class EmbeddingCollection:
                     own = (keys >= 0) & ((keys % sl["k"]) == sl["s"])
                     ht = self._dyn_hash(t.name, sl)
                     k = torch.where(own, keys, torch.full_like(keys, -1)).reshape(-1)
-                    # bounded insert: a key that finds no free row reads as empty (-1) and raises the
-                    # table's sticky device flag -- no host sync here, see check_overflow()
-                    rows = (ht.get_insert(k) if self.is_train else ht.get(k)).reshape(keys.shape)
-                    out = torch.where(own & (rows >= 0), rows.to(torch.int64), out)
+                    if self.is_train and ht.sketch is not None:
+                        ht.admit_count(k)
+                    parts.append((own, ht, k))
+            growing.append((region, keys, parts))
+        for region, keys, parts in growing:
+            out = torch.full_like(keys, -1)
+            for own, ht, k in parts:
+                if self.is_train and ht.sketch is not None:
+                    ht.admit_filter(k)
+                # bounded insert: a key that finds no free row reads as empty (-1) and raises the
+                # table's sticky device flag -- no host sync here, see check_overflow()
+                rows = (ht.get_insert(k) if self.is_train else ht.get(k)).reshape(keys.shape)
+                out = torch.where(own & (rows >= 0), rows.to(torch.int64), out)
             region.copy_(out.to(region.dtype))
         if any(t.evict_strategy is not None for t in self.tables):
             self._translate_evicting(buf)
@@ -1024,6 +1090,7 @@ class EmbeddingCollection:
         keys, rows = ht.dump()
         from .hashtable import HashTable
         nh = HashTable(new, self.device)
+        nh.sketch = ht.sketch                  # the admission sketch is never resized
         if keys.numel():
             nh.set(keys, rows)
         self._dyn_tables[(name, cpart, s_)] = nh
@@ -1318,7 +1385,8 @@ class EmbeddingCollection:
     def _evict_admit(self, grp, sl, keys):
         """(checkpoint load) local rows of ``keys`` in an evicting shard: present keys keep theirs, the
         others take empty ways with the clock as stamp and a count of 1, and start from fresh weights and
-        state (overwritten by the caller).  Never evicts: raises when a key finds no free way."""
+        state (overwritten by the caller).  Never evicts, never applies admission: raises when a key finds no
+        free way."""
         ht = self._dyn_hash(sl["table"], sl)
         dev = self.device
         kk = keys.to(dev, torch.int64).view(1, -1).clone()
@@ -1382,4 +1450,4 @@ class EmbeddingCollection:
             for t in (grp.table, grp.s0, grp.s1):
                 if t is not None:
                     tot += t.numel() * t.element_size()
-        return tot
+        return tot + sum(sk.nbytes() for sk in self._admit_sketches())

@@ -6,6 +6,10 @@ get_size), capacity = max_vocabulary_size / 0.75 (nv_hashtable.hpp:179).
 SetAssocTable: the fixed-capacity, evicting key -> row map of a dynamic table with an
 ``evict_strategy`` (LRU / LFU over 32-way sets).  GPU: csrc/evict_table.cu; CPU: the same rules
 in Python, the oracle of the tests.
+
+AdmitSketch: the count-min admission sketch of a dynamic table with ``admit_threshold`` > 1, used by
+both tables above.  GPU: csrc/admit_sketch.cuh (+ the count / filter kernels of csrc/hashtable.cu and
+the folded ones of csrc/evict_table.cu); CPU: the same rules in Python.
 """
 from __future__ import annotations
 
@@ -31,13 +35,15 @@ def lib():
         l.hctr_ht_translate.restype = i
         for n in ("hctr_ht_get_insert", "hctr_ht_set", "hctr_ht_dump"):
             getattr(l, n).restype = i
-        l.hctr_evict_touch.argtypes = [vp, vp, vp]
-        l.hctr_evict_insert.argtypes = [vp, vp, vp, vp, i, vp]
+        l.hctr_evict_touch.argtypes = [vp, vp, vp, vp]
+        l.hctr_evict_insert.argtypes = [vp, vp, vp, vp, i, vp, vp]
+        l.hctr_ht_admit.argtypes = [vp, ull, vp, ll, vp, i, vp]
+        l.hctr_admit_decay.argtypes = [vp, ll, vp, ull, vp]
         l.hctr_evict_get.argtypes = [vp, vp, vp]
         l.hctr_evict_dump.argtypes = [vp, ll, vp, vp, vp, vp]
         l.hctr_evict_reinit.argtypes = [vp, ll, i, vp]
         for n in ("hctr_evict_touch", "hctr_evict_insert", "hctr_evict_get", "hctr_evict_dump",
-                  "hctr_evict_reinit"):
+                  "hctr_evict_reinit", "hctr_ht_admit", "hctr_admit_decay"):
             getattr(l, n).restype = i
         _lib = l
     return _lib
@@ -53,6 +59,8 @@ class HashTable:
         while cap < max(16, int(self.max_rows / self.LOAD_FACTOR)):
             cap <<= 1
         self.capacity = cap
+        # admission sketch of an admitting growing table (set by the owner; kept when the shard grows)
+        self.sketch: "AdmitSketch | None" = None
         if self.device.type == "cuda":
             self.keys = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
             self.vals = torch.full((cap,), -1, dtype=torch.int64, device=self.device)
@@ -131,6 +139,36 @@ class HashTable:
         kk = torch.where(own, k, torch.full_like(k, -1))
         out.reshape(-1).copy_(self._lookup(kk, insert))
         return out
+
+    def admit_count(self, keys: torch.Tensor):
+        """count, in the sketch, every occurrence of a key >= 0 of ``keys`` (int64, 1-D) that has no row: one
+        training lookup calls this on every key region of the table before any ``admit_filter`` / ``get_insert``"""
+        sk = self.sketch
+        if self.device.type == "cuda":
+            if lib().hctr_ht_admit(self.keys.data_ptr(), self.capacity, keys.data_ptr(), keys.numel(),
+                                   C.byref(sk.view()), 0, self._st()):
+                raise RuntimeError("hash admit count failed")
+            D._count()
+            return
+        sk.count([x for x in keys.tolist() if x >= 0 and x not in self.map])
+
+    def admit_filter(self, keys: torch.Tensor):
+        """in place: every key >= 0 without a row whose sketch count is below the threshold becomes -1
+        (rejected: no row, counted in the sketch's ``rejected``)"""
+        sk = self.sketch
+        if self.device.type == "cuda":
+            if lib().hctr_ht_admit(self.keys.data_ptr(), self.capacity, keys.data_ptr(), keys.numel(),
+                                   C.byref(sk.view()), 1, self._st()):
+                raise RuntimeError("hash admit filter failed")
+            D._count()
+            return
+        kl = keys.tolist()
+        miss = [i for i, x in enumerate(kl) if x >= 0 and x not in self.map]
+        if miss:
+            ok = sk.admits([kl[i] for i in miss])
+            rej = [i for i, a in zip(miss, ok) if not a]
+            keys[rej] = -1
+            sk.stats[1] += len(rej)
 
     def set(self, keys: torch.Tensor, vals: torch.Tensor):
         k, v = keys.reshape(-1).to(torch.int64), vals.reshape(-1).to(torch.int64)
@@ -227,7 +265,8 @@ class SetAssocTable:
     [key_off, key_off + n) of every row, keys with key >= 0 and key % key_mod == key_rem are handled,
     the others become -1.  Rules in docs/embedding.md; the CPU implementation is the reference."""
 
-    def __init__(self, max_capacity: int, strategy: str, clock: torch.Tensor, device):
+    def __init__(self, max_capacity: int, strategy: str, clock: torch.Tensor, device, sketch=None):
+        """``sketch``: the shard's AdmitSketch (admitting tables), else None"""
         if strategy not in EVICT_STRATEGIES:
             raise ValueError(f"evict_strategy must be one of {EVICT_STRATEGIES}, not {strategy!r}")
         self.capacity = (int(max_capacity) + WAYS - 1) // WAYS * WAYS
@@ -240,6 +279,7 @@ class SetAssocTable:
         self.counts = torch.zeros(self.capacity, dtype=torch.int64, device=dev)
         self.locks = torch.zeros(self.num_sets, dtype=torch.int32, device=dev)
         self.stats = torch.zeros(3, dtype=torch.int64, device=dev)      # admitted, evicted, dropped
+        self.sketch = sketch
 
     # ---- device plumbing
     def _view(self, stats=None):
@@ -306,11 +346,13 @@ class SetAssocTable:
     def touch(self, buf, key_off: int, n: int, key_mod: int = 1, key_rem: int = 0):
         """stamp the ways of the present keys with the clock, count the occurrences"""
         if self.device.type == "cuda":
+            sk = None if self.sketch is None else C.byref(self.sketch.view())
             self._call("hctr_evict_touch", C.byref(self._view()),
-                       C.byref(self._region(buf, key_off, n, key_mod, key_rem)), self._st())
+                       C.byref(self._region(buf, key_off, n, key_mod, key_rem)), sk, self._st())
             return
         now = int(self.clock[0])
         k, own = self._owned_keys(buf[:, key_off:key_off + n], key_mod, key_rem)
+        missing = []
         for key in k[own].tolist():
             base = int(evict_set_of([key], self.num_sets)[0]) * WAYS
             slot = self._find(base, key)
@@ -318,18 +360,25 @@ class SetAssocTable:
                 g = base + slot
                 self.stamps[g] = now
                 self.counts[g] += 1
+            else:
+                missing.append(key)
+        if self.sketch is not None:
+            self.sketch.count(missing)
 
     def insert(self, buf, key_off: int, n: int, key_mod: int = 1, key_rem: int = 0, adm=None, evict=True,
                stats=None):
         """rows of the keys written in place over them: present keys keep their way, missing keys are
         admitted (an empty way, else the victim of the strategy among the unprotected ways) or dropped
-        (-1).  ``adm``: (list [m] int64, count [1] int32) collecting the admitted ways.  ``evict=False``
-        takes empty ways only (checkpoint load)."""
+        (-1).  With a sketch, a missing key below the admission threshold is rejected first (-1).
+        ``adm``: (list [m] int64, count [1] int32) collecting the admitted ways.  ``evict=False`` takes
+        empty ways only and skips admission (checkpoint load)."""
         stats = self.stats if stats is None else stats
+        sk = self.sketch if evict else None
         if self.device.type == "cuda":
             a, an = (adm[0].data_ptr(), adm[1].data_ptr()) if adm is not None else (None, None)
             self._call("hctr_evict_insert", C.byref(self._view(stats)),
-                       C.byref(self._region(buf, key_off, n, key_mod, key_rem)), a, an, int(evict), self._st())
+                       C.byref(self._region(buf, key_off, n, key_mod, key_rem)), a, an, int(evict),
+                       None if sk is None else C.byref(sk.view()), self._st())
             return
         now = int(self.clock[0])
         region = buf[:, key_off:key_off + n]
@@ -337,7 +386,12 @@ class SetAssocTable:
         out = torch.full_like(k, -1)
         got = [] if adm is not None else None
         for idx in own.reshape(-1).nonzero()[:, 0].tolist():
-            out.view(-1)[idx] = self._insert_one(int(k.view(-1)[idx]), now, evict, got, stats)
+            key = int(k.view(-1)[idx])
+            if sk is not None and self._find(int(evict_set_of([key], self.num_sets)[0]) * WAYS, key) < 0 \
+                    and not sk.admits([key])[0]:
+                sk.stats[1] += 1
+                continue
+            out.view(-1)[idx] = self._insert_one(key, now, evict, got, stats)
         region.copy_(out.to(region.dtype))
         if adm is not None and got:
             m = int(adm[1][0])
@@ -403,3 +457,99 @@ class SetAssocTable:
     def live(self) -> torch.Tensor:
         """number of live keys, as a device scalar"""
         return (self.keys >= 0).sum()
+
+
+# ------------------------------------------------------------------------- admission sketch
+SKETCH_ROWS = 4
+SKETCH_MAX = (1 << 32) - 1
+SKETCH_SALT = 0x9E3779B97F4A7C15
+
+
+class _AdmitSketch(C.Structure):
+    _fields_ = [("counters", C.c_void_p), ("stats", C.c_void_p), ("width_mask", C.c_uint),
+                ("threshold", C.c_uint)]
+
+
+def sketch_width(rows: int) -> int:
+    """counters per sketch row: the smallest power of two >= 2 * rows, at least 1024"""
+    w = 1024
+    while w < 2 * int(rows):
+        w <<= 1
+    return w
+
+
+def sketch_slots(keys, width: int):
+    """flat counter index [n, 4] of every key, row r at r * width + (lo32(h) + r * (hi32(h) | 1)) mod width,
+    h = fmix64(key ^ SKETCH_SALT) (sketch_counter in csrc/admit_sketch.cuh); int64 numpy array"""
+    import numpy as np
+    from .ops import _fmix64
+    h = _fmix64(np.asarray(keys, dtype=np.int64).reshape(-1).astype(np.uint64) ^ np.uint64(SKETCH_SALT))
+    lo, hi = h & np.uint64(0xFFFFFFFF), (h >> np.uint64(32)) | np.uint64(1)
+    r = np.arange(SKETCH_ROWS, dtype=np.uint64)
+    with np.errstate(over="ignore"):
+        col = (lo[:, None] + r[None, :] * hi[:, None]) & np.uint64(width - 1)
+    return (r[None, :] * np.uint64(width) + col).astype(np.int64)
+
+
+class AdmitSketch:
+    """Count-min admission sketch of one row shard of a dynamic table with ``admit_threshold`` > 1: 4 rows
+    of ``sketch_width(rows)`` uint32 counters that saturate at 2**32 - 1, allocated once.  A training lookup
+    counts every owned occurrence of a key without a row (all counts of the table before any insert), and a
+    missing key may take a row only when the minimum of its four counters is >= ``threshold``.  With
+    ``decay_steps`` P > 0, ``decay`` (called once per training step, after the clock tick) halves every
+    counter when the clock is a multiple of P.  ``stats``: counted occurrences and rejected positions.
+    Rules in docs/embedding.md; the CPU implementation is the reference."""
+
+    def __init__(self, rows: int, threshold: int, decay_steps: int, clock: torch.Tensor, device):
+        self.width = sketch_width(rows)
+        self.threshold, self.decay_steps, self.clock = int(threshold), int(decay_steps), clock
+        self.device = torch.device(device)
+        # uint32 counters stored in int32 words (torch has no general uint32 arithmetic)
+        self.counters = torch.zeros(SKETCH_ROWS * self.width, dtype=torch.int32, device=self.device)
+        self.stats = torch.zeros(2, dtype=torch.int64, device=self.device)      # counted, rejected
+
+    def view(self):
+        return _AdmitSketch(self.counters.data_ptr(), self.stats.data_ptr(), self.width - 1, self.threshold)
+
+    def values(self) -> torch.Tensor:
+        """the counters as int64 [4, width] on CPU (host synchronisation)"""
+        return (self.counters.cpu().to(torch.int64) & SKETCH_MAX).view(SKETCH_ROWS, self.width)
+
+    def nbytes(self) -> int:
+        return self.counters.numel() * self.counters.element_size()
+
+    # ---- CPU rules (the reference the kernels are tested against)
+    def _u32(self):
+        import numpy as np
+        return self.counters.numpy().view(np.uint32)
+
+    def count(self, keys):
+        """one occurrence of every key in ``keys`` (a list of missing keys, repeats counted)"""
+        import numpy as np
+        if not len(keys):
+            return
+        c = self._u32()
+        v = c.astype(np.int64)
+        np.add.at(v, sketch_slots(keys, self.width).reshape(-1), 1)
+        c[:] = np.minimum(v, SKETCH_MAX).astype(np.uint32)          # saturating adds commute
+        self.stats[0] += len(keys)
+
+    def admits(self, keys):
+        """bool numpy array: the minimum of each key's counters reaches the threshold"""
+        c = self._u32()
+        return c[sketch_slots(keys, self.width)].min(axis=1).astype("int64") >= self.threshold
+
+    def decay(self):
+        """halve every counter (rounding down) when the clock is a multiple of ``decay_steps`` (no host read
+        on CUDA: the kernel tests the clock)"""
+        if self.decay_steps <= 0:
+            return
+        if self.device.type == "cuda":
+            if lib().hctr_admit_decay(self.counters.data_ptr(), self.counters.numel(), self.clock.data_ptr(),
+                                      self.decay_steps, torch.cuda.current_stream(self.device).cuda_stream):
+                raise RuntimeError("hctr_admit_decay failed")
+            D._count()
+            return
+        if int(self.clock[0]) % self.decay_steps == 0:
+            c = self._u32()
+            c >>= 1

@@ -210,6 +210,10 @@ def model_to_json(model) -> dict:
                 tj.update(init_capacity=t.init_capacity, max_capacity=t.max_capacity)
                 if t.evict_strategy is not None:
                     tj["evict_strategy"] = t.evict_strategy
+                if t.admit_threshold != 1:
+                    tj["admit_threshold"] = t.admit_threshold
+                if t.admit_decay_steps != 0:
+                    tj["admit_decay_steps"] = t.admit_decay_steps
             if getattr(t, "weight_dtype", "fp32") != "fp32":
                 tj["weight_dtype"] = t.weight_dtype
             if t.init_param is not None and getattr(t.init_param, "up_bound", 0) > 0:
@@ -261,7 +265,8 @@ def add_from_json(model, graph: dict, include_dense_network: bool = True):
             from .embedding.collection import InitParams
             tabs = {}
             for tt in j["tables"]:
-                kw = {k: tt[k] for k in ("init_capacity", "max_capacity", "weight_dtype", "evict_strategy") if k in tt}
+                kw = {k: tt[k] for k in ("init_capacity", "max_capacity", "weight_dtype", "evict_strategy",
+                                         "admit_threshold", "admit_decay_steps") if k in tt}
                 ip = InitParams(up_bound=tt["init_up_bound"]) if "init_up_bound" in tt else None
                 tabs[tt["name"]] = EmbeddingTableConfig(
                     tt["name"], tt["max_vocabulary_size"], tt["ev_size"],

@@ -942,7 +942,8 @@ class Model:
         ebcs = [e for e in getattr(self, "ebcs_train", []) if getattr(e, "has_dynamic", False)]
         if not ebcs:
             return
-        # evicting tables never grow: their counters are logged, the step graph stays
+        # evicting tables never grow: their counters are logged, the step graph stays (the admission counters of
+        # admitting tables are logged as well)
         seen = self.__dict__.setdefault("_evict_dropped", {})
         for ei, e in enumerate(ebcs):
             for (name, shard), st in e.eviction_stats().items():
@@ -954,6 +955,9 @@ class Model:
                                    "dropped since the last report (every way of their set held a key of the "
                                    "running step); they read as empty rows and got no update")
                 seen[(ei, name, shard)] = st["dropped"]
+            for (name, shard), st in e.admission_stats().items():
+                logger.info(f"admitting embedding table {name} shard {shard}: counted {st['counted']} "
+                            f"rejected {st['rejected']}")
         if os.environ.get("HCTR_DYNAMIC_GROW", "1") == "0":
             for e in ebcs:
                 e.check_overflow()
