@@ -27,10 +27,15 @@ namespace hctr {
 // One group of G lanes per (src rank, lookup, sample) bucket; each lane owns VEC consecutive
 // floats per 32*VEC-wide column chunk.  G*VEC >= ev for ev <= 128 (VEC=4), wider rows loop over
 // up to MAXC chunks per lane: one launch covers columns [col_base, col_base + MAXC * G * VEC).
-// WT: weight type of the arena (fp32, or bf16 loaded 8 bytes per 4 columns); pooling is in fp32.
+// WT: weight type of the arena (fp32, bf16 loaded 8 bytes per 4 columns, or e4m3: VEC = 16 columns in one
+// 16-byte load per lane when the rows are whole 16-byte units, else 4 or 1 columns); pooling is in fp32.
 // WGT: weighted lookups may be present; a row enters as fma(w, row, acc) (w = 1 for unweighted
 // lookups and 0 for skipped keys: fma(1, v, acc) == acc + v, so all-ones weights pool bit for bit as
 // the unweighted kernel does).
+// e4m3 arenas (FP8) always take the fma path: the lane that resolves a key also reads its row's
+// exponent byte and folds 2^e into the key's weight, which travels with the row as the weights do.
+// w * 2^e and q * 2^e are exact, so fma(w * 2^e, q, acc) == fma(w, q * 2^e, acc): the lookup pools bit
+// for bit as the fp32 kernel over the dequantized rows.
 template <typename KeyT, typename OutT, int VEC, int U, typename WT, bool WGT>
 __global__ void __launch_bounds__(256, 3)
     emb_fwd_kernel(const EmbParams p, const int G, const int col_base) {
@@ -52,12 +57,15 @@ __global__ void __launch_bounds__(256, 3)
   if (active && lk.nnz_off >= 0) nnz = min(lk.hotness, p.nnz[src][lk.nnz_off + s]);
   if (!active) nnz = 0;
   const WT* table = static_cast<const WT*>(p.table);
+  constexpr bool FP8 = std::is_same<WT, __nv_fp8_e4m3>::value;
+  constexpr bool SCALED = WGT || FP8;   // rows enter as fma(factor, row, acc)
   const bool lw = WGT && lk.weighted;
   const float* wbase = WGT ? p.weights[src] + lk.key_off + static_cast<long long>(s) * lk.key_stride : nullptr;
 
   // chunks per lane.  Weighted vector rows keep 8 chunks at 4 rows in flight: the U weights beside 8 rows' loads
   // and the accumulators exceed the 80 registers of __launch_bounds__(256, 3) and spill
-  constexpr int MAXC = (U >= 8 || (WGT && VEC == 4)) ? 8 : 4;
+  // (e4m3 rows: exactly the chunks kMaxEmbWidth needs at 32 lanes, so that no chunk's accumulators are held in vain)
+  constexpr int MAXC = (FP8 && VEC >= 4) ? kMaxEmbWidth / (32 * VEC) : ((U >= 8 || (WGT && VEC == 4)) ? 8 : 4);
   float acc[MAXC][VEC];
 #pragma unroll
   for (int c = 0; c < MAXC; ++c)
@@ -65,7 +73,7 @@ __global__ void __launch_bounds__(256, 3)
     for (int v = 0; v < VEC; ++v) acc[c][v] = 0.f;
   const int nchunk = (ev - col_base + G * VEC - 1) / (G * VEC);
 
-  // gathers U rows (rp[u] == nullptr: skip) with weights wv (WGT only) into the accumulators
+  // gathers U rows (rp[u] == nullptr: skip) with factors wv (SCALED only) into the accumulators
   auto gather = [&](const WT* const (&rp)[U], const float (&wv)[U]) {
 #pragma unroll
     for (int c = 0; c < MAXC; ++c) {
@@ -79,11 +87,29 @@ __global__ void __launch_bounds__(256, 3)
               v[u] = rp[u] ? ldg_row4(rp[u] + col) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
             for (int u = 0; u < U; ++u) {
-              if constexpr (WGT) {
+              if constexpr (SCALED) {
                 acc[c][0] = fmaf(wv[u], v[u].x, acc[c][0]); acc[c][1] = fmaf(wv[u], v[u].y, acc[c][1]);
                 acc[c][2] = fmaf(wv[u], v[u].z, acc[c][2]); acc[c][3] = fmaf(wv[u], v[u].w, acc[c][3]);
               } else {
                 acc[c][0] += v[u].x; acc[c][1] += v[u].y; acc[c][2] += v[u].z; acc[c][3] += v[u].w;
+              }
+            }
+          } else if constexpr (VEC == 16) {
+            // e4m3 rows only: 16 bytes per lane and chunk in one load per row (docs/performance.md: faster than
+            // 4 or 8 bytes per lane at ev 128 and 256)
+            uint4 v[U];
+#pragma unroll
+            for (int u = 0; u < U; ++u)
+              v[u] = rp[u] ? __ldg(reinterpret_cast<const uint4*>(rp[u] + col)) : make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+            for (int u = 0; u < U; ++u) {
+#pragma unroll
+              for (int k = 0; k < VEC / 4; ++k) {
+                const float4 f = e4m3x4_to_float4(word_of(v[u], k));
+                acc[c][4 * k] = fmaf(wv[u], f.x, acc[c][4 * k]);
+                acc[c][4 * k + 1] = fmaf(wv[u], f.y, acc[c][4 * k + 1]);
+                acc[c][4 * k + 2] = fmaf(wv[u], f.z, acc[c][4 * k + 2]);
+                acc[c][4 * k + 3] = fmaf(wv[u], f.w, acc[c][4 * k + 3]);
               }
             }
           } else {
@@ -92,7 +118,7 @@ __global__ void __launch_bounds__(256, 3)
             for (int u = 0; u < U; ++u) v[u] = rp[u] ? ldg_row1(rp[u] + col) : 0.f;
 #pragma unroll
             for (int u = 0; u < U; ++u) {
-              if constexpr (WGT) acc[c][0] = fmaf(wv[u], v[u], acc[c][0]);
+              if constexpr (SCALED) acc[c][0] = fmaf(wv[u], v[u], acc[c][0]);
               else acc[c][0] += v[u];
             }
           }
@@ -110,7 +136,7 @@ __global__ void __launch_bounds__(256, 3)
     const unsigned int ns = static_cast<unsigned int>(lk.num_shards);
     for (int h0 = 0; h0 < nnz; h0 += KPL * G) {
       unsigned int rowv[4] = {0u, 0u, 0u, 0u};
-      float wtv[4] = {1.f, 1.f, 1.f, 1.f};   // WGT: the weights travel with rowv
+      float wtv[4] = {1.f, 1.f, 1.f, 1.f};   // SCALED: the weights (times 2^e) travel with rowv
       unsigned int m = 0;
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -134,6 +160,9 @@ __global__ void __launch_bounds__(256, 3)
               ok = rem == static_cast<unsigned int>(lk.shard_idx) && q < static_cast<unsigned long long>(lk.rows);
               rowv[i] = static_cast<unsigned int>(q);
               if (lw && ok) wtv[i] = wbase[h];
+              if constexpr (FP8) {
+                if (ok) wtv[i] *= row_scale(p.row_exp, lk.table_row_off + static_cast<long long>(q));
+              }
             }
           }
           const unsigned int bal = (__ballot_sync(gmask, ok) >> (gi * G)) & ((G == 32) ? 0xffffffffu : ((1u << G) - 1u));
@@ -153,7 +182,7 @@ __global__ void __launch_bounds__(256, 3)
           const unsigned int cand = i == 0 ? rowv[0] : (i == 1 ? rowv[1] : (i == 2 ? rowv[2] : rowv[3]));
           const unsigned int r = __shfl_sync(gmask, cand, gi * G + sl);
           if (take) rp[u] = table + (lk.table_row_off + r) * static_cast<long long>(p.ev_size);
-          if constexpr (WGT) {
+          if constexpr (SCALED) {
             const float cw = i == 0 ? wtv[0] : (i == 1 ? wtv[1] : (i == 2 ? wtv[2] : wtv[3]));
             const float w = __shfl_sync(gmask, cw, gi * G + sl);
             wv[u] = take ? w : 0.f;
@@ -169,6 +198,9 @@ __global__ void __launch_bounds__(256, 3)
       if (h0 + gl < nnz) mykey = static_cast<long long>(kbase[h0 + gl]);
       float myw = 1.f;
       if (lw && h0 + gl < nnz) myw = wbase[h0 + gl];
+      if constexpr (FP8) {
+        if (mykey >= 0 && mykey < lk.rows) myw *= row_scale(p.row_exp, lk.table_row_off + mykey);
+      }
       const int cnt = min(G, nnz - h0);
       for (int j0 = 0; j0 < cnt; j0 += U) {
         const WT* rp[U];
@@ -179,7 +211,7 @@ __global__ void __launch_bounds__(256, 3)
           const long long key = __shfl_sync(gmask, mykey, gi * G + (j < cnt ? j : 0));
           const bool ok = (j < cnt) && key >= 0 && key < lk.rows;
           rp[u] = ok ? table + (lk.table_row_off + key) * static_cast<long long>(p.ev_size) : nullptr;
-          if constexpr (WGT) {
+          if constexpr (SCALED) {
             const float w = __shfl_sync(gmask, myw, gi * G + (j < cnt ? j : 0));
             wv[u] = ok ? w : 0.f;
           }
@@ -198,9 +230,11 @@ __global__ void __launch_bounds__(256, 3)
     if (c < nchunk) {
       const int col = col_base + (c * G + gl) * VEC;
       if (col < ev) {
-        if constexpr (VEC == 4) {
-          store_vec4<OutT>(o + col, acc[c][0] * scale, acc[c][1] * scale, acc[c][2] * scale,
-                           acc[c][3] * scale);
+        if constexpr (VEC >= 4) {
+#pragma unroll
+          for (int k = 0; k < VEC / 4; ++k)
+            store_vec4<OutT>(o + col + 4 * k, acc[c][4 * k] * scale, acc[c][4 * k + 1] * scale,
+                             acc[c][4 * k + 2] * scale, acc[c][4 * k + 3] * scale);
         } else {
           o[col] = from_f<OutT>(acc[c][0] * scale);
         }
@@ -489,6 +523,36 @@ __global__ void emb_gather_rows_kernel(const WT* __restrict__ table, const long 
     out[w * ev + c] = from_f<OutT>(r < 0 ? 0.f : to_f<WT>(table[r * ev + c]));
 }
 
+// Serving arenas: quantizes fp32 rows src [n, pitch] into arena rows rows[i] of the e4m3 arena q
+// [*, pitch], one warp per row: exps[row] = e + 127 with e = e4m3_scale_exp(amax of the row) and
+// q = e4m3_satfinite_rn(x * 2^-e) (mirrored by embedding/ops.py::fp8_rows_quantize).  A non-finite
+// value sets *bad; the caller reads the flag once per load and rejects the load.
+__global__ void __launch_bounds__(256)
+    emb_quantize_rows_kernel(const float* __restrict__ src, const long long* __restrict__ rows, long long n,
+                             int pitch, uint8_t* __restrict__ q, uint8_t* __restrict__ exps, int* bad) {
+  const long long w = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n) return;
+  const float* x = src + w * pitch;
+  float amax = 0.f;
+  bool finite = true;
+  for (int c = lane; c < pitch; c += 32) {
+    const float v = x[c];
+    finite &= isfinite(v);
+    amax = fmaxf(amax, fabsf(v));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+  if (!__all_sync(0xffffffffu, finite) && lane == 0) *bad = 1;
+  const int e = e4m3_scale_exp(amax);
+  const float inv = ldexpf(1.f, -e);
+  const long long r = rows[w];
+  uint8_t* d = q + r * pitch;
+  for (int c = lane; c < pitch; c += 32)
+    d[c] = static_cast<uint8_t>(__nv_cvt_float_to_fp8(x[c] * inv, __NV_SATFINITE, __NV_E4M3));
+  if (lane == 0) exps[r] = static_cast<uint8_t>(e + 127);
+}
+
 }  // namespace hctr
 
 using namespace hctr;
@@ -501,13 +565,17 @@ static inline int pick_group(int ev, int vec) {
 }
 
 // key_bytes: 4 or 8 ; out_bf16 / grad_bf16 : element type of activations ; table_bf16 : of the arena
-// aligned4: every lookup's ev_size, out_off and out_stride, the table pitch and the base pointers are
+// (hctr_emb_forward's table_type: 0 fp32, 1 bf16, 2 e4m3 with p->row_exp)
+// aligned4 (4, or 16 for an e4m3 arena whose lookup widths and pitch are multiples of 16): every lookup's
+// ev_size, out_off and out_stride, the table pitch and the base pointers are
 // multiples of 4 elements (whole-vector table rows and output stores); 0 selects scalar accesses
 extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, int out_bf16,
-                                int aligned4, int table_bf16, void* stream_) {
+                                int aligned4, int table_type, void* stream_) {
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   if (max_ev > kMaxEmbWidth) return -4;
-  const int vec = (aligned4 && max_ev % 4 == 0) ? 4 : 1;
+  int vec = (aligned4 && max_ev % 4 == 0) ? 4 : 1;
+  // e4m3 arenas whose rows are whole 16-byte units (aligned4 == 16): one 16-byte load per lane and row
+  if (table_type == 2 && aligned4 == 16 && max_ev % 16 == 0) vec = 16;
   int G = pick_group(max_ev, vec);
   // wide rows: 8 lanes per bucket, every lane owns up to 4 float4 chunks of the row -> 4 buckets
   // per warp and 16 independent 16-byte loads in flight per lane (latency-bound -> bandwidth-bound)
@@ -521,17 +589,23 @@ extern "C" int hctr_emb_forward(const EmbParams* p, int max_ev, int key_bytes, i
                     p->num_ranks * p->num_lookups);
   // one pass covers every column, except scalar rows wider than 8 chunks x 32 lanes: those take
   // passes of 256 columns (keeps the accumulators of the scalar kernel in registers)
-  const int pass = (vec == 4) ? max_ev : 8 * G;
+  const int pass = (vec >= 4) ? max_ev : 8 * G;
   for (int c0 = 0; c0 < max_ev; c0 += pass) {
-    with_key(key_bytes, [&](auto k) { with_elem(out_bf16, [&](auto o) { with_elem(table_bf16, [&](auto w) {
+    with_key(key_bytes, [&](auto k) { with_elem(out_bf16, [&](auto o) { with_table(table_type, [&](auto w) {
       with_weighted(*p, [&](auto wgt) {
         auto launch = [&](auto v, auto u) {   // vector width, rows in flight per gather round
           emb_fwd_kernel<type_of<decltype(k)>, type_of<decltype(o)>, decltype(v)::value, decltype(u)::value,
                          type_of<decltype(w)>, decltype(wgt)::value><<<blocks, threads, 0, st>>>(*p, G, c0);
         };
-        if (vec == 1) launch(Int<1>{}, Int<8>{});
-        else if (narrow) launch(Int<4>{}, Int<4>{});
-        else launch(Int<4>{}, Int<decltype(wgt)::value ? 4 : 8>{});
+        if constexpr (std::is_same<type_of<decltype(w)>, __nv_fp8_e4m3>::value) {
+          if (vec == 16) launch(Int<16>{}, Int<4>{});
+          else if (vec == 4) launch(Int<4>{}, Int<2>{});
+          else launch(Int<1>{}, Int<8>{});
+        } else {
+          if (vec == 1) launch(Int<1>{}, Int<8>{});
+          else if (narrow) launch(Int<4>{}, Int<4>{});
+          else launch(Int<4>{}, Int<decltype(wgt)::value ? 4 : 8>{});
+        }
       });
     }); }); });
   }
@@ -622,5 +696,16 @@ extern "C" int hctr_emb_gather_rows(const void* table, const long long* rows, vo
     using WT = type_of<decltype(w)>;
     emb_gather_rows_kernel<OutT, WT><<<blocks, 256, 0, st>>>((const WT*)table, rows, (OutT*)out, n, ev);
   }); });
+  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+// rows: int64 [n] arena rows (distinct), src: fp32 [n, pitch] contiguous, q / exps: the e4m3 arena and
+// its exponent bytes, bad: int32 flag set on a non-finite value
+extern "C" int hctr_emb_quantize_rows(const float* src, const long long* rows, long long n, int pitch, void* q,
+                                      unsigned char* exps, int* bad, void* stream_) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+  if (n == 0) return 0;
+  const unsigned blocks = static_cast<unsigned>((n * 32 + 255) / 256);
+  emb_quantize_rows_kernel<<<blocks, 256, 0, st>>>(src, rows, n, pitch, static_cast<uint8_t*>(q), exps, bad);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

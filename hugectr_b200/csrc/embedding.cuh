@@ -1,6 +1,7 @@
 // Shared declarations of the embedding kernels (see embedding.cu / embedding_bwd.cu).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -44,11 +45,13 @@ struct EmbParams {
   void* out[kMaxRanks];          // per source rank: output activation base
   const void* grad[kMaxRanks];   // per source rank: top-grad base
   const EmbLookup* lookups;      // device array [num_lookups]
-  void* table;                   // [rows, ev] arena of fp32 or bf16 weights (the launcher's table_bf16)
+  void* table;                   // [rows, ev] arena of fp32, bf16 or e4m3 weights (the launcher's table_type)
   int ev_size;                   // row pitch of the arena (all tables of a group share it)
   // per source rank: fp32 per-key weights in the layout of keys (same element offsets); all null
   // when no lookup of the launch is weighted, which selects the unweighted kernels
   const float* weights[kMaxRanks];
+  // e4m3 arena: one byte e + 127 per arena row, the row dequantizes to q * 2^e; null for fp32 and bf16
+  const uint8_t* row_exp;
 };
 
 // Weight of key h of bucket (src, s) of a lookup: 1 unless the lookup is weighted
@@ -161,6 +164,32 @@ HCTR_DEVICE float4 ldg_row4(const __nv_bfloat16* p) {
 }
 HCTR_DEVICE float ldg_row1(const float* p) { return __ldg(p); }
 HCTR_DEVICE float ldg_row1(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+// e4m3 rows (serving arenas): 4 bytes per 4 columns, unpacked by the hardware conversion; the row's
+// power-of-two scale is applied by the caller (row_scale)
+HCTR_DEVICE float4 e4m3x4_to_float4(unsigned int v) {
+  const float2 lo = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(
+      static_cast<__nv_fp8x2_storage_t>(v & 0xFFFFu), __NV_E4M3)));
+  const float2 hi = __half22float2(__half2(__nv_cvt_fp8x2_to_halfraw2(
+      static_cast<__nv_fp8x2_storage_t>(v >> 16), __NV_E4M3)));
+  return make_float4(lo.x, lo.y, hi.x, hi.y);
+}
+HCTR_DEVICE float4 ldg_row4(const __nv_fp8_e4m3* p) {
+  return e4m3x4_to_float4(__ldg(reinterpret_cast<const unsigned int*>(p)));
+}
+// 4-byte word k of a 16-byte load (k known at compile time)
+HCTR_DEVICE unsigned int word_of(const uint4& v, int k) {
+  return k == 0 ? v.x : (k == 1 ? v.y : (k == 2 ? v.z : v.w));
+}
+HCTR_DEVICE float ldg_row1(const __nv_fp8_e4m3* p) {
+  const unsigned char b = __ldg(reinterpret_cast<const unsigned char*>(p));
+  return __half2float(__half(__nv_cvt_fp8_to_halfraw(static_cast<__nv_fp8_storage_t>(b), __NV_E4M3)));
+}
+// 2^e of arena row `row` of an e4m3 arena (exps[row] = e + 127), exact.  Byte 0 gives 0 instead of the
+// subnormal 2^-127: the device quantizer writes it for all-zero rows only (rows with amax below
+// 448 * 2^-126 flush to e = -1 and zero bytes), so the pooled value is 0 either way.
+HCTR_DEVICE float row_scale(const uint8_t* exps, long long row) {
+  return __uint_as_float(static_cast<unsigned int>(__ldg(exps + row)) << 23);
+}
 
 // ------------------------------------------------------------------ unique (transient hash)
 HCTR_DEVICE unsigned int unique_get_insert(const UniqueTable& t, unsigned long long row) {
@@ -223,6 +252,12 @@ template <typename Fn>
 inline void with_elem(int is_bf16, Fn&& fn) {
   if (is_bf16) fn(Tag<__nv_bfloat16>{});
   else fn(Tag<float>{});
+}
+// weight type of an arena: 0 fp32, 1 bf16, 2 e4m3 (serving arenas, lookup only)
+template <typename Fn>
+inline void with_table(int table_type, Fn&& fn) {
+  if (table_type == 2) fn(Tag<__nv_fp8_e4m3>{});
+  else with_elem(table_type, fn);
 }
 // key type: 8-byte or 4-byte integers
 template <typename Fn>

@@ -150,15 +150,7 @@ __global__ void __launch_bounds__(256)
 #pragma unroll
       for (int j = 0; j < 32; ++j) v[j] = 0.f;
     }
-    // power-of-two scale: smallest 2^e with amax / 2^e <= 448 (e4m3 max)
-    // (frexp instead of log2: exact and independent of --use_fast_math; v = m * 2^ex, m in [0.5, 1))
-    int e = -127;
-    if (amax > 0.f) {
-      int ex;
-      const float m = frexpf(amax * (1.f / 448.f), &ex);
-      e = (m > 0.5f) ? ex : ex - 1;
-      e = max(-127, min(127, e));
-    }
+    const int e = e4m3_scale_exp(amax);
     const float inv = ldexpf(1.f, -e);
     uint32_t w[8];
 #pragma unroll

@@ -14,6 +14,21 @@ HCTR_DEVICE uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
+// Exponent e of the power-of-two scale of a block (or row) of e4m3 values whose largest magnitude is amax:
+// the smallest 2^e with amax / 2^e <= 448 (e4m3 max), clamped to [-127, 127]; -127 when amax == 0.
+// (frexp instead of log2: exact and independent of --use_fast_math; v = m * 2^ex, m in [0.5, 1))
+// Mirrored by ops/mxfp8.py::e4m3_scale_exponent.
+HCTR_DEVICE int e4m3_scale_exp(float amax) {
+  int e = -127;
+  if (amax > 0.f) {
+    int ex;
+    const float m = frexpf(amax * (1.f / 448.f), &ex);
+    e = (m > 0.5f) ? ex : ex - 1;
+    e = max(-127, min(127, e));
+  }
+  return e;
+}
+
 HCTR_DEVICE uint32_t lane_id() {
   uint32_t l;
   asm volatile("mov.u32 %0, %%laneid;" : "=r"(l));

@@ -37,6 +37,11 @@ def _stable_seed(*parts) -> int:
 
 # ------------------------------------------------------------------------- configs
 WEIGHT_DTYPES = {"fp32": torch.float32, "bf16": torch.bfloat16}
+# arena storage of a group: a table's weight_dtype, or "fp8" for every table of a serving collection built with
+# fp8_quant (e4m3 rows with one power-of-two scale per row, see embedding/ops.py::fp8_rows_quantize)
+STORAGE_DTYPES = {**WEIGHT_DTYPES, "fp8": torch.float8_e4m3fn}
+# rows an fp8 arena quantizes per launch: the fp32 staging of a fill or a checkpoint chunk on the device
+FP8_STORE_CHUNK_ROWS = 1 << 16
 
 
 @dataclass
@@ -205,6 +210,19 @@ def _uniform_fill(view, bound, gen):
         view.copy_(torch.empty(view.shape, dtype=torch.float32, device=view.device).uniform_(-bound, bound, generator=gen))
 
 
+def _rows_fp32(grp, lo: int, hi: int) -> torch.Tensor:
+    """fp32 values [hi - lo, pitch] of arena rows [lo, hi) of ``grp``.  An fp8 arena's rows are dequantized a
+    bounded chunk at a time into a host tensor, so that no fp32 copy of a table is made on the device."""
+    t = grp.table.view(-1, grp.pitch)
+    if grp.exps is None:
+        return t[lo:hi].float()
+    out = torch.empty(hi - lo, grp.pitch, dtype=torch.float32)
+    for c in range(lo, hi, FP8_STORE_CHUNK_ROWS):
+        d = min(hi, c + FP8_STORE_CHUNK_ROWS)
+        out[c - lo:d - lo] = E.fp8_rows_dequantize(t[c:d], grp.exps[c:d]).cpu()
+    return out
+
+
 def shard_rows(vocab: int, k: int, s: int) -> int:
     """number of keys in [0, vocab) with key % k == s"""
     return (vocab - s + k - 1) // k if vocab > s else 0
@@ -219,6 +237,7 @@ class _Group:
     def __init__(self, kind, pitch, wdtype="fp32", rowwise=False):
         self.kind, self.pitch, self.wdtype = kind, pitch, wdtype
         self.rowwise = rowwise
+        self.exps = None         # fp8 arena: uint8 [rows], e + 127 of each row's scale 2^e
         self.rows = 0
         self.table_slices = []   # (table name, col part, row_off, rows, num_shards, shard_idx, col0)
         self.lookups: List[E.LookupDesc] = []
@@ -268,10 +287,17 @@ class EmbeddingCollection:
     def __init__(self, cfg: EmbeddingCollectionConfig, batch_per_gpu: int, hotness: Dict[str, int],
                  device, act_dtype, comm, default_opt: OptParamsPy, key_dtype=torch.int32,
                  scaler: float = 1.0, state_dtype=torch.float32, seed: int = 0,
-                 fused: Optional[bool] = None, is_train: bool = True, weighted=()):
+                 fused: Optional[bool] = None, is_train: bool = True, weighted=(), fp8_quant: bool = False):
         """``weighted``: names of the sparse inputs whose keys carry an fp32 weight each (see
         docs/embedding.md): every lookup of such an input pools ``sum_h w_h * T[key_h]`` (mean: divided
-        by ``sum_h w_h``, or by 1 when that is 0)."""
+        by ``sum_h w_h``, or by 1 when that is 0).
+        ``fp8_quant`` (serving collections, ``is_train=False``): every table is stored as e4m3 rows with one
+        power-of-two scale per row, quantized by every write (initial fill, checkpoint load); lookups pool the
+        dequantized rows in fp32 (see docs/embedding.md)."""
+        if fp8_quant and is_train:
+            raise ValueError("fp8_quant stores tables for serving: it needs is_train=False")
+        self.fp8_quant = bool(fp8_quant)
+        self._fp8_bad = {}       # table name -> int32 device flag of a non-finite value met by the quantizer
         self.cfg, self.b, self.device, self.act_dtype = cfg, batch_per_gpu, device, act_dtype
         self.weighted_inputs = frozenset(weighted)
         # who am I / whom do I talk to: through the backend-neutral interface (core.py; reference core.hpp)
@@ -474,7 +500,7 @@ class EmbeddingCollection:
         b = self.b
         wdtype = {t.name: getattr(t, "weight_dtype", "fp32") for t in self.tables}
         dp_bf16 = [n for n, w in wdtype.items() if w != "fp32" and self.placement[n].kind == "dp"]
-        if dp_bf16 and share_from is None:
+        if dp_bf16 and share_from is None and not self.fp8_quant:
             from ..utils import logger
             logger.info(f"weight_dtype: data-parallel tables {sorted(dp_bf16)} keep fp32 weights (their gradients "
                         "take the dense all-reduce and the dense optimizer)")
@@ -496,7 +522,8 @@ class EmbeddingCollection:
             o = t.opt_params or self.default_opt
             rowwise = o is not None and o.optimizer_type == Optimizer_t.RowWiseAdaGrad
             for (cpart, k, s) in parts:
-                wdt = wdtype[t.name] if pl.kind == "mp" else "fp32"
+                # (a serving collection takes no gradient: its data-parallel tables may be fp8 too)
+                wdt = "fp8" if self.fp8_quant else (wdtype[t.name] if pl.kind == "mp" else "fp32")
                 key = (pl.kind, ev_part, wdt)
                 if rowwise:
                     # never shares an arena (and its first table's optimizer) with another optimizer
@@ -566,7 +593,9 @@ class EmbeddingCollection:
             return
         for grp in self.groups:
             n = max(grp.rows, 1) * grp.pitch
-            grp.table = torch.empty(n, dtype=WEIGHT_DTYPES[grp.wdtype], device=dev)
+            grp.table = torch.empty(n, dtype=STORAGE_DTYPES[grp.wdtype], device=dev)
+            if grp.wdtype == "fp8":
+                grp.exps = torch.empty(max(grp.rows, 1), dtype=torch.uint8, device=dev)
             self._init_group(grp, gen, seed)
             sdt = self.state_dtype if grp.kind == "mp" else torch.float32
             grp.s0, grp.s1 = opt_states(grp.opt, n, sdt, dev) if self.is_train else (None, None)
@@ -619,11 +648,53 @@ class EmbeddingCollection:
                 full_rows = t.max_vocabulary_size
                 if not t.dynamic and full_rows * grp.pitch <= (1 << 26):
                     full = (torch.rand(full_rows, grp.pitch, generator=gen) * 2 - 1) * bound
+                    if grp.exps is not None:
+                        self._store_rows(grp, sl["table"], torch.arange(sl["row_off"], sl["row_off"] + sl["rows"],
+                                                                        device=self.device), full[sl["s"]::sl["k"]])
+                        continue
                     view.copy_(full[sl["s"]::sl["k"]].reshape(-1).to(view.device))   # bf16: to nearest
                     continue
             g2 = torch.Generator(device=self.device)
             g2.manual_seed(_stable_seed(seed, sl["table"], sl["cpart"], sl["s"]))
-            _uniform_fill(view, bound, g2)
+            self._fill_uniform(grp, sl["table"], sl["row_off"], sl["rows"], bound, g2)
+
+    def _fill_uniform(self, grp, name, lo, n, bound, gen):
+        """U(-bound, bound) into arena rows [lo, lo + n) of ``grp``: drawn in fp32, a bf16 arena rounds them
+        to nearest, an fp8 arena quantizes them a bounded chunk of rows at a time"""
+        if grp.exps is None:
+            _uniform_fill(grp.table[lo * grp.pitch:(lo + n) * grp.pitch], bound, gen)
+            return
+        for c in range(lo, lo + n, FP8_STORE_CHUNK_ROWS):
+            m = min(FP8_STORE_CHUNK_ROWS, lo + n - c)
+            v = torch.empty(m, grp.pitch, dtype=torch.float32, device=self.device).uniform_(-bound, bound, generator=gen)
+            self._store_rows(grp, name, torch.arange(c, c + m, device=self.device), v)
+
+    def _store_rows(self, grp, name, rows, values):
+        """The one write path of an fp8 arena: fp32 rows ``values`` [n, pitch] (any device) quantized into
+        arena rows ``rows`` [n] (ops.fp8_rows_quantize), a bounded chunk of rows at a time, so that no fp32
+        copy of a table is ever on the device.  A non-finite value raises ValueError on the CPU; on CUDA it
+        sets the table's device flag, which check_quantized() reads once per load."""
+        bad = self._fp8_bad.get(name)
+        if bad is None:
+            bad = self._fp8_bad[name] = torch.zeros(1, dtype=torch.int32, device=self.device)
+        for lo in range(0, rows.numel(), FP8_STORE_CHUNK_ROWS):
+            hi = lo + FP8_STORE_CHUNK_ROWS
+            try:
+                E.quantize_rows(values[lo:hi], rows[lo:hi], grp.table, grp.exps, bad)
+            except ValueError:
+                raise ValueError(f"table {name}: a row holds NaN or Inf; an fp8 table quantizes finite "
+                                 "values only") from None
+
+    def check_quantized(self):
+        """Raise ValueError naming a table of an fp8 collection whose rows held NaN or Inf when they were
+        quantized on the device (reads the tables' flags: one host sync, once per checkpoint load)"""
+        if not self._fp8_bad:
+            return
+        names = list(self._fp8_bad)
+        flags = torch.cat([self._fp8_bad[n] for n in names]).cpu().tolist()
+        for n, f in zip(names, flags):
+            if f:
+                raise ValueError(f"table {n}: a row holds NaN or Inf; an fp8 table quantizes finite values only")
 
     def _alloc_buffers(self):
         dev, b, W = self.device, self.b, self.world
@@ -934,6 +1005,12 @@ class EmbeddingCollection:
         bound = math.sqrt(1.0 / max(t.init_capacity, 1))
         if t.init_param is not None and t.init_param.up_bound > 0:
             bound = t.init_param.up_bound
+        if grp.exps is not None:
+            # serving (fp8) arenas admit keys only while a checkpoint loads: the admitted ways are read back
+            ways = adm[0][:int(adm[1][0])]
+            vals = E.evict_init_rows(self.evict_init_key(t.name), ht.keys[ways], sl["col0"], grp.pitch, bound)
+            self._store_rows(grp, t.name, ways + sl["row_off"], vals)
+            return
         o = grp.opt
         s0_init = o.initial_accu_value if (o is not None and o.optimizer_type in
                                            (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad)) else 0.0
@@ -1118,7 +1195,10 @@ class EmbeddingCollection:
             bound = t.init_param.up_bound
         gen = torch.Generator(device=dev)
         gen.manual_seed(_stable_seed(self.seed, sl["table"], sl["cpart"], sl["s"], new_rows))
-        table = relayout(grp.table, lambda v: _uniform_fill(v, bound, gen))
+        fp8 = grp.exps is not None
+        # (an fp8 arena's new rows are filled below, through the quantizing write path)
+        table = relayout(grp.table, (lambda v: None) if fp8 else (lambda v: _uniform_fill(v, bound, gen)))
+        grp.exps = relayout(grp.exps, lambda v: None, 1)
         accu = grp.opt.initial_accu_value if (grp.opt is not None and grp.opt.optimizer_type in
                                               (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad)) else 0.0
         s0 = relayout(grp.s0, lambda v: v.fill_(accu), grp.state_pitch)
@@ -1130,11 +1210,13 @@ class EmbeddingCollection:
                 other["row_off"] += delta
         sl["rows"] = new_rows
         grp.rows += delta
+        if fp8:
+            self._fill_uniform(grp, sl["table"], old_end, delta, bound, gen)
 
     def _resync_storage(self, owner):
         """after a growth: this plan's groups point at the owner's arrays and carry the new row windows"""
         for grp, src in zip(self.groups, owner.groups):
-            grp.table, grp.s0, grp.s1, grp.rows = src.table, src.s0, src.s1, src.rows
+            grp.table, grp.s0, grp.s1, grp.rows, grp.exps = src.table, src.s0, src.s1, src.rows, src.exps
             for sl, so in zip(grp.table_slices, src.table_slices):
                 sl["row_off"], sl["rows"] = so["row_off"], so["rows"]
             for d, sl in zip(grp.lookups, getattr(grp, "lookup_slices", [])):
@@ -1144,7 +1226,7 @@ class EmbeddingCollection:
     def _lookup(self, grp):
         s = grp.src
         E.forward(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, s.keys, s.out, self.b, self.rank,
-                  nnz_bufs=s.nnz, key_bytes=self._kb, act_bf16=self._abf, weight_bufs=s.weights)
+                  nnz_bufs=s.nnz, key_bytes=self._kb, act_bf16=self._abf, weight_bufs=s.weights, row_exp=grp.exps)
 
     def forward_compute(self):
         collective = self.world > 1 and not self.fused
@@ -1327,11 +1409,10 @@ class EmbeddingCollection:
     # ------------------------------------------------------------------ checkpoint helpers
     def local_table_items(self):
         """yield (table name, column part, global keys tensor, weights [rows, ev], group, slice); the
-        weights are fp32 (a view of an fp32 arena, an exact fp32 copy of a bf16 one)"""
+        weights are fp32 (a view of an fp32 arena, an exact fp32 copy of a bf16 or fp8 one)"""
         for grp in self.groups:
             for sl in grp.table_slices:
-                w = grp.table[sl["row_off"] * grp.pitch:(sl["row_off"] + sl["rows"]) * grp.pitch] \
-                    .view(sl["rows"], grp.pitch).float()
+                w = _rows_fp32(grp, sl["row_off"], sl["row_off"] + sl["rows"])
                 keys = torch.arange(sl["rows"], dtype=torch.int64) * sl["k"] + sl["s"]
                 yield sl["table"], sl, keys, w, grp
 
@@ -1370,6 +1451,9 @@ class EmbeddingCollection:
                         continue
                     rows = (sl["row_off"] + keys[m] // sl["k"]).to(grp.table.device)
                 c0, ev = sl["col0"], sl["ev"]
+                if grp.exps is not None:
+                    self._store_rows(grp, name, rows, values[m][:, c0:c0 + ev])
+                    continue           # (a serving arena keeps no optimizer state)
                 grp.table.view(-1, grp.pitch)[rows] = values[m][:, c0:c0 + ev].to(grp.table.device,
                                                                                  torch.float32).to(grp.table.dtype)
                 if state is not None:
@@ -1420,7 +1504,7 @@ class EmbeddingCollection:
 
     def dump_table_local(self, name: str, only=None):
         """-> list of (keys int64 [n], values fp32 [n, ev_part], col0, states list) local shards (a bf16
-        arena's values widen to fp32 exactly).
+        arena's values widen to fp32 exactly, an fp8 arena's dequantize exactly).
         ``only``: optional set of part indices to materialise (others are returned as None)."""
         res = []
         for grp in self.groups:
@@ -1431,7 +1515,7 @@ class EmbeddingCollection:
                     res.append(None)
                     continue
                 lo, hi = sl["row_off"], sl["row_off"] + sl["rows"]
-                w = grp.table.view(-1, grp.pitch)[lo:hi].detach().float().cpu()
+                w = _rows_fp32(grp, lo, hi).detach().cpu()
                 keys = torch.arange(sl["rows"], dtype=torch.int64) * sl["k"] + sl["s"]
                 sts = [None if t is None else t.view(-1, grp.state_pitch)[lo:hi].detach().float().cpu()
                        .expand(hi - lo, grp.pitch).contiguous() for t in (grp.s0, grp.s1)]
@@ -1447,7 +1531,7 @@ class EmbeddingCollection:
     def memory_bytes(self) -> int:
         tot = 0
         for grp in self.groups:
-            for t in (grp.table, grp.s0, grp.s1):
+            for t in (grp.table, grp.exps, grp.s0, grp.s1):
                 if t is not None:
                     tot += t.numel() * t.element_size()
         return tot + sum(sk.nbytes() for sk in self._admit_sketches())

@@ -423,8 +423,8 @@ class SetAssocTable:
                              None if s0 is None else s0.data_ptr(), None if s1 is None else s1.data_ptr(),
                              int(row_off), int(init_key) & ((1 << 64) - 1), float(bound), float(s0_init),
                              int(pitch), int(col0), int(s0_pitch), sbf)
-            from .ops import table_bf16
-            self._call("hctr_evict_reinit", C.byref(p), int(max_adm), table_bf16(table), self._st())
+            from .ops import table_type
+            self._call("hctr_evict_reinit", C.byref(p), int(max_adm), table_type(table), self._st())
             return
         from .ops import evict_init_rows
         ways = adm[0][:int(adm[1][0])]

@@ -37,7 +37,7 @@ class CEmbParams(C.Structure):
                 ("num_lookups", C.c_int), ("keys", C.c_void_p * MAX_RANKS),
                 ("nnz", C.c_void_p * MAX_RANKS), ("out", C.c_void_p * MAX_RANKS),
                 ("grad", C.c_void_p * MAX_RANKS), ("lookups", C.c_void_p), ("table", C.c_void_p),
-                ("ev_size", C.c_int), ("weights", C.c_void_p * MAX_RANKS)]
+                ("ev_size", C.c_int), ("weights", C.c_void_p * MAX_RANKS), ("row_exp", C.c_void_p)]
 
 
 class CUniqueTable(C.Structure):
@@ -76,9 +76,10 @@ def lib():
                                                  C.POINTER(CBwdIndex), vp, vp, i, i,
                                                  C.POINTER(COptHyper), f, i, vp, i, i, vp]
         l.hctr_emb_dp_rowwise_update.argtypes = [vp, vp, vp, ll, i, C.POINTER(COptHyper), i, vp]
+        l.hctr_emb_quantize_rows.argtypes = [vp, vp, ll, i, vp, vp, vp, vp]
         for n in ("hctr_emb_forward", "hctr_emb_backward_accum", "hctr_emb_update",
                   "hctr_emb_gather_rows", "hctr_emb_bwd_index", "hctr_emb_bwd_reduce_update",
-                  "hctr_emb_dp_rowwise_update"):
+                  "hctr_emb_dp_rowwise_update", "hctr_emb_quantize_rows"):
             getattr(l, n).restype = i
         # ABI self-check: ctypes mirrors vs the structs the kernels were compiled with
         if hasattr(l, "hctr_abi_sizes_emb"):
@@ -242,11 +243,12 @@ def dispatch(src: torch.Tensor, routes: List[Route], routes_dev, dst_bufs, nnz_b
 
 # ----------------------------------------------------------------------------- forward
 def _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes, act_bf16,
-            nnz_bufs=None, weight_bufs=None, out_bufs=None, grad_bufs=None):
+            nnz_bufs=None, weight_bufs=None, out_bufs=None, grad_bufs=None, row_exp=None):
     """CEmbParams of a launch over one source rank per entry of ``key_bufs`` (tensors, or int device
     pointers for peers), with the key width and whether the outputs / gradients are bf16: read from the
     buffers that are tensors, ``key_bytes`` / ``act_bf16`` where every one is a pointer.  The weight
-    pointers stay null without a weighted lookup (the kernels' unweighted instantiations)."""
+    pointers stay null without a weighted lookup (the kernels' unweighted instantiations); ``row_exp``
+    (uint8 [rows]) is the exponent array of an e4m3 arena."""
     def ptr(x):
         return x if isinstance(x, int) else x.data_ptr()
     p = CEmbParams()
@@ -269,6 +271,7 @@ def _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key
     p.lookups = lookups_dev.data_ptr()
     p.table = table.data_ptr()
     p.ev_size = ev_pitch
+    p.row_exp = None if row_exp is None else row_exp.data_ptr()
     return p, kb, abf
 
 
@@ -283,22 +286,28 @@ def _key_weights(lk, weight_bufs, src, batch, own):
 
 
 def forward(lookups, lookups_dev, table, ev_pitch, key_bufs, out_bufs, batch, my_rank=0,
-            nnz_bufs=None, key_bytes=4, act_bf16=True, weight_bufs=None):
+            nnz_bufs=None, key_bytes=4, act_bf16=True, weight_bufs=None, row_exp=None):
     """key_bufs / out_bufs (/ weight_bufs, fp32 per-key weights of weighted lookups): one entry per
-    source rank (tensor, or int device pointer for peers)."""
+    source rank (tensor, or int device pointer for peers).  An e4m3 ``table`` takes its exponent array
+    ``row_exp`` (see fp8_rows_quantize)."""
+    ttype = table_type(table, fp8=True)
+    if (ttype == FP8) != (row_exp is not None):
+        raise ValueError("an e4m3 arena, and only one, takes its row exponents (row_exp)")
     if table.is_cuda:
         p, kb, out_bf16 = _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes,
-                                  act_bf16, nnz_bufs, weight_bufs, out_bufs=out_bufs)
+                                  act_bf16, nnz_bufs, weight_bufs, out_bufs=out_bufs, row_exp=row_exp)
         max_ev = max((l.ev_size for l in lookups), default=ev_pitch)
         check_ev_size(max_ev)
         al4 = int(vec4_aligned(lookups, ev_pitch, [table, *out_bufs], grad=False))
-        rc = lib().hctr_emb_forward(C.byref(p), max_ev, kb, out_bf16, al4, table_bf16(table),
-                                    _st(table.device))
+        if al4 and ttype == FP8 and ev_pitch % FP8_ROW_UNIT == 0 and \
+                all(l.ev_size % FP8_ROW_UNIT == 0 for l in lookups) and table.data_ptr() % 16 == 0:
+            al4 = FP8_ROW_UNIT        # whole 16-byte units: one 16-byte load per lane and row
+        rc = lib().hctr_emb_forward(C.byref(p), max_ev, kb, out_bf16, al4, ttype, _st(table.device))
         if rc:
             raise RuntimeError(f"hctr_emb_forward failed rc={rc}")
         D._count()
         return
-    forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs, weight_bufs)
+    forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs, weight_bufs, row_exp)
 
 
 def _bag(lk: LookupDesc, key_bufs, nnz_bufs, src, batch):
@@ -319,13 +328,15 @@ def _bag(lk: LookupDesc, key_bufs, nnz_bufs, src, batch):
     return own, lk.table_row_off + torch.where(own, r, torch.zeros_like(r)), nnz
 
 
-def forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs=None, weight_bufs=None):
+def forward_reference(lookups, table, ev_pitch, key_bufs, out_bufs, batch, nnz_bufs=None, weight_bufs=None,
+                      row_exp=None):
     tab = table.view(-1, ev_pitch)
     for src in range(len(key_bufs)):
         obuf = out_bufs[src].reshape(-1)
         for lk in lookups:
             own, rows, nnz = _bag(lk, key_bufs, nnz_bufs, src, batch)
-            v = tab[rows][..., :lk.ev_size].float() * _key_weights(lk, weight_bufs, src, batch, own).unsqueeze(-1)
+            r = tab[rows] if row_exp is None else fp8_rows_dequantize(tab[rows], row_exp[rows])
+            v = r[..., :lk.ev_size].float() * _key_weights(lk, weight_bufs, src, batch, own).unsqueeze(-1)
             pooled = v.sum(1)
             if lk.combiner == 1:
                 pooled = pooled / nnz.clamp(min=1).view(-1, 1).float()
@@ -476,12 +487,61 @@ def backward_accum(lookups, lookups_dev, table, ev_pitch, key_bufs, grad_bufs, b
     ws.ref_rows, ws.ref_grads = rows, grads
 
 
-# ----------------------------------------------------------------------------- bf16 weights
-def table_bf16(table) -> int:
-    """1 when the arena stores bf16 weights (the kernels' WT = __nv_bfloat16), 0 for fp32"""
-    if table.dtype not in (torch.float32, torch.bfloat16):
-        raise TypeError(f"embedding tables are fp32 or bf16, not {table.dtype}")
-    return int(table.dtype == torch.bfloat16)
+# ----------------------------------------------------------------------------- bf16 and fp8 weights
+FP32, BF16, FP8 = 0, 1, 2
+# e4m3 rows whose every lookup width and pitch are multiples of 16 columns are gathered with one 16-byte load per
+# lane and row (docs/performance.md: faster than 4 or 8 bytes per lane at ev 128 and 256); others 4 or 1 columns
+FP8_ROW_UNIT = 16
+_TABLE_TYPES = {torch.float32: FP32, torch.bfloat16: BF16, torch.float8_e4m3fn: FP8}
+
+
+def table_type(table, fp8: bool = False) -> int:
+    """storage code of an arena for the launchers (the kernels' WT): FP32, BF16, or FP8 (e4m3 with one
+    power-of-two scale per row; serving arenas, which only the lookup takes: ``fp8`` allows it)"""
+    t = _TABLE_TYPES.get(table.dtype)
+    if t is None or (t == FP8 and not fp8):
+        raise TypeError(f"embedding tables are fp32 or bf16{' or e4m3' if fp8 else ''}, not {table.dtype}")
+    return t
+
+
+def fp8_rows_quantize(x: torch.Tensor):
+    """e4m3 rows of the fp32 rows ``x`` [n, ev] with one power-of-two scale per row, bit for bit as
+    hctr_emb_quantize_rows: (q float8_e4m3fn [n, ev], exps uint8 [n] = e + 127), where e is the exponent
+    rule of the MX blocks (ops.mxfp8.e4m3_scale_exponent) over the row's amax and q = e4m3(x * 2^-e),
+    saturating and rounded to nearest even.  ``x`` must be finite; an all-zero row gets e = -127."""
+    from ..ops.mxfp8 import e4m3_scale_exponent
+    xf = x.detach().float()
+    e = e4m3_scale_exponent(xf.abs().amax(-1) if xf.shape[-1] else torch.zeros(xf.shape[:-1]))
+    # x * 2^-e <= 448, below torch's e4m3 overflow to NaN (~464)
+    q = (xf * torch.ldexp(torch.ones_like(e), (-e).to(torch.int32)).unsqueeze(-1)).to(torch.float8_e4m3fn)
+    return q, (e + 127).to(torch.uint8)
+
+
+def fp8_rows_dequantize(q: torch.Tensor, exps: torch.Tensor) -> torch.Tensor:
+    """fp32 rows q * 2^e of e4m3 rows ``q`` [..., ev] and their exponent bytes ``exps`` [...] (exact)"""
+    e = exps.to(torch.int32) - 127
+    return q.float() * torch.ldexp(torch.ones(e.shape, dtype=torch.float32, device=q.device), e).unsqueeze(-1)
+
+
+def quantize_rows(values: torch.Tensor, rows: torch.Tensor, table: torch.Tensor, exps: torch.Tensor, bad):
+    """Store the fp32 rows ``values`` [n, pitch] at arena rows ``rows`` (int64 [n], distinct) of the e4m3
+    arena ``table`` and its exponents ``exps`` (fp8_rows_quantize).  On CUDA a non-finite value sets the
+    int32 device flag ``bad`` (no host sync); on CPU it raises ValueError."""
+    pitch = values.shape[1]
+    if table.is_cuda:
+        v = values.to(table.device, torch.float32).contiguous()
+        r = rows.to(table.device, torch.int64).contiguous()
+        rc = lib().hctr_emb_quantize_rows(v.data_ptr(), r.data_ptr(), r.numel(), pitch, table.data_ptr(),
+                                          exps.data_ptr(), bad.data_ptr(), _st(table.device))
+        if rc:
+            raise RuntimeError(f"hctr_emb_quantize_rows failed rc={rc}")
+        D._count()
+        return
+    if not bool(torch.isfinite(values).all()):
+        raise ValueError("non-finite value in rows to quantize")
+    q, e = fp8_rows_quantize(values)
+    table.view(-1, pitch)[rows] = q
+    exps[rows] = e
 
 
 _M64 = (1 << 64) - 1
@@ -559,7 +619,7 @@ def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: d
         rc = lib().hctr_emb_update(table.data_ptr(), 0 if s0 is None else s0.data_ptr(),
                                    0 if s1 is None else s1.data_ptr(), ws.wgrad.data_ptr(),
                                    C.byref(ws.c), ev_pitch, OPT_CODE[opt], sbf, C.byref(h),
-                                   ws.overflow.data_ptr(), num_sms, table_bf16(table),
+                                   ws.overflow.data_ptr(), num_sms, table_type(table),
                                    _st(table.device))
         if rc:
             raise RuntimeError("hctr_emb_update failed")
@@ -592,7 +652,7 @@ def update_rows(opt: Optimizer_t, table, s0, s1, ev_pitch, rows, grads, hp: dict
         a = a.view(-1)
     step = int(step_t.item())
     sparse_opt_reference(opt, w, a, b, g, hp, float(lr_t.item()), step)
-    if table_bf16(table):
+    if table_type(table) == BF16:
         idx = uniq.view(-1, 1) * ev_pitch + torch.arange(ev_pitch, device=uniq.device).view(1, -1)
         w = sr_round_bf16(w, sr_seed(hp), step, idx)
     tab[uniq] = w
@@ -629,7 +689,7 @@ def gather_rows(table, ev_pitch, rows, out):
     if table.is_cuda and rows.dtype == torch.int64:
         rc = lib().hctr_emb_gather_rows(table.data_ptr(), rows.data_ptr(), out.data_ptr(),
                                         rows.numel(), ev_pitch, int(out.dtype == torch.bfloat16),
-                                        table_bf16(table), _st(table.device))
+                                        table_type(table), _st(table.device))
         if rc:
             raise RuntimeError("hctr_emb_gather_rows failed")
         D._count()
@@ -674,7 +734,7 @@ def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_
                                           0 if s0 is None else s0.data_ptr(),
                                           0 if s1 is None else s1.data_ptr(), OPT_CODE[opt], sbf,
                                           C.byref(h), float(grad_scale), gbf, ws.overflow.data_ptr(),
-                                          num_sms, table_bf16(table), _st(table.device))
+                                          num_sms, table_type(table), _st(table.device))
     if rc:
         raise RuntimeError(f"hctr_emb_bwd_reduce_update failed rc={rc}")
     D._count(3)

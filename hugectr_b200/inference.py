@@ -30,6 +30,9 @@ class InferenceParams:
     i64_input_key: bool = False
     use_mixed_precision: bool = False
     embedding_collection_path: str = ""
+    # serve every embedding-collection table as fp8: e4m3 rows with one power-of-two scale per row, quantized
+    # while the tables load, dequantized per looked-up row (the dense network still gets fp32 / bf16 inputs)
+    fp8_quant: bool = False
 
 
 class InferenceModel:
@@ -48,7 +51,15 @@ class InferenceModel:
         if weighted:
             # predict() takes keys only: the weights of these inputs would be dropped
             raise ValueError(f"weighted input {weighted[0]}: the inference session does not take per-key weights")
+        if params.fp8_quant and not self.model.ebc_configs:
+            raise ValueError("fp8_quant quantizes embedding-collection tables; this model has none (legacy "
+                             "SparseEmbedding tables keep their storage)")
+        self.model.serving, self.model.fp8_quant = True, bool(params.fp8_quant)
         self.model.compile()
+        if params.fp8_quant:
+            from .utils import logger
+            logger.info("fp8_quant: embedding-collection tables served as fp8: "
+                        + ", ".join(t.name for e in self.model.ebcs_eval for t in e.tables))
         if params.dense_model_file:
             self.model.load_dense_weights(params.dense_model_file)
         self.hps = {}

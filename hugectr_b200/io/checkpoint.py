@@ -475,6 +475,7 @@ def embedding_load(model, path: str, table_names=None):
             for tid, keys, W, S in iter_ebc_folder(folder, chunk):
                 if table_names is None or names[tid] in table_names:
                     ebc.load_table_rows(names[tid], keys, W, S)
+            ebc.check_quantized()
             continue
         tabs = read_ebc_folder(folder, fs)
         names = [t.name for t in ebc.tables]
@@ -483,4 +484,5 @@ def embedding_load(model, path: str, table_names=None):
             if table_names is not None and n not in table_names:
                 continue
             ebc.load_table_rows(n, keys, W, S)
+        ebc.check_quantized()
     model.comm.barrier()

@@ -81,6 +81,10 @@ class Model:
             torch.backends.cudnn.allow_tf32 = True
         self.key_dtype = torch.int64 if solver.i64_input_key else torch.int32
         self.launches_per_step = 0
+        # set before compile() by an inference session: the embedding collections are built for serving (no
+        # optimizer state, workspace or gradient buffers), with fp8 tables when fp8_quant is set
+        self.serving = False
+        self.fp8_quant = False
 
     # ------------------------------------------------------------------ graph construction
     def add(self, obj):
@@ -208,13 +212,16 @@ class Model:
                     if prm[0].slot_num != 1:
                         raise ValueError("EmbeddingCollection requires slot_num == 1 per sparse param")
             cfg = self._apply_device_layout(cfg)
-            e = EmbeddingCollection(cfg, self.b_train, hot, self.device, self.act_dtype, self.comm,
-                                    self.opt_params, self.key_dtype,
+            # a serving model has one collection at the eval batch: it serves the eval graph and is the one
+            # embedding_load / embedding_dump reach through ebcs_train
+            kw = dict(is_train=False, fp8_quant=self.fp8_quant) if self.serving else {}
+            e = EmbeddingCollection(cfg, self.b_eval if self.serving else self.b_train, hot, self.device,
+                                    self.act_dtype, self.comm, self.opt_params, self.key_dtype,
                                     scaler=s.scaler if self.mixed else 1.0, state_dtype=state_dtype,
                                     seed=s.seed,
-                                    fused=None if s.fused_embedding_comm else False, weighted=weighted)
+                                    fused=None if s.fused_embedding_comm else False, weighted=weighted, **kw)
             self.ebcs_train.append(e)
-            self.ebcs_eval.append(e.eval_clone(self.b_eval))
+            self.ebcs_eval.append(e if self.serving else e.eval_clone(self.b_eval))
         self.legacy_train, self.legacy_eval = [], []
         if self.sparse_embeddings:
             from .embedding.sparse_embedding import SparseEmbeddingRuntime
@@ -244,9 +251,14 @@ class Model:
         for e in (self.ebcs_train if is_train else self.ebcs_eval):
             for name, shp in e.top_shapes().items():
                 tb = TensorBag(name, shp, self.act_dtype)
-                tb.data = e.top_data[name]
-                tb.grad = e.top_grad[name] if is_train else None
-                tb.ebc, tb.ebc_top = e, name          # lets a Concat alias the top into its output
+                if is_train and not e.is_train:
+                    # the training graph of a serving model is never run: stand-in tops
+                    tb.data = torch.zeros(shp, dtype=self.act_dtype, device=self.device)
+                    tb.grad = torch.zeros_like(tb.data)
+                else:
+                    tb.data = e.top_data[name]
+                    tb.grad = e.top_grad[name] if is_train else None
+                    tb.ebc, tb.ebc_top = e, name          # lets a Concat alias the top into its output
                 src[name] = tb
                 emb_tops.append(name)
         for rt in (self.legacy_train if is_train else self.legacy_eval):

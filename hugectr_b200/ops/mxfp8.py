@@ -61,17 +61,22 @@ def mx_quantize(x: torch.Tensor, q=None, sf=None, transposed: bool = False):
     return q, sf
 
 
+def e4m3_scale_exponent(amax: torch.Tensor) -> torch.Tensor:
+    """fp32 exponents e of the power-of-two scales of blocks whose largest magnitudes are ``amax`` (fp32): the
+    smallest 2^e with amax / 2^e <= 448 (e4m3 max), clamped to [-127, 127], -127 for amax == 0 -- computed exactly
+    as e4m3_scale_exp in csrc/ptx.cuh (fp32 frexp of amax * (1 / 448))"""
+    m, ex = torch.frexp(amax * torch.tensor(1.0 / 448.0, dtype=torch.float32))
+    e = torch.where(m > 0.5, ex, ex - 1).to(torch.float32)
+    return torch.where(amax > 0, e, torch.full_like(e, -127.0)).clamp(-127, 127)
+
+
 def mx_quantize_reference(x: torch.Tensor):
     rows, cols = x.shape
     rp = _pad128(rows)
     xf = torch.zeros(rp, cols, dtype=torch.float32)
     xf[:rows] = x.float().cpu()
     blk = xf.view(rp, cols // 32, 32)
-    amax = blk.abs().amax(-1)
-    # smallest power of two 2^e with amax / 2^e <= 448, computed exactly like the kernel (fp32 frexp)
-    m, ex = torch.frexp(amax * torch.tensor(1.0 / 448.0, dtype=torch.float32))
-    e = torch.where(m > 0.5, ex, ex - 1).to(torch.float32)
-    e = torch.where(amax > 0, e, torch.full_like(e, -127.0)).clamp(-127, 127)
+    e = e4m3_scale_exponent(blk.abs().amax(-1))
     qv = (blk * torch.ldexp(torch.ones_like(e), (-e).to(torch.int32)).unsqueeze(-1)).reshape(rp, cols).to(torch.float8_e4m3fn)
     q = qv.view(torch.uint8)
     sfb = (e + 127).to(torch.uint8)                                   # [rp, cols / 32]
