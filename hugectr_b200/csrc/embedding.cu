@@ -553,6 +553,32 @@ __global__ void __launch_bounds__(256)
   if (lane == 0) exps[r] = static_cast<uint8_t>(e + 127);
 }
 
+// Update tracking (embedding/collection.py, track_updates): stamp[rows[i]] = *clock for the first
+// min(*counter, max_unique) entries of a step's unique-row list.  The count and the clock are read on the
+// device, so a replayed graph stamps with the clock of its own step.  The rows of a list are distinct: plain
+// stores.  Rows at or beyond row_bound are skipped.  Every thread loads kStampIlp list entries before it stores
+// any, so that each thread keeps that many independent loads in flight.
+constexpr int kStampIlp = 4;
+__global__ void __launch_bounds__(256)
+    emb_stamp_rows_kernel(int* __restrict__ stamp, const unsigned long long* __restrict__ rows,
+                          const unsigned int* __restrict__ counter, unsigned int max_unique,
+                          long long row_bound, const long long* __restrict__ clock) {
+  const unsigned int n = min(*counter, max_unique);
+  const int c = static_cast<int>(*clock);
+  const unsigned int stride = gridDim.x * blockDim.x;
+  for (unsigned int i0 = blockIdx.x * blockDim.x + threadIdx.x; i0 < n; i0 += kStampIlp * stride) {
+    unsigned long long r[kStampIlp];
+#pragma unroll
+    for (int k = 0; k < kStampIlp; ++k) {
+      const unsigned long long i = i0 + static_cast<unsigned long long>(k) * stride;
+      r[k] = i < n ? __ldg(rows + i) : ~0ull;
+    }
+#pragma unroll
+    for (int k = 0; k < kStampIlp; ++k)
+      if (r[k] < static_cast<unsigned long long>(row_bound)) stamp[r[k]] = c;
+  }
+}
+
 }  // namespace hctr
 
 using namespace hctr;
@@ -707,5 +733,20 @@ extern "C" int hctr_emb_quantize_rows(const float* src, const long long* rows, l
   if (n == 0) return 0;
   const unsigned blocks = static_cast<unsigned>((n * 32 + 255) / 256);
   emb_quantize_rows_kernel<<<blocks, 256, 0, st>>>(src, rows, n, pitch, static_cast<uint8_t*>(q), exps, bad);
+  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+// stamp: int32 [row_bound] per-row step stamps; rows / counter / max_unique: a unique-row list (UniqueTable's
+// rows and counter); clock: int64 device clock.  The grid covers max_unique and exits at the device count.
+extern "C" int hctr_emb_stamp_rows(int* stamp, const unsigned long long* rows, const unsigned int* counter,
+                                   unsigned int max_unique, long long row_bound, const long long* clock,
+                                   int num_sms, void* stream_) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+  if (max_unique == 0) return 0;
+  // one entry per thread up to 16 blocks per SM; longer lists take kStampIlp entries per thread and pass
+  long long blocks = (static_cast<long long>(max_unique) + 255) / 256;
+  if (blocks > num_sms * 16ll) blocks = num_sms * 16ll;
+  emb_stamp_rows_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(stamp, rows, counter, max_unique,
+                                                                       row_bound, clock);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -103,6 +103,11 @@ class EmbeddingTableConfig:
         if self.admit_decay_steps > 0 and self.admit_threshold == 1:
             raise ValueError(f"table {self.name}: admit_decay_steps needs admit_threshold > 1 (a threshold of 1 "
                              "keeps no counts)")
+        # update tracking (see docs/embedding.md): every training step stamps the rows it updates with the
+        # collection clock, so that Model.embedding_dump_delta can write the rows changed since a clock value
+        self.track_updates = kw.get("track_updates", False)
+        if not isinstance(self.track_updates, bool):
+            raise ValueError(f"table {self.name}: track_updates must be a bool, not {self.track_updates!r}")
 
 
 class EmbeddingCollectionConfig:
@@ -238,6 +243,7 @@ class _Group:
         self.kind, self.pitch, self.wdtype = kind, pitch, wdtype
         self.rowwise = rowwise
         self.exps = None         # fp8 arena: uint8 [rows], e + 127 of each row's scale 2^e
+        self.stamp = None        # int32 [rows]: clock of the last write of each row (groups with a tracked table)
         self.rows = 0
         self.table_slices = []   # (table name, col part, row_off, rows, num_shards, shard_idx, col0)
         self.lookups: List[E.LookupDesc] = []
@@ -320,6 +326,9 @@ class EmbeddingCollection:
             if t.admit_threshold > 1 and (pl.kind != "mp" or pl.col_factor > 1):
                 raise ValueError(f"table {t.name}: an admitting table (admit_threshold > 1) is model parallel, "
                                  f"table-wise or row-wise (placement {pl.kind!r}, column factor {pl.col_factor})")
+            if t.track_updates and t.evict_strategy is not None:
+                raise ValueError(f"table {t.name}: track_updates does not support an evicting table (a delta "
+                                 "records no deletions, so a key evicted in training would stay on the server)")
         self.native = device.type == "cuda"
         self.has_dynamic = any(t.dynamic for t in self.tables)
         self.fused = (self.native and self.world > 1 and comm.p2p_available) if fused is None else fused
@@ -345,9 +354,10 @@ class EmbeddingCollection:
         self._abf = act_dtype == torch.bfloat16
         # clock of the evicting tables: ticked once per training step inside the step (not Model.step_t,
         # which a learning-rate scheduler reset zeroes and Adam's bias correction reads)
-        # and of the admitting tables' sketch decay
+        # and of the admitting tables' sketch decay, and the stamps of the tracked tables' updated rows
         self.evict_clock = torch.zeros(1, dtype=torch.int64, device=device)
-        self.ticks_clock = any(t.evict_strategy is not None or t.admit_threshold > 1 for t in self.tables)
+        self.ticks_clock = any(t.evict_strategy is not None or t.admit_threshold > 1 or t.track_updates
+                               for t in self.tables)
         self._build_layout(hotness)
         self._build_storage(seed)
         self._alloc_buffers()
@@ -596,6 +606,10 @@ class EmbeddingCollection:
             grp.table = torch.empty(n, dtype=STORAGE_DTYPES[grp.wdtype], device=dev)
             if grp.wdtype == "fp8":
                 grp.exps = torch.empty(max(grp.rows, 1), dtype=torch.uint8, device=dev)
+            if self.is_train and grp.kind == "mp" and any(self.tmap[sl["table"]].track_updates
+                                                          for sl in grp.table_slices):
+                # (a data-parallel table is written whole in every delta: no stamps)
+                grp.stamp = torch.zeros(max(grp.rows, 1), dtype=torch.int32, device=dev)
             self._init_group(grp, gen, seed)
             sdt = self.state_dtype if grp.kind == "mp" else torch.float32
             grp.s0, grp.s1 = opt_states(grp.opt, n, sdt, dev) if self.is_train else (None, None)
@@ -955,6 +969,10 @@ class EmbeddingCollection:
                     self.comm.all_to_all_v(recv, ch.slab.index_select(0, pk["key_all"]), [pk["kn_me"]] * W, pk["kn"])
                     if pk["kn_me"]:
                         ch.all.index_copy_(1, pk["key_me"], recv.view(W, pk["kn_me"]))
+        if self.is_train and self.ticks_clock:
+            getattr(self, "_shared", self).evict_clock.add_(1)
+            for sk in self._admit_sketches():
+                sk.decay()
         if self.has_dynamic:
             self._translate_dynamic_keys()
 
@@ -1082,15 +1100,11 @@ class EmbeddingCollection:
         """Dynamic tables: overwrite the (gathered) keys of their lookups with local row indices -- new
         keys get the next free row while training, unknown keys read as empty (-1) in evaluation; keys
         owned by another shard become -1.  The lookup kernels then run exactly as for static tables.
-        A training step first ticks the clock of the evicting and admitting tables and decays the sketches
-        that are due; an admitting table counts its missing keys in every region before any insert, then
-        rejects the keys below its threshold (-1) ahead of each insert."""
+        (forward_begin has ticked the collection clock and decayed the sketches that are due.)  An admitting
+        table counts its missing keys in every region before any insert, then rejects the keys below its
+        threshold (-1) ahead of each insert."""
         b = self.b
         buf = self.key_slab.view(1, -1) if self.world == 1 else self.key_chans[0].all
-        if self.is_train and self.ticks_clock:
-            getattr(self, "_shared", self).evict_clock.add_(1)
-            for sk in self._admit_sketches():
-                sk.decay()
         growing = []
         for gl in self.glookups:
             t = self.tmap[gl["table"]]
@@ -1203,6 +1217,7 @@ class EmbeddingCollection:
                                               (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad)) else 0.0
         s0 = relayout(grp.s0, lambda v: v.fill_(accu), grp.state_pitch)
         s1 = relayout(grp.s1, lambda v: v.zero_())
+        grp.stamp = relayout(grp.stamp, lambda v: v.zero_(), 1)     # a new row has no key: never written
         grp.table, grp.s0, grp.s1 = table, s0, s1
         old_end = sl["row_off"] + sl["rows"]
         for other in grp.table_slices:
@@ -1217,6 +1232,7 @@ class EmbeddingCollection:
         """after a growth: this plan's groups point at the owner's arrays and carry the new row windows"""
         for grp, src in zip(self.groups, owner.groups):
             grp.table, grp.s0, grp.s1, grp.rows, grp.exps = src.table, src.s0, src.s1, src.rows, src.exps
+            grp.stamp = src.stamp
             for sl, so in zip(grp.table_slices, src.table_slices):
                 sl["row_off"], sl["rows"] = so["row_off"], so["rows"]
             for d, sl in zip(grp.lookups, getattr(grp, "lookup_slices", [])):
@@ -1313,7 +1329,14 @@ class EmbeddingCollection:
             if grp.kind == "mp" and getattr(grp, "indexed", False) and grp.lookups:
                 E.bwd_index(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, grp.src.keys, self.b, grp.ws,
                             self.rank, nnz_bufs=grp.src.nnz, key_bytes=self._kb, weight_bufs=grp.src.weights)
+                self._stamp(grp)
         self._index_done = True
+
+    def _stamp(self, grp):
+        """stamp the rows of ``grp``'s unique-row list of this step with the collection clock (tracked groups;
+        the update consumes the list, so this runs between the index and the update)"""
+        if grp.stamp is not None:
+            E.stamp_rows(grp.stamp, grp.ws, getattr(self, "_shared", self).evict_clock)
 
     def backward(self, lr_t, step_t, dp_stream=None):
         """Consumes top grads (grad slab), updates local tables. grads are already / global batch.
@@ -1388,6 +1411,7 @@ class EmbeddingCollection:
             E.backward_accum(grp.lookups, grp.lookups_dev, grp.table, grp.pitch, s.keys, s.grads,
                              self.b, grp.ws, 1.0, self.rank, nnz_bufs=s.nnz, key_bytes=self._kb,
                              act_bf16=self._abf, weight_bufs=s.weights)
+            self._stamp(grp)
             E.update(o.optimizer_type, grp.table, grp.s0, grp.s1, grp.pitch, grp.ws, self._hp(o),
                      lr_t, step_t)
         else:
@@ -1420,7 +1444,7 @@ class EmbeddingCollection:
         """Scatter (key, row-vector) pairs of table ``name`` into the local shards (re-sharding on
         load: only keys with key % num_shards == shard_id are kept, parameter_IO.cpp:262-350).
         ``state``: optional list of per-state [n, ev] tensors (optimizer states).  A bf16 arena stores
-        the values rounded to nearest."""
+        the values rounded to nearest.  Rows of a tracked group are stamped with the clock + 1."""
         keys = keys.to(torch.int64).cpu()
         for grp in self.groups:
             for sl in grp.table_slices:
@@ -1451,6 +1475,9 @@ class EmbeddingCollection:
                         continue
                     rows = (sl["row_off"] + keys[m] // sl["k"]).to(grp.table.device)
                 c0, ev = sl["col0"], sl["ev"]
+                if grp.stamp is not None:
+                    # written outside a training step: a delta since the current clock holds them
+                    grp.stamp[rows] = (getattr(self, "_shared", self).evict_clock + 1).to(torch.int32)
                 if grp.exps is not None:
                     self._store_rows(grp, name, rows, values[m][:, c0:c0 + ev])
                     continue           # (a serving arena keeps no optimizer state)
@@ -1528,10 +1555,51 @@ class EmbeddingCollection:
                 res.append((keys, w, sl["col0"], sts, grp.kind))
         return res
 
+    def delta_table_local(self, name: str, since: int, keys: Optional[torch.Tensor] = None):
+        """-> list of (keys int64 [n] ascending, values fp32 [n, ev_part], col0, [], kind), one per local shard
+        of table ``name`` in ``dump_table_local`` order, on the host: the keys whose rows were stamped after the
+        clock value ``since`` (every key of a data-parallel shard, which is written whole), or, with ``keys``
+        (int64, host), the given keys that the shard holds.  Values only, no optimizer state.  The selection
+        runs as tensor ops on the stamps; only the selected rows are gathered and moved to the host."""
+        if not self.tmap[name].track_updates:
+            raise ValueError(f"table {name}: it does not track updates (track_updates=False)")
+        res = []
+        for grp in self.groups:
+            for sl in grp.table_slices:
+                if sl["table"] != name:
+                    continue
+                lo, dev = sl["row_off"], grp.table.device
+                if sl.get("dynamic"):
+                    k, r = self._dyn_hash(name, dict(sl, cpart=0)).dump()
+                    k, r = k.to(torch.int64), r.to(torch.int64)
+                    if keys is not None:
+                        sel = torch.isin(k, keys)
+                    elif grp.kind == "dp":
+                        sel = torch.ones_like(k, dtype=torch.bool)
+                    else:
+                        sel = (grp.stamp[lo + r.to(dev)] > since).cpu()
+                    k, r = k[sel], r[sel]
+                else:
+                    if keys is not None:
+                        kk = keys[(keys >= 0) & (keys % sl["k"] == sl["s"]) & (keys // sl["k"] < sl["rows"])]
+                        r = kk // sl["k"]
+                    elif grp.kind == "dp":
+                        r = torch.arange(sl["rows"], dtype=torch.int64)
+                    else:
+                        r = torch.nonzero(grp.stamp[lo:lo + sl["rows"]] > since).view(-1).cpu()
+                    k = r * sl["k"] + sl["s"]
+                order = torch.argsort(k)
+                k, r = k[order], r[order]
+                vals = torch.empty(k.numel(), grp.pitch, dtype=torch.float32, device=dev)
+                if k.numel():
+                    E.gather_rows(grp.table, grp.pitch, (r + lo).to(dev), vals)
+                res.append((k, vals.cpu(), sl["col0"], [], grp.kind))
+        return res
+
     def memory_bytes(self) -> int:
         tot = 0
         for grp in self.groups:
-            for t in (grp.table, grp.exps, grp.s0, grp.s1):
+            for t in (grp.table, grp.exps, grp.s0, grp.s1, grp.stamp):
                 if t is not None:
                     tot += t.numel() * t.element_size()
         return tot + sum(sk.nbytes() for sk in self._admit_sketches())

@@ -77,9 +77,10 @@ def lib():
                                                  C.POINTER(COptHyper), f, i, vp, i, i, vp]
         l.hctr_emb_dp_rowwise_update.argtypes = [vp, vp, vp, ll, i, C.POINTER(COptHyper), i, vp]
         l.hctr_emb_quantize_rows.argtypes = [vp, vp, ll, i, vp, vp, vp, vp]
+        l.hctr_emb_stamp_rows.argtypes = [vp, vp, vp, C.c_uint, ll, vp, i, vp]
         for n in ("hctr_emb_forward", "hctr_emb_backward_accum", "hctr_emb_update",
                   "hctr_emb_gather_rows", "hctr_emb_bwd_index", "hctr_emb_bwd_reduce_update",
-                  "hctr_emb_dp_rowwise_update", "hctr_emb_quantize_rows"):
+                  "hctr_emb_dp_rowwise_update", "hctr_emb_quantize_rows", "hctr_emb_stamp_rows"):
             getattr(l, n).restype = i
         # ABI self-check: ctypes mirrors vs the structs the kernels were compiled with
         if hasattr(l, "hctr_abi_sizes_emb"):
@@ -608,6 +609,28 @@ def evict_init_rows(init_key: int, keys, col0: int, width: int, bound: float, dt
     u = (h >> np.uint64(40)).astype(np.float32) * np.float32(1.0 / 16777216.0)
     w = np.float32(bound) * (np.float32(2.0) * u - np.float32(1.0))
     return torch.from_numpy(w.astype(np.float32)).to(dtype)
+
+
+def stamp_rows(stamp: torch.Tensor, ws, clock: torch.Tensor, num_sms: int = 132):
+    """Update tracking: ``stamp[row] = clock`` for every row of the step's unique-row list of ``ws`` (int32
+    ``stamp`` [arena rows], int64 ``clock`` [1] on the device).  On CUDA one launch reads the list's count and
+    the clock from device memory (capturable; the first min(counter, max_unique) entries of ``ws.rows``).  On
+    the CPU the rows accumulated in ``ws.ref_rows`` are stamped with tensor ops, the kernel's reference.  Rows
+    at or beyond ``stamp.numel()`` are skipped.  Call it after the list is built and before the update that
+    clears it."""
+    if stamp.is_cuda:
+        rc = lib().hctr_emb_stamp_rows(stamp.data_ptr(), ws.rows.data_ptr(), ws.counter.data_ptr(),
+                                       int(ws.max_unique), stamp.numel(), clock.data_ptr(), num_sms,
+                                       _st(stamp.device))
+        if rc:
+            raise RuntimeError(f"hctr_emb_stamp_rows failed rc={rc}")
+        D._count()
+        return
+    rows = ws.ref_rows
+    if rows is None or rows.numel() == 0:
+        return
+    rows = rows[(rows >= 0) & (rows < stamp.numel())]
+    stamp[rows] = clock.to(torch.int32)
 
 
 def update(opt: Optimizer_t, table, s0, s1, ev_pitch, ws: UniqueWorkspace, hp: dict, lr_t, step_t,

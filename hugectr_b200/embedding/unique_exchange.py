@@ -156,6 +156,8 @@ class UniqueExchange:
                 continue
             g = torch.zeros(int(ok.sum()), grp.pitch, dtype=torch.float32, device=dev)
             g[:, :ev] = got[sel[ok], :ev].float()
+            if grp.stamp is not None:
+                grp.stamp[row[ok]] = getattr(e, "_shared", e).evict_clock.to(torch.int32)
             E.update_rows(grp.opt.optimizer_type, grp.table, grp.s0, grp.s1, grp.pitch, row[ok], g,
                           e._hp(grp.opt), lr_t, step_t)
 

@@ -216,6 +216,8 @@ def model_to_json(model) -> dict:
                     tj["admit_decay_steps"] = t.admit_decay_steps
             if getattr(t, "weight_dtype", "fp32") != "fp32":
                 tj["weight_dtype"] = t.weight_dtype
+            if t.track_updates:
+                tj["track_updates"] = True
             if t.init_param is not None and getattr(t.init_param, "up_bound", 0) > 0:
                 tj["init_up_bound"] = float(t.init_param.up_bound)
             tabs.append(tj)
@@ -266,7 +268,7 @@ def add_from_json(model, graph: dict, include_dense_network: bool = True):
             tabs = {}
             for tt in j["tables"]:
                 kw = {k: tt[k] for k in ("init_capacity", "max_capacity", "weight_dtype", "evict_strategy",
-                                         "admit_threshold", "admit_decay_steps") if k in tt}
+                                         "admit_threshold", "admit_decay_steps", "track_updates") if k in tt}
                 ip = InitParams(up_bound=tt["init_up_bound"]) if "init_up_bound" in tt else None
                 tabs[tt["name"]] = EmbeddingTableConfig(
                     tt["name"], tt["max_vocabulary_size"], tt["ev_size"],

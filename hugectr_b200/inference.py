@@ -76,6 +76,36 @@ class InferenceModel:
         if params.embedding_collection_path:
             self.model.embedding_load(params.embedding_collection_path)
         self.params = params
+        # {collection id: the until clock of the last delta applied} (update_embedding)
+        self.delta_clocks = {}
+
+    def update_embedding(self, path: str):
+        """Apply a delta folder written by ``Model.embedding_dump_delta`` in place (new keys of a growing table
+        are inserted, fp8 tables quantize the rows as they load).  Deltas apply in clock order: one whose
+        ``since`` is after the ``until`` of the last delta applied to a collection leaves a gap and raises
+        ValueError, and so does one whose ``until`` is before that clock (it would roll rows back to older values);
+        an overlap is fine (rows carry absolute values).  The first delta after the full load is
+        accepted whatever its ``since``.  A table the session lacks raises ValueError."""
+        from .io.checkpoint import read_delta_info
+        m = self.model
+        info = read_delta_info(path, m)
+        for eid, d in info.items():
+            if eid >= len(m.ebcs_train):
+                raise ValueError(f"delta {path}: embedding collection {eid} is not in this session")
+            have = {t.name for t in m.ebcs_train[eid].tables}
+            for n in d["tables"]:
+                if n not in have:
+                    raise ValueError(f"delta {path}: table {n} of embedding collection {eid} is not in this session")
+            last = self.delta_clocks.get(eid)
+            if last is not None and d["since"] > last:
+                raise ValueError(f"delta {path}: embedding collection {eid} starts after clock {d['since']}, but the "
+                                 f"session holds the rows of clock {last}: the deltas in between are missing")
+            if last is not None and d["until"] < last:
+                raise ValueError(f"delta {path}: embedding collection {eid} ends at clock {d['until']}, but the "
+                                 f"session holds the rows of clock {last}: applying it would roll rows back")
+        m.embedding_load(path)
+        for eid, d in info.items():
+            self.delta_clocks[eid] = int(d["until"])
 
     def predict(self, dense: np.ndarray, keys: np.ndarray) -> np.ndarray:
         """dense [n, dense_dim] float32, keys: feature-major key vector of the batch -> predictions"""

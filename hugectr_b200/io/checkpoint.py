@@ -201,9 +201,10 @@ def _file_head(ftype: int, table_id: int) -> bytes:
     return head.tobytes()
 
 
-def _gather_table(model, ebc, name):
-    """rank 0 gets the whole table: (keys int64 [n], weights [n, ev], states)"""
-    parts = ebc.dump_table_local(name)
+def _gather_table(model, ebc, name, parts=None):
+    """rank 0 gets the whole table: (keys int64 [n], weights [n, ev], states); ``parts``: this rank's shards in
+    the form of ``dump_table_local`` (default: all of them)"""
+    parts = ebc.dump_table_local(name) if parts is None else parts
     allp = model.comm.all_gather_object(parts) if model.world > 1 else [parts]
     if model.comm.rank != 0:
         return None
@@ -347,25 +348,82 @@ def embedding_dump(model, path: str, table_names=None):
         for tid in ids:
             tabs[tid] = _gather_table(model, ebc, names[tid])
         if model.comm.rank == 0:
-            fs.create_dir(folder)
-            head = np.zeros(5, dtype="<i4")
-            head[0] = len(ids)
-            head[1] = 1 if model.key_dtype == torch.int64 else 0
-            head[2] = 0   # fp32 values
-            meta = head.tobytes() + np.asarray(ids, dtype="<i4").tobytes() + \
-                np.asarray([tabs[t][0].numel() for t in ids], dtype="<u8").tobytes() + \
-                np.asarray([ebc.tables[t].ev_size for t in ids], dtype="<i4").tobytes()
-            fs.write(f"{folder}/meta_data", meta)
-            kd = "<i8" if model.key_dtype == torch.int64 else "<u4"
-            for tid in ids:
-                keys, W, S = tabs[tid]
-                fs.write(f"{folder}/key{tid}", _file_head(1, tid) + keys.numpy().astype(kd).tobytes())
-                fs.write(f"{folder}/weight{tid}", _file_head(2, tid) + W.numpy().astype("<f4").tobytes())
-                st = [s for s in S if s is not None]
-                if st:
-                    fs.write(f"{folder}/opt{tid}", _file_head(3, tid) +
-                             b"".join(s.numpy().astype("<f4").tobytes() for s in st))
+            _write_ebc_folder(model, fs, folder, ebc, ids, tabs)
         model.comm.barrier()
+
+
+def _write_ebc_folder(model, fs, folder, ebc, ids, tabs):
+    """(rank 0) one collection's folder from whole tables ``tabs`` {table id: (keys, weights, states)}"""
+    fs.create_dir(folder)
+    head = np.zeros(5, dtype="<i4")
+    head[0] = len(ids)
+    head[1] = 1 if model.key_dtype == torch.int64 else 0
+    head[2] = 0   # fp32 values
+    meta = head.tobytes() + np.asarray(ids, dtype="<i4").tobytes() + \
+        np.asarray([tabs[t][0].numel() for t in ids], dtype="<u8").tobytes() + \
+        np.asarray([ebc.tables[t].ev_size for t in ids], dtype="<i4").tobytes()
+    fs.write(f"{folder}/meta_data", meta)
+    kd = "<i8" if model.key_dtype == torch.int64 else "<u4"
+    for tid in ids:
+        keys, W, S = tabs[tid]
+        fs.write(f"{folder}/key{tid}", _file_head(1, tid) + keys.numpy().astype(kd).tobytes())
+        fs.write(f"{folder}/weight{tid}", _file_head(2, tid) + W.numpy().astype("<f4").tobytes())
+        st = [s for s in S if s is not None]
+        if st:
+            fs.write(f"{folder}/opt{tid}", _file_head(3, tid) +
+                     b"".join(s.numpy().astype("<f4").tobytes() for s in st))
+
+
+# a delta's clocks: the stamps are int32
+DELTA_CLOCK_LIMIT = 1 << 31
+
+
+def embedding_dump_delta(model, path: str, since=None, table_names=None):
+    """Write, for every table with ``track_updates`` (of ``table_names``, when given), the keys whose rows were
+    stamped after ``since[collection id]`` (0 when absent) with their current fp32 values, in the
+    ``embedding_collection_<id>/`` layout, and ``delta.json`` with each collection's ``since`` / ``until``
+    clocks, tracked tables and data-parallel tables (written whole).  Every rank takes part.  Returns the
+    clocks at the time of the dump {collection id: clock}: the ``since`` of the next delta."""
+    clocks = model.embedding_clocks()
+    for eid, c in clocks.items():
+        if c >= DELTA_CLOCK_LIMIT:
+            raise RuntimeError(f"embedding collection {eid}: clock {c} reached 2^31, beyond the int32 row stamps")
+    since = {eid: int((since or {}).get(eid, 0)) for eid in clocks}
+    fs = _fs(path, model)
+    info = {}
+    for eid, ebc in enumerate(model.ebcs_train):
+        names = [t.name for t in ebc.tables]
+        tracked = [n for n in names if ebc.tmap[n].track_updates and (table_names is None or n in table_names)]
+        ids = [names.index(n) for n in tracked]
+        tabs = {}
+        for tid in ids:
+            n = names[tid]
+            parts = ebc.delta_table_local(n, since[eid])
+            if ebc.placement[n].col_factor > 1:
+                # a key whose row any column slice stamped is written with its full row: every slice reads the
+                # union of the stamped keys (the slices of a key are updated in the same steps, so they agree)
+                mine = [p[0] for p in parts]
+                allk = model.comm.all_gather_object(mine) if model.world > 1 else [mine]
+                keys = [k for r in allk for k in r]
+                keys = torch.unique(torch.cat(keys)) if keys else torch.zeros(0, dtype=torch.int64)
+                parts = ebc.delta_table_local(n, since[eid], keys=keys)
+            tabs[tid] = _gather_table(model, ebc, n, parts)
+        if model.comm.rank == 0:
+            _write_ebc_folder(model, fs, f"{path}/embedding_collection_{eid}", ebc, ids, tabs)
+        info[str(eid)] = {"since": since[eid], "until": clocks[eid], "tables": tracked,
+                          "data_parallel": [n for n in tracked if ebc.placement[n].kind == "dp"]}
+    if model.comm.rank == 0:
+        fs.write(f"{path}/delta.json", json.dumps({"collections": info}, indent=1).encode())
+    model.comm.barrier()
+    return clocks
+
+
+def read_delta_info(path: str, model=None) -> dict:
+    """{collection id: {since, until, tables, data_parallel}} of a folder written by embedding_dump_delta"""
+    fs = _fs(path, model)
+    if not fs.exists(f"{path}/delta.json"):
+        raise ValueError(f"{path}: no delta.json, not a folder written by embedding_dump_delta")
+    return {int(k): v for k, v in json.loads(fs.read(f"{path}/delta.json").decode())["collections"].items()}
 
 
 def _embedding_dump_parallel(model, path, table_names, fs):

@@ -856,7 +856,10 @@ class Model:
 
     # ------------------------------------------------------------------ fit
     def fit(self, num_epochs: int = 0, max_iter: int = 2000, display: int = 200,
-            eval_interval: int = 1000, snapshot: int = 10000, snapshot_prefix: str = ""):
+            eval_interval: int = 1000, snapshot: int = 10000, snapshot_prefix: str = "",
+            delta_interval: int = 0, delta_prefix: str = ""):
+        """``delta_interval`` = N > 0: every N iterations write ``embedding_dump_delta(f"{delta_prefix}{iter}")``
+        of the rows changed since the previous one (the first since the clocks at the start of fit)."""
         s = self.solver
         if not self.compiled:
             raise RuntimeError("call compile() before fit()")
@@ -885,6 +888,7 @@ class Model:
         epoch = 0
         stop = False
         total_iters = max_iter if not epoch_mode else 1 << 62
+        delta_since = self.embedding_clocks() if delta_interval > 0 else None
         while it < total_iters and not stop:
             ok = self.train()
             if not ok:                                  # end of an epoch
@@ -907,6 +911,8 @@ class Model:
                 stop = self._evaluate(it, t_start) or stop
             if snapshot > 0 and it % snapshot == 0 and it != max_iter:
                 self.save_params_to_files(snapshot_prefix, it)
+            if delta_interval > 0 and it % delta_interval == 0:
+                delta_since = self.embedding_dump_delta(f"{delta_prefix}{it}", delta_since)
         for cb in self.callbacks:
             cb.on_training_end(it)
         if rank0:
@@ -1028,6 +1034,24 @@ class Model:
     def embedding_load(self, path: str, table_names=None):
         from .io.checkpoint import embedding_load
         embedding_load(self, path, table_names)
+
+    def embedding_clocks(self) -> Dict[int, int]:
+        """{collection id: clock} of the embedding collections, read with one host synchronisation: each clock
+        ticks once per training step of a collection with a tracked (or evicting, or admitting) table.  Record
+        them beside a full ``embedding_dump`` as the base of a chain of ``embedding_dump_delta``."""
+        ebcs = getattr(self, "ebcs_train", [])
+        if not ebcs:
+            return {}
+        return {i: int(c) for i, c in enumerate(torch.cat([e.evict_clock for e in ebcs]).cpu().tolist())}
+
+    def embedding_dump_delta(self, path: str, since: Optional[Dict[int, int]] = None,
+                             table_names=None) -> Dict[int, int]:
+        """Write the rows of the tables with ``track_updates`` that changed after the clocks ``since``
+        {collection id: clock} (None: 0) with their current fp32 values, in the ``embedding_dump`` layout plus
+        ``delta.json``; returns the clocks at the dump, the ``since`` of the next delta (docs/embedding.md).
+        Every rank takes part.  ``InferenceModel.update_embedding`` applies such a folder."""
+        from .io.checkpoint import embedding_dump_delta
+        return embedding_dump_delta(self, path, since, table_names)
 
     # ------------------------------------------------------------------ debugging
     def check_out_tensor(self, name: str, which: Tensor_t = Tensor_t.Train):
