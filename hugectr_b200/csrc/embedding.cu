@@ -407,12 +407,14 @@ __global__ void __launch_bounds__(256)
   }
 }
 
-// Row-wise AdaGrad on one row by one warp (accumulate path and data-parallel tables): a warp-reduced
-// pass over the row's fp32 gradient gives sum g^2, rowwise_row_step updates the row's accumulator *s,
-// then the update pass applies the factor to every column and zeroes the gradient.
-template <typename WT>
-HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, float* gsrc, long long base, int ev,
-                                      float inv_scaler, const OptHyper& hp, float lr,
+// A row-reduced rule (row-wise AdaGrad, partial row-wise Adam) on one row by one warp (accumulate path
+// and data-parallel tables): a warp-reduced pass over the row's fp32 gradient gives sum g^2,
+// row_reduce_step updates the row's state *s, then the update pass applies the factor to every column
+// (partial row-wise Adam: through the first moments m0 of the arena's element indices) and zeroes the
+// gradient.
+template <int OPT, typename StateT, typename WT>
+HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, StateT* m0, float* gsrc, long long base, int ev,
+                                      float inv_scaler, const OptHyper& hp, const OptStep& st,
                                       unsigned long long srk, int lane) {
   const bool v4 = (ev & 3) == 0;
   float sq = 0.f;
@@ -428,13 +430,13 @@ HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, float* gsrc, long long
     }
   }
   const float s_old = lane == 0 ? *s : 0.f;
-  const float f = rowwise_row_step<32>(0xffffffffu, 0, lane, sq, s_old, s, ev, hp, lr);
+  const float f = row_reduce_step<OPT, 32>(0xffffffffu, 0, lane, sq, s_old, s, ev, hp, st);
   if (v4) {
     for (int col = lane * 4; col < ev; col += 128) {
       const float4 g = *reinterpret_cast<float4*>(gsrc + col);
       *reinterpret_cast<float4*>(gsrc + col) = make_float4(0.f, 0.f, 0.f, 0.f);
       float4 w = load_vec4<WT>(table + base + col);
-      apply_rowwise4(w, scale4(g, inv_scaler), f);
+      row_apply4<OPT, StateT>(w, scale4(g, inv_scaler), f, m0, base + col, hp);
       store_w4<WT>(table + base + col, w, srk, base + col);
     }
   } else {
@@ -442,7 +444,7 @@ HCTR_DEVICE void rowwise_update_warp(WT* table, float* s, float* gsrc, long long
       const float g = gsrc[col] * inv_scaler;
       gsrc[col] = 0.f;
       float w = to_f<WT>(table[base + col]);
-      w -= f * g;
+      row_apply1<OPT, StateT>(w, g, f, m0, base + col, hp);
       store_w<WT>(table + base + col, w, srk, base + col);
     }
   }
@@ -465,8 +467,9 @@ __global__ void __launch_bounds__(256)
     const unsigned long long row = ut.rows[uid];
     float* gsrc = wgrad_unique + static_cast<long long>(uid) * ev;
     const long long base = static_cast<long long>(row) * ev;
-    if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
-      rowwise_update_warp<WT>(table, s0 + row, gsrc, base, ev, inv_scaler, hp, step.lr, srk, lane);
+    if constexpr (kRowRule<OPT>) {
+      rowwise_update_warp<OPT, StateT, WT>(table, row_state<OPT>(s0, s1) + row, s0, gsrc, base, ev, inv_scaler,
+                                           hp, step, srk, lane);
     } else if ((ev & 3) == 0) {
       for (int col = lane * 4; col < ev; col += 128) {
         float4 g = *reinterpret_cast<float4*>(gsrc + col);
@@ -495,14 +498,37 @@ __global__ void __launch_bounds__(256)
     emb_dp_rowwise_update_kernel(float* __restrict__ table, float* __restrict__ s,
                                  float* __restrict__ wgrad, const long long rows, const int pitch,
                                  const OptHyper hp) {
-  const float lr = opt_step<OPT_ROWWISE_ADAGRAD>(hp).lr;
+  const OptStep step = opt_step<OPT_ROWWISE_ADAGRAD>(hp);
   const float inv_scaler = 1.f / hp.scaler;
   const int lane = threadIdx.x & 31;
   const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
   for (long long r = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; r < rows;
        r += warps)
-    rowwise_update_warp<float>(table, s + r, wgrad + r * pitch, r * pitch, pitch, inv_scaler, hp, lr,
-                               0ull, lane);
+    rowwise_update_warp<OPT_ROWWISE_ADAGRAD, float, float>(table, s + r, nullptr, wgrad + r * pitch, r * pitch,
+                                                          pitch, inv_scaler, hp, step, 0ull, lane);
+}
+
+// Data-parallel tables with partial row-wise Adam: table and first moments m [rows, pitch] fp32, second
+// moments v [rows] fp32.  A row whose all-reduced gradient is all zero is skipped: its weights and both
+// moments stay as they are, as an all-zero row leaves them under row-wise AdaGrad (a model-parallel row that
+// was looked up takes the step with g = 0 instead, and its moments decay).
+__global__ void __launch_bounds__(256)
+    emb_dp_prow_adam_update_kernel(float* __restrict__ table, float* __restrict__ m, float* __restrict__ v,
+                                   float* __restrict__ wgrad, const long long rows, const int pitch,
+                                   const OptHyper hp) {
+  const OptStep step = opt_step<OPT_PARTIAL_ROWWISE_ADAM>(hp);
+  const float inv_scaler = 1.f / hp.scaler;
+  const int lane = threadIdx.x & 31;
+  const long long warps = (static_cast<long long>(gridDim.x) * blockDim.x) >> 5;
+  for (long long r = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; r < rows;
+       r += warps) {
+    const float* g = wgrad + r * pitch;
+    bool any = false;
+    for (int c = lane; c < pitch; c += 32) any |= g[c] != 0.f;
+    if (!__any_sync(0xffffffffu, any)) continue;
+    rowwise_update_warp<OPT_PARTIAL_ROWWISE_ADAM, float, float>(table, v + r, m, wgrad + r * pitch, r * pitch,
+                                                               pitch, inv_scaler, hp, step, 0ull, lane);
+  }
 }
 
 __global__ void emb_finish_kernel(unsigned int* counter, unsigned int* overflow_flag,
@@ -709,6 +735,19 @@ extern "C" int hctr_emb_dp_rowwise_update(float* table, float* s, float* wgrad, 
   if (blocks > num_sms * 8ll) blocks = num_sms * 8ll;
   emb_dp_rowwise_update_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(table, s, wgrad, rows,
                                                                               pitch, *hp);
+  return cudaGetLastError() == cudaSuccess ? 0 : -1;
+}
+
+// Partial row-wise Adam of a data-parallel table: table and m [rows, pitch] fp32, v [rows] fp32, wgrad the
+// all-reduced dense gradient [rows, pitch] (zeroed on return; all-zero rows are skipped)
+extern "C" int hctr_emb_dp_prow_adam_update(float* table, float* m, float* v, float* wgrad, long long rows,
+                                            int pitch, const OptHyper* hp, int num_sms, void* stream_) {
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+  if (rows <= 0) return 0;
+  long long blocks = (rows * 32 + 255) / 256;
+  if (blocks > num_sms * 8ll) blocks = num_sms * 8ll;
+  emb_dp_prow_adam_update_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(table, m, v, wgrad, rows,
+                                                                                pitch, *hp);
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }
 

@@ -274,7 +274,9 @@ inline void with_weighted(const EmbParams& p, Fn&& fn) {
 // The sparse optimizers: calls fn(Int<OPT>, Tag<StateT>, Tag<WT>) for optimizer `opt`, state type (bf16
 // when state_bf16) and weight type (bf16 when table_bf16).  SGD (no state) and row-wise AdaGrad (a
 // [rows] fp32 accumulator, never bf16: a value that only grows would drop small increments) run with the
-// fp32 state type.  Returns 0, -2 for an unknown optimizer, or -7 for row-wise AdaGrad with bf16 state.
+// fp32 state type.  Partial row-wise Adam's StateT is the type of its first moment s0; its second moment
+// s1 is one fp32 value per row whatever StateT is (the kernels read it through row_state).  Returns 0, -2
+// for an unknown optimizer, or -7 for row-wise AdaGrad with bf16 state.
 template <typename Fn>
 inline int dispatch_opt(int opt, int state_bf16, int table_bf16, Fn&& fn) {
   auto run = [&](auto o) {
@@ -295,6 +297,7 @@ inline int dispatch_opt(int opt, int state_bf16, int table_bf16, Fn&& fn) {
     case OPT_NESTEROV: run(Int<OPT_NESTEROV>{}); break;
     case OPT_RMSPROP: run(Int<OPT_RMSPROP>{}); break;
     case OPT_ROWWISE_ADAGRAD: run(Int<OPT_ROWWISE_ADAGRAD>{}); break;
+    case OPT_PARTIAL_ROWWISE_ADAM: run(Int<OPT_PARTIAL_ROWWISE_ADAM>{}); break;
     default: return -2;
   }
   return 0;

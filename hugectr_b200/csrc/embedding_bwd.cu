@@ -546,14 +546,16 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
       load_a(i + groups, 1, 1);
       const unsigned int uid = rec[0].x;
       const long long base = static_cast<long long>(row[0]) * ev;
-      if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
-        // Row-wise AdaGrad needs the whole row's sum of g^2 before any of its weights is stored.
-        // The gradient sums of all NC chunks stay in registers (they take the place of the
-        // per-element state vectors of the other optimizers), so a row is gathered exactly once
-        // even when it spans two passes (G == 32, ev > 512).  The weights of the first four
-        // chunks and the row's accumulator (one 4-byte load by the group's first lane) are
-        // requested with the gradients; a second pass loads its weights once the factor is known.
+      if constexpr (kRowRule<OPT>) {
+        // The row-reduced rules (row-wise AdaGrad, partial row-wise Adam) need the whole row's sum of
+        // g^2 before any of its weights is stored.  The gradient sums of all NC chunks stay in
+        // registers (they take the place of the per-element state vectors of the other optimizers),
+        // so a row is gathered exactly once even when it spans two passes (G == 32, ev > 512).  The
+        // weights of the first four chunks and the row's state (one 4-byte load by the group's first
+        // lane) are requested with the gradients; a second pass loads its weights, and partial
+        // row-wise Adam its first moments, once the factor is known.
         const unsigned int gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (gi * G));
+        float* const rs = row_state<OPT>(s0, s1);
         typename Row4<WT>::type wv[4];
         float4 acc[NC];
 #pragma unroll
@@ -562,7 +564,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
           wv[c] = {};
           if (col < ev) wv[c] = load_row4<WT>(static_cast<const WT*>(p.table) + base + col);
         }
-        const float s_old = gl == 0 ? s0[row[0]] : 0.f;
+        const float s_old = gl == 0 ? rs[row[0]] : 0.f;
         float sq = 0.f;
 #pragma unroll
         for (int c = 0; c < NC; ++c) {
@@ -574,7 +576,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
             sq += sumsq4(acc[c]);
           }
         }
-        const float f = rowwise_row_step<G>(gmask, gi * G, lane, sq, s_old, s0 + row[0], ev, hp, step.lr);
+        const float f = row_reduce_step<OPT, G>(gmask, gi * G, lane, sq, s_old, rs + row[0], ev, hp, step);
 #pragma unroll
         for (int c = 0; c < NC; ++c) {
           const int col = (c * G + gl) * 4;
@@ -582,7 +584,7 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
             float4 w;
             if (c < 4) w = widen4(wv[c & 3]);
             else w = load_vec4<WT>(static_cast<const WT*>(p.table) + base + col);
-            apply_rowwise4(w, acc[c], f);
+            row_apply4<OPT, StateT>(w, acc[c], f, s0, base + col, hp);
             store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
           }
         }
@@ -637,11 +639,12 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
     const unsigned int uid = r.x, o0 = r.y;
     const unsigned int o1 = ix.offsets[uid + 1];
     const long long base = static_cast<long long>(ut.rows[uid]) * ev;
-    if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
+    if constexpr (kRowRule<OPT>) {
       // as the light rows: the sums of all (up to 8) column iterations stay in registers until the
       // row's sum of g^2 is known, then every column takes the row's factor
       const unsigned long long arow = ut.rows[uid];
-      const float s_old = lane == 0 ? s0[arow] : 0.f;
+      float* const rs = row_state<OPT>(s0, s1);
+      const float s_old = lane == 0 ? rs[arow] : 0.f;
       constexpr int kIters = (G == 8) ? 1 : kMaxEmbWidth / 128;   // G == 8 launches have ev <= 128
       float4 acc[kIters];
       float sq = 0.f;
@@ -654,13 +657,13 @@ __global__ void __launch_bounds__(256, (G == 8) ? 3 : 2)
           sq += sumsq4(acc[c]);
         }
       }
-      const float f = rowwise_row_step<32>(0xffffffffu, 0, lane, sq, s_old, s0 + arow, ev, hp, step.lr);
+      const float f = row_reduce_step<OPT, 32>(0xffffffffu, 0, lane, sq, s_old, rs + arow, ev, hp, step);
 #pragma unroll
       for (int c = 0; c < kIters; ++c) {
         const int col = lane * 4 + c * 128;
         if (col < ev) {
           float4 w = load_vec4<WT>(static_cast<const WT*>(p.table) + base + col);
-          apply_rowwise4(w, acc[c], f);
+          row_apply4<OPT, StateT>(w, acc[c], f, s0, base + col, hp);
           store_w4<WT>(static_cast<WT*>(p.table) + base + col, w, srk, base + col);
         }
       }
@@ -723,9 +726,9 @@ __global__ void __launch_bounds__(256)
       const unsigned long long row = ut.rows[uid];
       const long long base = static_cast<long long>(row) * ev;
       const unsigned long long srk = sr_key<WT>(hp.sr_seed, hp.step_ptr);
-      if constexpr (OPT == OPT_ROWWISE_ADAGRAD) {
-        // the block reduces the row's sum of g^2 over the scratch row, thread 0 updates the
-        // accumulator once, then every column is applied; scratch is zeroed only by this second read
+      if constexpr (kRowRule<OPT>) {
+        // the block reduces the row's sum of g^2 over the scratch row, thread 0 updates the row
+        // state once, then every column is applied; scratch is zeroed only by this second read
         __shared__ float sq_s[8];
         __shared__ float f_s;
         float sq = 0.f;
@@ -741,7 +744,8 @@ __global__ void __launch_bounds__(256)
           float t = 0.f;
 #pragma unroll
           for (int w = 0; w < 8; ++w) t += sq_s[w];
-          f_s = rowwise_state_step(s0[row], t, s0 + row, ev, hp, step.lr);
+          float* const rs = row_state<OPT>(s0, s1);
+          f_s = row_state_step<OPT>(rs[row], t, rs + row, ev, hp, step);
         }
         __syncthreads();
         const float f = f_s;
@@ -749,7 +753,7 @@ __global__ void __launch_bounds__(256)
           const float g = __ldcg(scratch + c) * inv_scaler;
           scratch[c] = 0.f;
           float w = to_f<WT>(static_cast<const WT*>(p.table)[base + c]);
-          w -= f * g;
+          row_apply1<OPT, StateT>(w, g, f, s0, base + c, hp);
           store_w<WT>(static_cast<WT*>(p.table) + base + c, w, srk, base + c);
         }
       } else

@@ -212,11 +212,12 @@ struct EvictReinit {
   const int* adm_n;
   void* table;            // arena (fp32 or bf16), row pitch `pitch`
   void* s0;               // optional, pitch s0_pitch (1: row-wise)
-  void* s1;               // optional, pitch `pitch`
+  void* s1;               // optional, pitch `pitch` (s1_row: fp32, one value per row)
   long long row_off;      // first arena row of the shard
   unsigned long long init_key;
   float bound, s0_init;
   int pitch, col0, s0_pitch, state_bf16;
+  int s1_row;             // 1: s1 is fp32 with one value per row (partial row-wise Adam's second moment)
 };
 
 HCTR_DEVICE void store_state(void* p, long long i, float v, int bf16) {
@@ -226,7 +227,8 @@ HCTR_DEVICE void store_state(void* p, long long i, float v, int bf16) {
     static_cast<float*>(p)[i] = v;
 }
 
-template <typename WT>
+// S1_ROW: p.s1_row is set (the other instantiations are those of the optimizers with per-element states)
+template <typename WT, bool S1_ROW>
 __global__ void __launch_bounds__(256) evict_reinit_kernel(EvictReinit p) {
   const int lane = threadIdx.x & 31;
   const int n = *p.adm_n;
@@ -242,10 +244,13 @@ __global__ void __launch_bounds__(256) evict_reinit_kernel(EvictReinit p) {
         w[c] = __float2bfloat16_rn(v);
       else
         w[c] = v;
-      if (p.s1) store_state(p.s1, row * p.pitch + c, 0.0f, p.state_bf16);
+      if constexpr (!S1_ROW)
+        if (p.s1) store_state(p.s1, row * p.pitch + c, 0.0f, p.state_bf16);
     }
     if (p.s0)
       for (int c = lane; c < p.s0_pitch; c += 32) store_state(p.s0, row * p.s0_pitch + c, p.s0_init, p.state_bf16);
+    if constexpr (S1_ROW)
+      if (lane == 0) static_cast<float*>(p.s1)[row] = 0.0f;
   }
 }
 
@@ -323,9 +328,15 @@ extern "C" int hctr_evict_reinit(const EvictReinit* p, long long max_adm, int ta
   if (max_adm <= 0) return 0;
   const long long warps = max_adm < 8192 ? max_adm : 8192;
   const unsigned grid = static_cast<unsigned>((warps * 32 + 255) / 256);
-  if (table_bf16)
-    evict_reinit_kernel<__nv_bfloat16><<<grid, 256, 0, (cudaStream_t)stream>>>(*p);
+  auto launch = [&](auto s1_row) {
+    if (table_bf16)
+      evict_reinit_kernel<__nv_bfloat16, decltype(s1_row)::value><<<grid, 256, 0, (cudaStream_t)stream>>>(*p);
+    else
+      evict_reinit_kernel<float, decltype(s1_row)::value><<<grid, 256, 0, (cudaStream_t)stream>>>(*p);
+  };
+  if (p->s1_row && p->s1)
+    launch(std::true_type{});
   else
-    evict_reinit_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>(*p);
+    launch(std::false_type{});
   return cudaGetLastError() == cudaSuccess ? 0 : -1;
 }

@@ -46,7 +46,7 @@ HCTR_DEVICE __nv_bfloat16 from_f<__nv_bfloat16>(float v) { return __float2bfloat
 
 // ------------------------------------------------------------------ optimizer rules
 enum SparseOpt : int { OPT_SGD = 0, OPT_ADAGRAD, OPT_ADAM, OPT_FTRL, OPT_MOMENTUM, OPT_NESTEROV,
-                       OPT_RMSPROP, OPT_ROWWISE_ADAGRAD };
+                       OPT_RMSPROP, OPT_ROWWISE_ADAGRAD, OPT_PARTIAL_ROWWISE_ADAM };
 
 struct OptHyper {
   const float* lr_ptr;    // device learning rate (graph friendly)
@@ -69,7 +69,7 @@ struct OptStep {
 template <int OPT>
 HCTR_DEVICE OptStep opt_step(const OptHyper& hp) {
   OptStep st = {(hp.lr_ptr ? *hp.lr_ptr : 1.f) * hp.lr_scale, 1.f, 1.f};
-  if constexpr (OPT == OPT_ADAM) {
+  if constexpr (OPT == OPT_ADAM || OPT == OPT_PARTIAL_ROWWISE_ADAM) {
     const float t = static_cast<float>(hp.step_ptr ? *hp.step_ptr : 1u);
     st.bc1 = 1.f - powf(hp.beta1, t);
     st.bc2 = 1.f - powf(hp.beta2, t);
@@ -178,7 +178,7 @@ HCTR_DEVICE void apply_opt4_pre(float4& w, const float4 g, const float4 s0v, Sta
 
 // Row-wise AdaGrad (OPT_ROWWISE_ADAGRAD): ONE fp32 accumulator per row, s[row] (never bf16).
 //   s += (1/ev) * sum_c g[c]^2 ;  w[c] -= lr * g[c] / (sqrt(s) + eps)  for every column of the row
-// The caller reduces sum_c g[c]^2 over the whole row first (rowwise_row_step over the row's lanes, or
+// The caller reduces sum_c g[c]^2 over the whole row first (row_reduce_step over the row's lanes, or
 // its own block reduction followed by rowwise_state_step), and applies the returned factor
 // f = lr / (sqrt(s) + eps) to every column.  Square root and divisions round to nearest even whatever the fast-math flags, so a row
 // whose update is exact in fp32 is reproduced bit for bit by the CPU path (ops/optim.py).
@@ -194,22 +194,82 @@ HCTR_DEVICE float rowwise_state_step(float s_old, float sumsq, float* s, int ev,
   *s = s_new;
   return rowwise_factor(s_new, hp, lr);
 }
-// The WIDTH lanes of `mask` (a power of two, aligned) own one row and hold partial sums of g^2 in sq;
-// lane `leader`, the first of them, has s_old = *s (loaded early by the caller) and updates *s.  Every
-// lane returns the row's factor.
-template <int WIDTH>
-HCTR_DEVICE float rowwise_row_step(unsigned int mask, int leader, int lane, float sq, float s_old, float* s,
-                                   int ev, const OptHyper& hp, float lr) {
-#pragma unroll
-  for (int o = WIDTH / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(mask, sq, o);
-  float f = 0.f;
-  if (lane == leader) f = rowwise_state_step(s_old, sq, s, ev, hp, lr);
-  return __shfl_sync(mask, f, leader);
-}
 HCTR_DEVICE void apply_rowwise4(float4& w, const float4 g, float f) {
   w.x -= f * g.x; w.y -= f * g.y; w.z -= f * g.z; w.w -= f * g.w;
 }
 HCTR_DEVICE float sumsq4(const float4 g) { return g.x * g.x + g.y * g.y + g.z * g.z + g.w * g.w; }
 HCTR_DEVICE float4 scale4(const float4 g, float a) { return make_float4(g.x * a, g.y * a, g.z * a, g.w * a); }
+
+// Partial row-wise Adam (OPT_PARTIAL_ROWWISE_ADAM): the first moment m per element (state 0, StateT) and
+// the second moment ONE fp32 value per row, v[row] (state 1, never bf16: an EMA of a small quantity would
+// lose its increments).  For a row that receives gradients, t = the device step counter:
+//   m[c] = b1 m[c] + (1 - b1) g[c] ;  v = b2 v + (1 - b2) (1/ev) sum_c g[c]^2
+//   w[c] -= alpha m[c] / (sqrt(v) + eps),  alpha = lr sqrt(1 - b2^t) / (1 - b1^t)
+// with Adam's bias correction and epsilon placement (apply_opt<OPT_ADAM>).  As for row-wise AdaGrad the
+// caller reduces sum_c g[c]^2 over the whole row before it stores any weight or m of the row; the row step
+// updates v once and returns the row's factor f = alpha / (sqrt(v) + eps), and the element step updates m
+// and applies w -= f m.
+HCTR_DEVICE float prow_adam_state_step(float v_old, float sumsq, float* v, int ev, const OptHyper& hp,
+                                       const OptStep& st) {
+  const float v_new = hp.beta2 * v_old + (1.f - hp.beta2) * __fdiv_rn(sumsq, static_cast<float>(ev));
+  *v = v_new;
+  const float alpha = st.lr * sqrtf(st.bc2) / st.bc1;   // as apply_opt<OPT_ADAM>
+  return __fdiv_rn(alpha, __fsqrt_rn(v_new) + hp.epsilon);
+}
+template <typename StateT>
+HCTR_DEVICE void prow_adam_step4(float4& w, const float4 g, StateT* m, const OptHyper& hp, float f) {
+  float4 a = load_vec4<StateT>(m);
+  const float c = 1.f - hp.beta1;
+  a.x = hp.beta1 * a.x + c * g.x; a.y = hp.beta1 * a.y + c * g.y;
+  a.z = hp.beta1 * a.z + c * g.z; a.w = hp.beta1 * a.w + c * g.w;
+  store_vec4<StateT>(m, a.x, a.y, a.z, a.w);
+  w.x -= f * a.x; w.y -= f * a.y; w.z -= f * a.z; w.w -= f * a.w;
+}
+template <typename StateT>
+HCTR_DEVICE void prow_adam_step1(float& w, float g, StateT* m, const OptHyper& hp, float f) {
+  const float a = hp.beta1 * to_f<StateT>(*m) + (1.f - hp.beta1) * g;
+  *m = from_f<StateT>(a);
+  w -= f * a;
+}
+
+// The two row-reduced rules behind one interface, for the kernels that hold a whole row's sum of g^2
+// before they store any of it: the fp32 row state (row-wise AdaGrad: s0 [rows]; partial row-wise Adam:
+// s1 [rows], whatever StateT is), the row step of one thread (row_state_step) or of the lanes that own
+// the row (row_reduce_step), and the element steps (row_apply4 / row_apply1) on the gradient g of arena
+// element idx with the row's factor f.
+template <int OPT>
+constexpr bool kRowRule = (OPT == OPT_ROWWISE_ADAGRAD || OPT == OPT_PARTIAL_ROWWISE_ADAM);
+template <int OPT, typename StateT>
+HCTR_DEVICE float* row_state(StateT* s0, StateT* s1) {
+  if constexpr (OPT == OPT_ROWWISE_ADAGRAD) return reinterpret_cast<float*>(s0);
+  else return reinterpret_cast<float*>(s1);
+}
+template <int OPT>
+HCTR_DEVICE float row_state_step(float s_old, float sumsq, float* s, int ev, const OptHyper& hp, const OptStep& st) {
+  if constexpr (OPT == OPT_ROWWISE_ADAGRAD) return rowwise_state_step(s_old, sumsq, s, ev, hp, st.lr);
+  else return prow_adam_state_step(s_old, sumsq, s, ev, hp, st);
+}
+// The WIDTH lanes of `mask` (a power of two, aligned) own one row and hold partial sums of g^2 in sq;
+// lane `leader`, the first of them, has s_old = *s (loaded early by the caller) and updates *s.  Every
+// lane returns the row's factor.
+template <int OPT, int WIDTH>
+HCTR_DEVICE float row_reduce_step(unsigned int mask, int leader, int lane, float sq, float s_old, float* s,
+                                  int ev, const OptHyper& hp, const OptStep& st) {
+#pragma unroll
+  for (int o = WIDTH / 2; o > 0; o >>= 1) sq += __shfl_xor_sync(mask, sq, o);
+  float f = 0.f;
+  if (lane == leader) f = row_state_step<OPT>(s_old, sq, s, ev, hp, st);
+  return __shfl_sync(mask, f, leader);
+}
+template <int OPT, typename StateT>
+HCTR_DEVICE void row_apply4(float4& w, const float4 g, float f, StateT* s0, long long idx, const OptHyper& hp) {
+  if constexpr (OPT == OPT_ROWWISE_ADAGRAD) apply_rowwise4(w, g, f);
+  else prow_adam_step4<StateT>(w, g, s0 + idx, hp, f);
+}
+template <int OPT, typename StateT>
+HCTR_DEVICE void row_apply1(float& w, float g, float f, StateT* s0, long long idx, const OptHyper& hp) {
+  if constexpr (OPT == OPT_ROWWISE_ADAGRAD) w -= f * g;
+  else prow_adam_step1<StateT>(w, g, s0 + idx, hp, f);
+}
 
 }  // namespace hctr

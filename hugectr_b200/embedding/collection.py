@@ -237,11 +237,14 @@ def shard_rows(vocab: int, k: int, s: int) -> int:
 class _Group:
     """Local tables of one (kind, ev pitch, weight dtype) group: one arena + optimizer state.
     Row-wise AdaGrad tables form groups of their own, keyed also by their epsilon and initial value,
-    whose state ``s0`` holds one fp32 accumulator per arena row."""
+    whose state ``s0`` holds one fp32 accumulator per arena row.  So do partial row-wise Adam tables
+    (``prow_adam``), keyed also by their betas and epsilon: ``s0`` is the per-weight first moment in the
+    state dtype and ``s1`` one fp32 second moment per arena row."""
 
-    def __init__(self, kind, pitch, wdtype="fp32", rowwise=False):
+    def __init__(self, kind, pitch, wdtype="fp32", rowwise=False, prow_adam=False):
         self.kind, self.pitch, self.wdtype = kind, pitch, wdtype
         self.rowwise = rowwise
+        self.prow_adam = prow_adam
         self.exps = None         # fp8 arena: uint8 [rows], e + 127 of each row's scale 2^e
         self.stamp = None        # int32 [rows]: clock of the last write of each row (groups with a tracked table)
         self.rows = 0
@@ -250,9 +253,10 @@ class _Group:
         self.opt: Optional[OptParamsPy] = None
 
     @property
-    def state_pitch(self) -> int:
-        """state values per arena row: the pitch, or 1 for row-wise AdaGrad"""
-        return 1 if self.rowwise else self.pitch
+    def state_pitches(self):
+        """values per arena row of s0 and s1: the pitch, or 1 for a row state (row-wise AdaGrad's s0,
+        partial row-wise Adam's s1)"""
+        return (1 if self.rowwise else self.pitch, 1 if self.prow_adam else self.pitch)
 
 
 @dataclass
@@ -531,6 +535,7 @@ class EmbeddingCollection:
                         parts.append((idx // kk, kk, idx % kk))   # (col part, num row shards, shard)
             o = t.opt_params or self.default_opt
             rowwise = o is not None and o.optimizer_type == Optimizer_t.RowWiseAdaGrad
+            prow_adam = o is not None and o.optimizer_type == Optimizer_t.PartialRowWiseAdam
             for (cpart, k, s) in parts:
                 # (a serving collection takes no gradient: its data-parallel tables may be fp8 too)
                 wdt = "fp8" if self.fp8_quant else (wdtype[t.name] if pl.kind == "mp" else "fp32")
@@ -538,7 +543,9 @@ class EmbeddingCollection:
                 if rowwise:
                     # never shares an arena (and its first table's optimizer) with another optimizer
                     key += ("rowwise", float(o.epsilon), float(o.initial_accu_value))
-                grp = groups.setdefault(key, _Group(pl.kind, ev_part, wdt, rowwise))
+                if prow_adam:
+                    key += ("partial_rowwise_adam", float(o.beta1), float(o.beta2), float(o.epsilon))
+                grp = groups.setdefault(key, _Group(pl.kind, ev_part, wdt, rowwise, prow_adam))
                 if t.evict_strategy is not None:
                     rows = (t.max_capacity + 31) // 32 * 32       # whole 32-way sets, allocated once
                 else:
@@ -595,8 +602,8 @@ class EmbeddingCollection:
         gen = torch.Generator(device="cpu")
         if share_from is not None:
             for grp, src in zip(self.groups, share_from.groups):
-                assert (grp.kind, grp.pitch, grp.wdtype, grp.rowwise, len(grp.table_slices)) == \
-                    (src.kind, src.pitch, src.wdtype, src.rowwise, len(src.table_slices))
+                assert (grp.kind, grp.pitch, grp.wdtype, grp.rowwise, grp.prow_adam, len(grp.table_slices)) == \
+                    (src.kind, src.pitch, src.wdtype, src.rowwise, src.prow_adam, len(src.table_slices))
                 grp.opt = src.opt
                 grp.ws = None
             self._resync_storage(share_from)     # arrays + row windows (dynamic shards may have grown since)
@@ -618,6 +625,10 @@ class EmbeddingCollection:
                 # would drop small increments)
                 grp.s0 = torch.full((max(grp.rows, 1),), float(grp.opt.initial_accu_value),
                                     dtype=torch.float32, device=dev)
+            if grp.prow_adam and self.is_train:
+                # the second moment: one fp32 value per row, whatever the state dtype (a bf16 EMA of a
+                # small quantity would lose its increments)
+                grp.s1 = torch.zeros(max(grp.rows, 1), dtype=torch.float32, device=dev)
             R = self.world if grp.kind == "mp" else 1
             po = 0
             for l in grp.lookups:
@@ -1032,8 +1043,8 @@ class EmbeddingCollection:
         o = grp.opt
         s0_init = o.initial_accu_value if (o is not None and o.optimizer_type in
                                            (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad)) else 0.0
-        ht.reinit(adm, adm[0].numel(), grp.table, grp.s0, grp.s1, sl["row_off"], grp.pitch, grp.state_pitch,
-                  s0_init, bound, self.evict_init_key(t.name), sl["col0"])
+        ht.reinit(adm, adm[0].numel(), grp.table, grp.s0, grp.s1, sl["row_off"], grp.pitch, grp.state_pitches[0],
+                  s0_init, bound, self.evict_init_key(t.name), sl["col0"], s1_row=grp.prow_adam)
 
     def evict_init_key(self, name: str) -> int:
         """key of the stateless initializer of table ``name``'s admitted rows (ops.evict_init_rows)"""
@@ -1215,8 +1226,8 @@ class EmbeddingCollection:
         grp.exps = relayout(grp.exps, lambda v: None, 1)
         accu = grp.opt.initial_accu_value if (grp.opt is not None and grp.opt.optimizer_type in
                                               (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad)) else 0.0
-        s0 = relayout(grp.s0, lambda v: v.fill_(accu), grp.state_pitch)
-        s1 = relayout(grp.s1, lambda v: v.zero_())
+        s0 = relayout(grp.s0, lambda v: v.fill_(accu), grp.state_pitches[0])
+        s1 = relayout(grp.s1, lambda v: v.zero_(), grp.state_pitches[1])
         grp.stamp = relayout(grp.stamp, lambda v: v.zero_(), 1)     # a new row has no key: never written
         grp.table, grp.s0, grp.s1 = table, s0, s1
         old_end = sl["row_off"] + sl["rows"]
@@ -1427,6 +1438,10 @@ class EmbeddingCollection:
             if grp.rowwise:
                 E.dp_rowwise_update(grp.table, grp.s0, grp.dense_wgrad, grp.pitch, self._hp(o), lr_t)
                 return
+            if grp.prow_adam:
+                E.dp_prow_adam_update(grp.table, grp.s0, grp.s1, grp.dense_wgrad, grp.pitch, self._hp(o), lr_t,
+                                      step_t)
+                return
             D.dense_opt_step(o.optimizer_type, grp.table, grp.dense_wgrad, None, grp.s0, grp.s1, lr_t,
                              step_t, self._hp(o), zero_grad=True)
 
@@ -1484,14 +1499,14 @@ class EmbeddingCollection:
                 grp.table.view(-1, grp.pitch)[rows] = values[m][:, c0:c0 + ev].to(grp.table.device,
                                                                                  torch.float32).to(grp.table.dtype)
                 if state is not None:
-                    for st, dst in zip(state, (grp.s0, grp.s1)):
+                    for st, dst, sp in zip(state, (grp.s0, grp.s1), grp.state_pitches):
                         if dst is not None and st is not None:
                             v = st[m][:, c0:c0 + ev]
-                            if grp.rowwise:
-                                # a row's accumulator: the mean of the state over the slice's columns
-                                # (exact for a row-wise file, the natural conversion of an AdaGrad one)
+                            if sp == 1:
+                                # a row state: the mean of the state over the slice's columns (exact for a
+                                # file of the row-wise rule, the natural conversion of an element-wise one)
                                 v = v.double().mean(1, keepdim=True).float()
-                            dst.view(-1, grp.state_pitch)[rows] = v.to(dst.device, dst.dtype)
+                            dst.view(-1, sp)[rows] = v.to(dst.device, dst.dtype)
 
     def _evict_admit(self, grp, sl, keys):
         """(checkpoint load) local rows of ``keys`` in an evicting shard: present keys keep theirs, the
@@ -1544,8 +1559,8 @@ class EmbeddingCollection:
                 lo, hi = sl["row_off"], sl["row_off"] + sl["rows"]
                 w = _rows_fp32(grp, lo, hi).detach().cpu()
                 keys = torch.arange(sl["rows"], dtype=torch.int64) * sl["k"] + sl["s"]
-                sts = [None if t is None else t.view(-1, grp.state_pitch)[lo:hi].detach().float().cpu()
-                       .expand(hi - lo, grp.pitch).contiguous() for t in (grp.s0, grp.s1)]
+                sts = [None if t is None else t.view(-1, sp)[lo:hi].detach().float().cpu()
+                       .expand(hi - lo, grp.pitch).contiguous() for t, sp in zip((grp.s0, grp.s1), grp.state_pitches)]
                 if sl.get("dynamic"):
                     dk, dr = self._dyn_hash(name, dict(sl, cpart=0)).dump()
                     order = torch.argsort(dk)

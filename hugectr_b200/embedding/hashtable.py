@@ -242,7 +242,7 @@ class _EvictReinit(C.Structure):
     _fields_ = [("keys", C.c_void_p), ("adm", C.c_void_p), ("adm_n", C.c_void_p), ("table", C.c_void_p),
                 ("s0", C.c_void_p), ("s1", C.c_void_p), ("row_off", C.c_longlong), ("init_key", C.c_ulonglong),
                 ("bound", C.c_float), ("s0_init", C.c_float), ("pitch", C.c_int), ("col0", C.c_int),
-                ("s0_pitch", C.c_int), ("state_bf16", C.c_int)]
+                ("s0_pitch", C.c_int), ("state_bf16", C.c_int), ("s1_row", C.c_int)]
 
 
 def evict_set_of(keys, num_sets: int):
@@ -415,14 +415,17 @@ class SetAssocTable:
         region.copy_(out.to(region.dtype))
 
     def reinit(self, adm, max_adm: int, table, s0, s1, row_off: int, pitch: int, s0_pitch: int, s0_init: float,
-               bound: float, init_key: int, col0: int = 0):
-        """fresh weights (ops.evict_init_rows) and initial optimizer state for the admitted ways"""
+               bound: float, init_key: int, col0: int = 0, s1_row: bool = False):
+        """fresh weights (ops.evict_init_rows) and initial optimizer state for the admitted ways; ``s1_row``:
+        ``s1`` holds one fp32 value per row (partial row-wise Adam), otherwise it has the row pitch and the
+        dtype of ``s0``"""
+        s1_row = bool(s1_row) and s1 is not None
         if self.device.type == "cuda":
             sbf = int(any(s is not None and s.dtype == torch.bfloat16 for s in (s0, s1)))
             p = _EvictReinit(self.keys.data_ptr(), adm[0].data_ptr(), adm[1].data_ptr(), table.data_ptr(),
                              None if s0 is None else s0.data_ptr(), None if s1 is None else s1.data_ptr(),
                              int(row_off), int(init_key) & ((1 << 64) - 1), float(bound), float(s0_init),
-                             int(pitch), int(col0), int(s0_pitch), sbf)
+                             int(pitch), int(col0), int(s0_pitch), sbf, int(s1_row))
             from .ops import table_type
             self._call("hctr_evict_reinit", C.byref(p), int(max_adm), table_type(table), self._st())
             return
@@ -435,7 +438,7 @@ class SetAssocTable:
         if s0 is not None:
             s0.view(-1, s0_pitch)[rows] = s0_init
         if s1 is not None:
-            s1.view(-1, pitch)[rows] = 0
+            s1.view(-1, 1 if s1_row else pitch)[rows] = 0
 
     # ---- whole-table views (host synchronisation: outside the step)
     def dump(self):

@@ -76,11 +76,12 @@ def lib():
                                                  C.POINTER(CBwdIndex), vp, vp, i, i,
                                                  C.POINTER(COptHyper), f, i, vp, i, i, vp]
         l.hctr_emb_dp_rowwise_update.argtypes = [vp, vp, vp, ll, i, C.POINTER(COptHyper), i, vp]
+        l.hctr_emb_dp_prow_adam_update.argtypes = [vp, vp, vp, vp, ll, i, C.POINTER(COptHyper), i, vp]
         l.hctr_emb_quantize_rows.argtypes = [vp, vp, ll, i, vp, vp, vp, vp]
         l.hctr_emb_stamp_rows.argtypes = [vp, vp, vp, C.c_uint, ll, vp, i, vp]
         for n in ("hctr_emb_forward", "hctr_emb_backward_accum", "hctr_emb_update",
                   "hctr_emb_gather_rows", "hctr_emb_bwd_index", "hctr_emb_bwd_reduce_update",
-                  "hctr_emb_dp_rowwise_update", "hctr_emb_quantize_rows", "hctr_emb_stamp_rows"):
+                  "hctr_emb_dp_rowwise_update", "hctr_emb_dp_prow_adam_update", "hctr_emb_quantize_rows", "hctr_emb_stamp_rows"):
             getattr(l, n).restype = i
         # ABI self-check: ctypes mirrors vs the structs the kernels were compiled with
         if hasattr(l, "hctr_abi_sizes_emb"):
@@ -659,30 +660,39 @@ def update_rows(opt: Optimizer_t, table, s0, s1, ev_pitch, rows, grads, hp: dict
     """One optimizer application per DISTINCT row (``rows`` [n] may repeat, ``grads`` [n, pitch] fp32 are
     summed per row first).  Plain tensor ops on the tables' device: the CPU path of ``update`` and the
     owner side of the Unique-compression exchange (embedding/unique_exchange.py).  A bf16 table is
-    updated in fp32 and stored with the kernels' stochastic rounding (sr_round_bf16)."""
+    updated in fp32 and stored with the kernels' stochastic rounding (sr_round_bf16).  Row-wise AdaGrad's
+    s0 and partial row-wise Adam's s1 hold one fp32 value per row (state_pitches)."""
     if rows.numel() == 0:
         return
     uniq, inv = torch.unique(rows, return_inverse=True)
     g = torch.zeros(uniq.numel(), ev_pitch, dtype=torch.float32, device=grads.device).index_add_(0, inv, grads.float())
     tab = table.view(-1, ev_pitch)
     w = tab[uniq].float().clone()
-    # row-wise state: s0 [rows], one accumulator per row
-    rowwise = opt == Optimizer_t.RowWiseAdaGrad
-    spitch = 1 if rowwise else ev_pitch
-    a = None if s0 is None else s0.view(-1, spitch)[uniq].float().clone()
-    b = None if s1 is None else s1.view(-1, ev_pitch)[uniq].float().clone()
-    if rowwise and a is not None:
-        a = a.view(-1)
+    pitches = state_pitches(opt, ev_pitch)
+    rs = ROW_STATE.get(opt)
+    # the rule takes a row state as [n], a per-element one as [n, ev]
+    a, b = [None if s is None else (s[uniq] if i == rs else s.view(-1, ev_pitch)[uniq]).float().clone()
+            for i, s in enumerate((s0, s1))]
     step = int(step_t.item())
     sparse_opt_reference(opt, w, a, b, g, hp, float(lr_t.item()), step)
     if table_type(table) == BF16:
         idx = uniq.view(-1, 1) * ev_pitch + torch.arange(ev_pitch, device=uniq.device).view(1, -1)
         w = sr_round_bf16(w, sr_seed(hp), step, idx)
     tab[uniq] = w
-    if a is not None:
-        s0.view(-1, spitch)[uniq] = a.view(-1, spitch).to(s0.dtype)
-    if b is not None:
-        s1.view(-1, ev_pitch)[uniq] = b.to(s1.dtype)
+    for s, v, p in zip((s0, s1), (a, b), pitches):
+        if v is not None:
+            s.view(-1, p)[uniq] = v.view(-1, p).to(s.dtype)
+
+
+# the state that holds one fp32 value per row: row-wise AdaGrad's accumulator s0, partial row-wise Adam's
+# second moment s1
+ROW_STATE = {Optimizer_t.RowWiseAdaGrad: 0, Optimizer_t.PartialRowWiseAdam: 1}
+
+
+def state_pitches(opt: Optimizer_t, ev_pitch: int):
+    """values per arena row of the optimizer's two states: the pitch, or 1 for its row state"""
+    rs = ROW_STATE.get(opt)
+    return tuple(1 if i == rs else ev_pitch for i in (0, 1))
 
 
 def dp_rowwise_update(table, s0, wgrad, pitch, hp: dict, lr_t, num_sms: int = 132):
@@ -704,6 +714,32 @@ def dp_rowwise_update(table, s0, wgrad, pitch, hp: dict, lr_t, num_sms: int = 13
     sparse_opt_reference(Optimizer_t.RowWiseAdaGrad, w, a, None, g.clone(), hp, float(lr_t.item()), 1)
     table.view(rows, pitch).copy_(w)
     s0.copy_(a)
+    wgrad.zero_()
+
+
+def dp_prow_adam_update(table, m, v, wgrad, pitch, hp: dict, lr_t, step_t, num_sms: int = 132):
+    """Partial row-wise Adam of a data-parallel table from its all-reduced dense gradient ``wgrad``
+    ([rows * pitch] fp32, zeroed on return): first moments ``m`` [rows * pitch] fp32, second moments ``v``
+    [rows] fp32.  A row whose gradient is all zero is skipped: weights and both moments keep their values
+    (on a model-parallel table a looked-up row takes the step with g = 0 and its moments decay)."""
+    rows = table.numel() // pitch
+    if table.is_cuda:
+        h = opt_hyper(hp, lr_t, step_t)
+        rc = lib().hctr_emb_dp_prow_adam_update(table.data_ptr(), m.data_ptr(), v.data_ptr(), wgrad.data_ptr(),
+                                                rows, pitch, C.byref(h), num_sms, _st(table.device))
+        if rc:
+            raise RuntimeError(f"hctr_emb_dp_prow_adam_update failed rc={rc}")
+        D._count()
+        return
+    g = wgrad[:rows * pitch].view(rows, pitch)
+    live = (g != 0).any(1).nonzero()[:, 0]
+    if live.numel():
+        w, a, b = table.view(rows, pitch)[live], m.view(rows, pitch)[live], v[live]
+        sparse_opt_reference(Optimizer_t.PartialRowWiseAdam, w, a, b, g[live].clone(), hp, float(lr_t.item()),
+                             int(step_t.item()))
+        table.view(rows, pitch)[live] = w
+        m.view(rows, pitch)[live] = a
+        v[live] = b
     wgrad.zero_()
 
 

@@ -138,6 +138,9 @@ class Optimizer_t(Enum):
     SGD = 6
     # embedding-collection tables only: one fp32 accumulator per row (docs/embedding.md)
     RowWiseAdaGrad = 7
+    # embedding-collection tables only: per-weight first moment, one fp32 second moment per row
+    # (docs/embedding.md)
+    PartialRowWiseAdam = 8
 
 
 class Update_t(Enum):
@@ -233,4 +236,5 @@ OPT_STATES_PER_WEIGHT = {
     Optimizer_t.Nesterov: 1,
     Optimizer_t.SGD: 0,
     Optimizer_t.RowWiseAdaGrad: 0,   # one value per row, not per weight
+    Optimizer_t.PartialRowWiseAdam: 1,   # the first moment; the second is one value per row
 }

@@ -47,12 +47,15 @@ def build_dlrm_dcnv2(batchsize: int = 55296, num_gpus: int = 8, table_sizes: Opt
                      comm=None, comm_strategy=None, compression_strategy=None,
                      embedding_optimizer: str = "adagrad", weight_dtype: str = "fp32",
                      **solver_kw) -> "hugectr.Model":
-    """``embedding_optimizer``: "adagrad" (the model optimizer for every table) or "rowwise_adagrad"
+    """``embedding_optimizer``: "adagrad" (the model optimizer for every table), "rowwise_adagrad"
     (every table gets row-wise AdaGrad with the model optimizer's epsilon and initial value, one fp32
-    accumulator per row; the dense layers keep the model optimizer).  ``weight_dtype``: "fp32" or
-    "bf16" storage of the tables' weights."""
-    if embedding_optimizer not in ("adagrad", "rowwise_adagrad"):
-        raise ValueError(f"embedding_optimizer must be 'adagrad' or 'rowwise_adagrad', not {embedding_optimizer!r}")
+    accumulator per row) or "partial_rowwise_adam" (every table gets partial row-wise Adam with
+    ``CreateOptimizer``'s Adam defaults: a per-weight first moment, one fp32 second moment per row); the
+    dense layers keep the model optimizer.  ``weight_dtype``: "fp32" or "bf16" storage of the tables'
+    weights."""
+    choices = ("adagrad", "rowwise_adagrad", "partial_rowwise_adam")
+    if embedding_optimizer not in choices:
+        raise ValueError(f"embedding_optimizer must be one of {choices}, not {embedding_optimizer!r}")
     table_sizes = list(table_sizes or CRITEO_TB_TABLE_SIZES)
     multi_hot = list(multi_hot or CRITEO_TB_MULTI_HOT)
     n = len(table_sizes)
@@ -79,6 +82,8 @@ def build_dlrm_dcnv2(batchsize: int = 55296, num_gpus: int = 8, table_sizes: Opt
     if embedding_optimizer == "rowwise_adagrad":
         table_opt = hugectr.CreateOptimizer(hugectr.Optimizer_t.RowWiseAdaGrad, hugectr.Update_t.Global,
                                             initial_accu_value=opt.initial_accu_value, epsilon=opt.epsilon)
+    elif embedding_optimizer == "partial_rowwise_adam":
+        table_opt = hugectr.CreateOptimizer(hugectr.Optimizer_t.PartialRowWiseAdam, hugectr.Update_t.Global)
     tables = [hugectr.EmbeddingTableConfig(name=str(i), max_vocabulary_size=table_sizes[i],
                                            ev_size=evs[i], opt_params=table_opt, weight_dtype=weight_dtype)
               for i in range(n)]

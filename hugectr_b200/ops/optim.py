@@ -13,7 +13,7 @@ from ..enums import OPT_STATES_PER_WEIGHT, Optimizer_t
 # SparseOpt in csrc/optim.cuh; the dense optimizer takes the first seven
 OPT_CODE = {Optimizer_t.SGD: 0, Optimizer_t.AdaGrad: 1, Optimizer_t.Adam: 2, Optimizer_t.Ftrl: 3,
             Optimizer_t.MomentumSGD: 4, Optimizer_t.Nesterov: 5, Optimizer_t.RMSProp: 6,
-            Optimizer_t.RowWiseAdaGrad: 7}
+            Optimizer_t.RowWiseAdaGrad: 7, Optimizer_t.PartialRowWiseAdam: 8}
 
 
 class COptHyper(C.Structure):
@@ -62,13 +62,21 @@ def opt_states(o, n: int, dtype=torch.float32, device=None):
 
 def opt_reference(opt: Optimizer_t, w, s0, s1, g, hp, lr, step):
     """fp32 PyTorch form of the update rules of csrc/optim.cuh, in place on ``w`` and the states
-    (same shapes as ``g``; RowWiseAdaGrad: ``g`` [n, ev] and s0 [n], one accumulator per row)."""
+    (same shapes as ``g``; RowWiseAdaGrad: ``g`` [n, ev] and s0 [n], one accumulator per row;
+    PartialRowWiseAdam: ``g`` and s0 = m [n, ev], s1 = v [n], one second moment per row)."""
     g = g / hp.get("scaler", 1.0)
     eps = hp.get("epsilon", 1e-7)
     if opt == Optimizer_t.RowWiseAdaGrad:
         # s += mean_c g^2 ; w -= (lr / (sqrt(s) + eps)) g  -- the factor first, as the kernels do
         s0 += (g * g).sum(1) / g.shape[1]
         w -= (lr / (s0.sqrt() + eps)).unsqueeze(1) * g
+    elif opt == Optimizer_t.PartialRowWiseAdam:
+        # m = b1 m + (1-b1) g ; v = b2 v + (1-b2) mean_c g^2 ; w -= (alpha / (sqrt(v) + eps)) m
+        b1, b2 = hp.get("beta1", 0.9), hp.get("beta2", 0.999)
+        s0.mul_(b1).add_((1 - b1) * g)
+        s1.mul_(b2).add_((1 - b2) * ((g * g).sum(1) / g.shape[1]))
+        alpha = lr * (1 - b2 ** step) ** 0.5 / (1 - b1 ** step)
+        w -= (alpha / (s1.sqrt() + eps)).unsqueeze(1) * s0
     elif opt == Optimizer_t.SGD:
         w -= lr * g
     elif opt == Optimizer_t.AdaGrad:

@@ -121,9 +121,9 @@ class OptParamsPy:
     beta: float = 0.0           # ftrl
     lambda1: float = 0.0        # ftrl
     lambda2: float = 0.0        # ftrl
-    beta1: float = 0.9          # adam
-    beta2: float = 0.999        # adam
-    epsilon: float = 1e-7       # adam / adagrad / row-wise adagrad
+    beta1: float = 0.9          # adam / partial row-wise adam
+    beta2: float = 0.999        # adam / partial row-wise adam
+    epsilon: float = 1e-7       # adam / adagrad / row-wise adagrad / partial row-wise adam
     initial_accu_value: float = 0.0  # adagrad / row-wise adagrad
     momentum_factor: float = 0.0     # momentum sgd / nesterov
     atomic_update: bool = True       # sgd
@@ -139,7 +139,7 @@ class OptParamsPy:
     def to_json(self) -> dict:
         t = self.optimizer_type
         d = {"type": t.name, "update_type": self.update_type.name}
-        if t == Optimizer_t.Adam:
+        if t in (Optimizer_t.Adam, Optimizer_t.PartialRowWiseAdam):
             d["adam_hparam"] = {"beta1": self.beta1, "beta2": self.beta2, "epsilon": self.epsilon}
         elif t in (Optimizer_t.AdaGrad, Optimizer_t.RowWiseAdaGrad):
             d["adagrad_hparam"] = {"initial_accu_value": self.initial_accu_value,
@@ -169,11 +169,12 @@ class OptParamsPy:
 
 
 def check_not_rowwise(opt: Optional[OptParamsPy], where: str) -> None:
-    """Row-wise AdaGrad keeps one accumulator per embedding row: only embedding-collection tables
-    have it.  Raises ValueError for any other user of an optimizer (``where``)."""
+    """Row-wise AdaGrad and partial row-wise Adam keep one state value per embedding row: only
+    embedding-collection tables have them.  Raises ValueError for any other user of an optimizer
+    (``where``)."""
     t = getattr(opt, "optimizer_type", opt)
-    if t == Optimizer_t.RowWiseAdaGrad:
-        raise ValueError(f"Optimizer_t.RowWiseAdaGrad is not supported for {where}; it applies to "
+    if t in (Optimizer_t.RowWiseAdaGrad, Optimizer_t.PartialRowWiseAdam):
+        raise ValueError(f"Optimizer_t.{t.name} is not supported for {where}; it applies to "
                          "embedding-collection tables only: pass it per table with "
                          "EmbeddingTableConfig(opt_params=...)")
 

@@ -108,7 +108,8 @@ def plan_tables(table_sizes: Sequence[int], hotness: Sequence[int], ev_sizes, nu
     of one table when ``num_nodes`` > 1) and that has memory left.
 
     ``state_bytes`` is optimizer state per weight, ``state_row_bytes`` per row and column slice (row-wise
-    AdaGrad: 4, with ``state_bytes=0``); both enter the memory and update terms.
+    AdaGrad: 4, with ``state_bytes=0``; partial row-wise Adam: 4, with ``state_bytes`` 4 or 2 for its fp32 or bf16
+    first moment); both enter the memory and update terms.
 
     Returns (shard_matrix, shard_strategy, report); strategy entries are ``name`` or
     ``(name, column_wise_factor)``."""

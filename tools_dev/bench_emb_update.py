@@ -1,18 +1,21 @@
 """Device time of the model-parallel embedding lookup (forward) and of the fused sparse update (bwd_index +
 bwd_reduce_update) at DLRM-DCNv2 shapes, per optimizer, optimizer-state dtype and weight dtype; and
-(--full-model) the uncapped DLRM-DCNv2 Criteo-TB tables with bf16 weights and row-wise AdaGrad on one GPU.
+(--full-model) the DLRM-DCNv2 Criteo-TB tables with bf16 weights and row-wise AdaGrad (or partial row-wise
+Adam) on one GPU.
 
   python tools_dev/bench_emb_update.py [--opts adagrad,rowwise_adagrad] [--ev 128] [--iters 20] [--rounds 5]
                                        [--max-rows N] [--tree DIR]
   python tools_dev/bench_emb_update.py --check-bits TREE [--keys uniform] [--opts all] [--ev 128] [--steps 3]
-  python tools_dev/bench_emb_update.py --full-model [--steps 20] [--warmup 3]
+  python tools_dev/bench_emb_update.py --full-model [--opts rowwise_adagrad] [--max-rows N] [--steps 20]
+                                       [--warmup 3]
 
 Kernel mode: one arena of the 26 Criteo-TB tables, ev 128 by default (the DLRM-DCNv2 width, which runs the
 G = 8 update kernels; --ev 256 runs the G = 32 ones), batch 6912, the DCNv2 multi-hot sizes, power-law keys
 (alpha 1.1), bf16 activations and gradients.  Rows are capped at --max-rows (default 4 M x 128 / ev, so the
 arena keeps its size, far larger than the 50 MB L2).  --opts takes a comma-separated list of
-sgd, adagrad, adam, ftrl, momentum, nesterov, rmsprop, rowwise_adagrad, or `all`.  Every optimizer with
-per-element state runs with fp32 and with bf16 state; each of these arms runs with fp32 and bf16 weights.
+sgd, adagrad, adam, ftrl, momentum, nesterov, rmsprop, rowwise_adagrad, partial_rowwise_adam, or `all`.
+Every optimizer with per-element state runs with fp32 and with bf16 state (partial row-wise Adam: its first
+moment; the second is one fp32 value per row); each of these arms runs with fp32 and bf16 weights.
 The default is the six arms {AdaGrad fp32 state, AdaGrad bf16 state, RowWiseAdaGrad} x {fp32, bf16 weights}.
 All arms live in one process and are timed alternately with CUDA events after a warm-up; the arms share
 their state buffers, which are zeroed before every timed block.  One JSON line per (weight dtype, forward)
@@ -31,9 +34,11 @@ buckets or the heavy rows' atomics land: every arm must agree bit for bit, and T
 tables whose rows then occur 16 times on average at most (and stops if a row has more than 64 occurrences), so
 that only the light- and medium-row code runs; the default power-law keys add the heavy rows.
 
-Full-model mode: build_dlrm_dcnv2(num_gpus=1, batchsize=6912, embedding_optimizer="rowwise_adagrad",
-weight_dtype="bf16") with the full table sizes, CUDA-graph training steps timed with CUDA events; prints
-the table + state bytes, torch.cuda.max_memory_allocated, the step time and the final loss.
+Full-model mode: build_dlrm_dcnv2(num_gpus=1, batchsize=6912, embedding_optimizer=--opts (rowwise_adagrad
+unless one of rowwise_adagrad / partial_rowwise_adam is given), weight_dtype="bf16") with the full table
+sizes, or each capped at --max-rows (the uncapped tables do not fit one 80 GB card under partial row-wise
+Adam), CUDA-graph training steps timed with CUDA events; prints the row cap, the table + state bytes,
+torch.cuda.max_memory_allocated, the step time and the final loss.
 
 Both modes print the card name and power limit read in the same run.  Without a CUDA device the tool
 exits with an error and measures nothing.
@@ -49,10 +54,13 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BATCH = 6912
-OPTS = ("sgd", "adagrad", "adam", "ftrl", "momentum", "nesterov", "rmsprop", "rowwise_adagrad")
-# per-element state vectors of each optimizer (row-wise AdaGrad: one fp32 value per row instead)
+OPTS = ("sgd", "adagrad", "adam", "ftrl", "momentum", "nesterov", "rmsprop", "rowwise_adagrad",
+        "partial_rowwise_adam")
+# per-element state vectors of each optimizer; ROW_STATE: the index of its state that is one fp32 value per
+# row instead (row-wise AdaGrad's accumulator, partial row-wise Adam's second moment)
 STATES = {"sgd": 0, "adagrad": 1, "adam": 2, "ftrl": 2, "momentum": 1, "nesterov": 1, "rmsprop": 1,
-          "rowwise_adagrad": 0}
+          "rowwise_adagrad": 0, "partial_rowwise_adam": 1}
+ROW_STATE = {"rowwise_adagrad": 0, "partial_rowwise_adam": 1}
 
 
 def card():
@@ -88,9 +96,11 @@ def kernels(a, name, plim):
     from hugectr_b200.embedding import ops as E
     from hugectr_b200.enums import Optimizer_t
     from hugectr_b200.models.dlrm import CRITEO_TB_MULTI_HOT, CRITEO_TB_TABLE_SIZES
-    opt_t = {"sgd": Optimizer_t.SGD, "adagrad": Optimizer_t.AdaGrad, "adam": Optimizer_t.Adam,
-             "ftrl": Optimizer_t.Ftrl, "momentum": Optimizer_t.MomentumSGD, "nesterov": Optimizer_t.Nesterov,
-             "rmsprop": Optimizer_t.RMSProp, "rowwise_adagrad": Optimizer_t.RowWiseAdaGrad}
+    names = {"sgd": "SGD", "adagrad": "AdaGrad", "adam": "Adam", "ftrl": "Ftrl", "momentum": "MomentumSGD",
+             "nesterov": "Nesterov", "rmsprop": "RMSProp", "rowwise_adagrad": "RowWiseAdaGrad",
+             "partial_rowwise_adam": "PartialRowWiseAdam"}
+    # (an older tree, timed or compared with --tree, may lack an optimizer: its arms are left out)
+    opt_t = {k: getattr(Optimizer_t, v) for k, v in names.items() if hasattr(Optimizer_t, v)}
     dev = torch.device("cuda")
     EV = a.ev
     max_rows = a.max_rows or (500_000 if a.digests else 4_000_000 * 128 // EV)
@@ -132,7 +142,7 @@ def kernels(a, name, plim):
         grad = (torch.randn(BATCH * width, device=dev) * 1e-3).to(torch.bfloat16)
     w32 = torch.empty(total_rows * EV, device=dev).uniform_(-0.01, 0.01)
     tables = {"fp32": w32, "bf16": w32.to(torch.bfloat16)}
-    opts = parse_opts(a.opts)
+    opts = [o for o in parse_opts(a.opts) if o in opt_t]
     # arms: (optimizer, state dtype or None); state buffers per dtype, shared by the arms
     arms = []
     for o in opts:
@@ -141,19 +151,20 @@ def kernels(a, name, plim):
     sdt = {"fp32": torch.float32, "bf16": torch.bfloat16}
     bufs = {sd: [torch.zeros(total_rows * EV, dtype=sdt[sd], device=dev) for _ in range(need)]
             for sd in {sd for _, sd in arms if sd}}
-    if "rowwise_adagrad" in opts:
+    if any(o in ROW_STATE for o in opts):
         bufs["row"] = [torch.zeros(total_rows, device=dev)]
     ws = E.UniqueWorkspace(pairs, EV, dev, indexed=True)
     lr_t = torch.full((1,), 1e-3, device=dev)
     st_t = torch.ones(1, dtype=torch.int32, device=dev)
-    hp = {"epsilon": 1e-8, "sr_seed": 1}
+    hp = {"epsilon": 1e-8, "sr_seed": 1, "beta1": 0.9, "beta2": 0.999}
 
     def arm_name(o, sd):
         return f"{o}_{sd}_state" if sd else o
 
     def states(o, sd):
-        b = bufs["row"] if o == "rowwise_adagrad" else bufs.get(sd, [])
-        s = b[:max(STATES[o], 1 if o == "rowwise_adagrad" else 0)]
+        s = bufs.get(sd, [])[:STATES[o]]
+        if o in ROW_STATE:
+            s.insert(ROW_STATE[o], bufs["row"][0])
         return s + [None] * (2 - len(s))
 
     def fwd(w):
@@ -231,7 +242,7 @@ def kernels(a, name, plim):
              pairs * EV * wb + pairs * 4 + BATCH * width * 2)
         for o, sd in arms:
             # weight read + write and state read + write per distinct row, one bf16 gradient row + locator per key
-            srow = 8 if o == "rowwise_adagrad" else EV * 2 * STATES[o] * (sdt[sd].itemsize if sd else 0)
+            srow = EV * 2 * STATES[o] * (sdt[sd].itemsize if sd else 0) + (8 if o in ROW_STATE else 0)
             row_bytes = EV * 2 * wb + srow
             line({"optimizer": arm_name(o, sd), "weights": w, "phase": "fused backward",
                   "update_bytes_per_row": row_bytes}, res[(w, (o, sd))], uniq * row_bytes + pairs * (EV * 2 + 4))
@@ -251,6 +262,8 @@ def check_bits(a):
         runs.append(json.loads(r.stdout.strip().splitlines()[-1]))
     mine, other, again = runs
     bad = 0
+    for arm in sorted(set(mine) - set(other)):     # optimizers TREE does not have
+        print(json.dumps({"arm": arm, "new": True}), flush=True)
     for arm in other:
         same = {k: mine.get(arm, {}).get(k) == v for k, v in other[arm].items()}
         stable = {k: again[arm][k] == v for k, v in other[arm].items()}
@@ -259,21 +272,23 @@ def check_bits(a):
         print(json.dumps({"arm": arm, "equal": same, "other_tree_equals_itself": stable, "fail": fail}), flush=True)
     print(json.dumps({"check_bits": os.path.abspath(a.check_bits), "keys": a.keys, "ev": a.ev, "steps": a.steps,
                       "arms": len(other), "failed": bad}), flush=True)
-    return 1 if bad or set(mine) != set(other) else 0
+    return 1 if bad or not set(other) <= set(mine) else 0
 
 
 def full_model(a, name, plim):
     from hugectr_b200.models.dlrm import CRITEO_TB_TABLE_SIZES, build_dlrm_dcnv2
     torch.cuda.set_device(0)
     t0 = time.time()
-    m = build_dlrm_dcnv2(batchsize=BATCH, num_gpus=1, embedding_optimizer="rowwise_adagrad", weight_dtype="bf16",
-                         use_cuda_graph=True)
+    opt = "partial_rowwise_adam" if "partial_rowwise_adam" in parse_opts(a.opts) else "rowwise_adagrad"
+    sizes = [min(s, a.max_rows) if a.max_rows else s for s in CRITEO_TB_TABLE_SIZES]
+    m = build_dlrm_dcnv2(batchsize=BATCH, num_gpus=1, table_sizes=sizes, embedding_optimizer=opt,
+                         weight_dtype="bf16", use_cuda_graph=True)
     m.compile()
     e = m.ebcs_train[0]
     tb = sum(g.table.numel() * g.table.element_size() for g in e.groups)
-    sb = sum(g.s0.numel() * g.s0.element_size() for g in e.groups if g.s0 is not None)
-    print(f"# built in {time.time() - t0:.0f} s: {sum(CRITEO_TB_TABLE_SIZES)} rows, tables {tb / 1e9:.2f} GB, "
-          f"row-wise state {sb / 1e9:.2f} GB", flush=True)
+    sb = sum(s.numel() * s.element_size() for g in e.groups for s in (g.s0, g.s1) if s is not None)
+    print(f"# built in {time.time() - t0:.0f} s: {opt}, {sum(sizes)} rows (cap {a.max_rows or 'none'}), tables "
+          f"{tb / 1e9:.2f} GB, state {sb / 1e9:.2f} GB", flush=True)
     for _ in range(a.warmup):
         m.train()
     torch.cuda.synchronize()
@@ -285,7 +300,8 @@ def full_model(a, name, plim):
     ev.synchronize()
     ms = s.elapsed_time(ev) / a.steps
     loss = m.get_current_loss()
-    print(json.dumps({"mode": "full-model", "table_GB": round(tb / 1e9, 2), "state_GB": round(sb / 1e9, 3),
+    print(json.dumps({"mode": "full-model", "optimizer": opt, "row_cap": a.max_rows or None, "rows": sum(sizes),
+                      "table_GB": round(tb / 1e9, 2), "state_GB": round(sb / 1e9, 3),
                       "max_memory_allocated_GB": round(torch.cuda.max_memory_allocated() / 1e9, 2),
                       "step_ms": round(ms, 3), "steps": a.steps, "final_loss": loss, "batch": BATCH,
                       "device": name, "power_limit": plim}), flush=True)
