@@ -3,7 +3,6 @@ import pytest
 import torch
 
 from hugectr_b200.embedding import ops as E
-from hugectr_b200.ops import dense as D
 
 pytestmark = pytest.mark.gpu
 
@@ -40,32 +39,6 @@ def test_dp_dense_wgrad_privatized_and_global(act):
     torch.cuda.synchronize()
     err = (out.cpu() - ref).abs().max().item()
     assert err < 2e-3 * max(1.0, ref.abs().max().item()), err
-
-
-@pytest.mark.parametrize("acc", [torch.bfloat16, torch.float32])
-def test_cross_bwd_elementwise(acc):
-    torch.manual_seed(0)
-    b, w = 300, 1160  # 145 column groups: exercises the partial column block
-    mk = lambda: torch.randn(b, w, device="cuda").bfloat16()
-    dy, x0, t = mk(), mk(), mk()
-    dt = torch.empty_like(dy)
-    dx0 = torch.zeros(b, w, device="cuda", dtype=acc)
-    db = torch.zeros(w, device="cuda")
-    ref_dx0 = torch.zeros(b, w)
-    ref_db = torch.zeros(w)
-    for step, (first, last) in enumerate([(True, False), (False, False), (False, True)]):
-        D.cross_bwd_ew(dy, x0, t, dt, dx0, first, db, last=last)
-        d = dy.float().cpu()
-        rdt = (d * x0.float().cpu()).bfloat16()
-        ref_db += rdt.float().sum(0)
-        accv = d * t.float().cpu() + (d if last else 0)
-        ref_dx0 = accv if first else ref_dx0 + accv
-        if acc == torch.bfloat16:
-            ref_dx0 = ref_dx0.bfloat16().float()
-        assert torch.equal(dt.cpu(), rdt)
-    tol = 0.05 if acc == torch.bfloat16 else 1e-4
-    assert (dx0.float().cpu() - ref_dx0).abs().max().item() < tol * max(1.0, ref_dx0.abs().max().item())
-    assert (db.cpu() - ref_db).abs().max().item() < 1e-2 * max(1.0, ref_db.abs().max().item())
 
 
 @pytest.mark.parametrize("ev,shards", [(128, 8), (64, 3), (16, 2), (256, 4)])

@@ -48,6 +48,12 @@ def test_ebc_fwd_bwd_matches_cpu(opt, ev):
             torch.testing.assert_close(gg.table.cpu(), cg.table, rtol=1e-3, atol=2e-4)
 
 
+# bf16 activations and gradients against the fp32 CPU path: the per-step gradients differ by ~1% of their
+# norm (see test_dense_path_fp64_gpu.py); 0.1 leaves margin for four steps and stays far below the 1.0 of
+# a step whose dense gradients are lost
+DELTA_REL = 0.1
+
+
 def test_dcnv2_step_matches_cpu_reference():
     """bf16 wgmma path vs fp32 CPU path: same init, same batch -> close loss and weights."""
     from hugectr_b200.models.dlrm import build_dlrm_dcnv2
@@ -58,7 +64,8 @@ def test_dcnv2_step_matches_cpu_reference():
     mg = build_dlrm_dcnv2(mixed=True, comm=Comm(torch.device("cuda")), **kw)
     mc = build_dlrm_dcnv2(mixed=False, comm=Comm(torch.device("cpu")), **kw)
     mg.compile(); mc.compile()
-    mc.arena.load_flat(mg.arena.dump_flat())
+    w0 = mg.arena.dump_flat()
+    mc.arena.load_flat(w0)
     for gg, cg in zip(mg.ebcs_train[0].groups, mc.ebcs_train[0].groups):
         cg.table.copy_(gg.table.cpu())
     hb = mc.reader_train.pool[0]
@@ -68,9 +75,11 @@ def test_dcnv2_step_matches_cpu_reference():
         lg.append(mg.get_current_loss()); lc.append(mc.get_current_loss())
     for a, b in zip(lg, lc):
         assert abs(a - b) < 0.03 * max(1.0, abs(b)), (lg, lc)
-    wg, wc = mg.arena.dump_flat(), mc.arena.dump_flat()
-    rel = (wg - wc).norm() / wc.norm()
-    assert rel < 0.03, rel
+    # four SGD steps at lr 0.01 move the dense weights by ~0.02% of their norm, so the weights themselves
+    # cannot show a wrong gradient: compare what the steps changed, relative to the size of that change
+    dg, dc = mg.arena.dump_flat() - w0, mc.arena.dump_flat() - w0
+    rel = ((dg - dc).norm() / dc.norm()).item()
+    assert rel < DELTA_REL, rel
 
 
 def test_cuda_graph_equals_eager():
