@@ -571,11 +571,10 @@ __global__ void __launch_bounds__(256)
   for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
   if (!__all_sync(0xffffffffu, finite) && lane == 0) *bad = 1;
   const int e = e4m3_scale_exp(amax);
-  const float inv = ldexpf(1.f, -e);
   const long long r = rows[w];
   uint8_t* d = q + r * pitch;
   for (int c = lane; c < pitch; c += 32)
-    d[c] = static_cast<uint8_t>(__nv_cvt_float_to_fp8(x[c] * inv, __NV_SATFINITE, __NV_E4M3));
+    d[c] = static_cast<uint8_t>(__nv_cvt_float_to_fp8(e4m3_scale_down(x[c], e), __NV_SATFINITE, __NV_E4M3));
   if (lane == 0) exps[r] = static_cast<uint8_t>(e + 127);
 }
 

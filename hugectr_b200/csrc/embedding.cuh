@@ -184,9 +184,10 @@ HCTR_DEVICE float ldg_row1(const __nv_fp8_e4m3* p) {
   const unsigned char b = __ldg(reinterpret_cast<const unsigned char*>(p));
   return __half2float(__half(__nv_cvt_fp8_to_halfraw(static_cast<__nv_fp8_storage_t>(b), __NV_E4M3)));
 }
-// 2^e of arena row `row` of an e4m3 arena (exps[row] = e + 127), exact.  Byte 0 gives 0 instead of the
-// subnormal 2^-127: the device quantizer writes it for all-zero rows only (rows with amax below
-// 448 * 2^-126 flush to e = -1 and zero bytes), so the pooled value is 0 either way.
+// 2^e of arena row `row` of an e4m3 arena (exps[row] = e + 127), exact for bytes 1..254.  Byte 0 gives 0 instead
+// of the subnormal 2^-127, which the fast-math (flush-to-zero) weight multiply would flush anyway: a row with
+// e = -127 -- all-zero, or amax at most 448 * 2^-127 (about 2^-118.2) with nonzero codes -- pools to zero in the
+// fp8 lookup (docs/embedding.md, fp8 serving tables: exactness).
 HCTR_DEVICE float row_scale(const uint8_t* exps, long long row) {
   return __uint_as_float(static_cast<unsigned int>(__ldg(exps + row)) << 23);
 }

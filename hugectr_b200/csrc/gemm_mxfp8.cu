@@ -4,6 +4,12 @@
 // format).  Hopper's fp8 wgmma has no block scaling, and one m64n128k32 wgmma covers exactly one 32-wide scale
 // slice, so every slice is accumulated into a temporary register tile and promoted into the fp32 accumulator
 // with the product of its row and column scales (powers of two: the promotion is exact up to fp32 rounding).
+// Scale range: the product s0 * sc = 2^(ea + eb - 254) of scale bytes ea, eb is a fast-math (flush-to-zero) fp32
+// multiply, so a slice is promoted exactly only while ea + eb - 254 lies in [-126, 127] and neither byte is 0.  A
+// slice with ea + eb < 128, or a scale byte of 0 (read as zero, not 2^-127), adds nothing, even where its products
+// times the scales would be normal fp32 numbers; above the range the scale product is +inf (and a zero partial sum
+// times it NaN).  Quantised activations and weights of a trained model sit far inside the range
+// (tests/test_mxfp8_fp64_gpu.py pins its ends).
 // CTA (one 128 x 128 output tile) = three warpgroups:
 //   warpgroup 0   TMA producer: A / B tiles (128 rows x 128 bytes, SWIZZLE_128B) + the 512-byte scale blocks of
 //                 the k-block (1-D bulk copies) into a ring of stages, completion on the stage's mbarrier
@@ -151,14 +157,13 @@ __global__ void __launch_bounds__(256)
       for (int j = 0; j < 32; ++j) v[j] = 0.f;
     }
     const int e = e4m3_scale_exp(amax);
-    const float inv = ldexpf(1.f, -e);
     uint32_t w[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
-      const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(make_float2(v[4 * j] * inv, v[4 * j + 1] * inv),
-                                                                  __NV_SATFINITE, __NV_E4M3);
-      const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(make_float2(v[4 * j + 2] * inv, v[4 * j + 3] * inv),
-                                                                  __NV_SATFINITE, __NV_E4M3);
+      const __nv_fp8x2_storage_t lo = __nv_cvt_float2_to_fp8x2(
+          make_float2(e4m3_scale_down(v[4 * j], e), e4m3_scale_down(v[4 * j + 1], e)), __NV_SATFINITE, __NV_E4M3);
+      const __nv_fp8x2_storage_t hi = __nv_cvt_float2_to_fp8x2(
+          make_float2(e4m3_scale_down(v[4 * j + 2], e), e4m3_scale_down(v[4 * j + 3], e)), __NV_SATFINITE, __NV_E4M3);
       w[j] = static_cast<uint32_t>(lo) | (static_cast<uint32_t>(hi) << 16);
     }
     uint4* dst = reinterpret_cast<uint4*>(q + static_cast<long long>(r) * cols + cb * 32);

@@ -1,6 +1,7 @@
 // D2: DLRM dot-product interaction on Hopper wgmma (fwd + bwd), bf16, n <= 32 rows, D <= 128, D % 16 == 0.
 //   fwd : out[s] = [ mlp[s] | strict lower triangle of X X^T (row-major) | 0 ],  X = [mlp[s]; emb[s]]
-//   bwd : dX = (G + G^T) X  with G the lower-triangular gradient matrix;  dmlp += dout[:, :D]
+//   bwd : dX = (G + G^T) X  with G the lower-triangular gradient matrix;  dmlp = dX[0] + dout[:, :D],
+//         demb = dX[1:] (both overwritten)
 // Reference: HugeCTR/src/layers/interaction_layer.cu:47-596 (Volta wmma 16x16x16, one warp per
 // sample).  Here FOUR samples share one tile: their (zero padded) 32-row blocks are stacked into a
 // 128-row operand that sits in shared memory in the canonical SWIZZLE_128B layout.  Each of the two

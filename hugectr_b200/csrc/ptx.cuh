@@ -14,19 +14,24 @@ HCTR_DEVICE uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-// Exponent e of the power-of-two scale of a block (or row) of e4m3 values whose largest magnitude is amax:
+// Exponent e of the power-of-two scale of a block (or row) of e4m3 values whose largest magnitude is amax >= 0:
 // the smallest 2^e with amax / 2^e <= 448 (e4m3 max), clamped to [-127, 127]; -127 when amax == 0.
-// (frexp instead of log2: exact and independent of --use_fast_math; v = m * 2^ex, m in [0.5, 1))
-// Mirrored by ops/mxfp8.py::e4m3_scale_exponent.
+// Integer arithmetic on the bits of amax = m * 2^ex (m in [0.5, 1)): 448 = 0.875 * 2^9, so e = ex - 9 + (m > 0.875).
+// A float multiply (amax * (1 / 448)) flushes to zero under --use_fast_math for amax below 448 * 2^-126; amax below
+// 2^-126 gives e < -127 anyway.  Mirrored by ops/mxfp8.py::e4m3_scale_exponent.
 HCTR_DEVICE int e4m3_scale_exp(float amax) {
-  int e = -127;
-  if (amax > 0.f) {
-    int ex;
-    const float m = frexpf(amax * (1.f / 448.f), &ex);
-    e = (m > 0.5f) ? ex : ex - 1;
-    e = max(-127, min(127, e));
-  }
-  return e;
+  const uint32_t b = __float_as_uint(amax);
+  if (b < 0x00800000u) return -127;                               // zero or subnormal
+  const int e = static_cast<int>(b >> 23) - 126 - 9 + ((b & 0x7fffffu) > 0x600000u);
+  return min(127, max(-127, e));
+}
+
+// x * 2^-e for an e4m3_scale_exp exponent e, rounded once as IEEE fp32 (subnormal operands and results kept):
+// fast math turns every fp32 multiply, __fmul_rn included, into mul.ftz, which would zero x below 2^-126.
+HCTR_DEVICE float e4m3_scale_down(float x, int e) {
+  float r;
+  asm("mul.rn.f32 %0, %1, %2;" : "=f"(r) : "f"(x), "f"(__uint_as_float(static_cast<uint32_t>(127 - e) << 23)));
+  return r;
 }
 
 HCTR_DEVICE uint32_t lane_id() {

@@ -37,7 +37,7 @@ def interaction_fwd(mlp, emb, out):
 
 def interaction_bwd(mlp, emb, dout, dmlp, demb):
     from . import interaction_native as N
-    if N.available(mlp, emb, dout) and dmlp is not None and demb is not None:
+    if dmlp is not None and demb is not None and N.available(mlp, emb, dout, dmlp, demb):
         return N.bwd(mlp, emb, dout, dmlp, demb)
     b, d = mlp.shape
     n = emb.shape[1] + 1

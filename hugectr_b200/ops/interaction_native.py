@@ -25,11 +25,14 @@ def _lib():
     return l
 
 
-def available(mlp, emb, out) -> bool:
-    if not (mlp.is_cuda and mlp.dtype == torch.bfloat16 and emb.dtype == torch.bfloat16
-            and out.dtype == torch.bfloat16):
+def available(mlp, emb, out, *grads) -> bool:
+    """The kernels take contiguous bf16 tensors on 16-byte bases (they move rows in 16-byte vectors), n <= 32 and
+    D <= 128, D % 16 == 0.  ``out`` is the forward's output or the backward's dout; ``grads`` the backward's
+    dmlp and demb."""
+    ts = (mlp, emb, out, *grads)
+    if not (mlp.is_cuda and all(t.dtype == torch.bfloat16 for t in ts)):
         return False
-    if not (mlp.is_contiguous() and emb.is_contiguous() and out.is_contiguous()):
+    if not all(t.is_contiguous() and t.data_ptr() % 16 == 0 for t in ts):
         return False
     _lib()
     n = emb.shape[1] + 1

@@ -62,12 +62,12 @@ def mx_quantize(x: torch.Tensor, q=None, sf=None, transposed: bool = False):
 
 
 def e4m3_scale_exponent(amax: torch.Tensor) -> torch.Tensor:
-    """fp32 exponents e of the power-of-two scales of blocks whose largest magnitudes are ``amax`` (fp32): the
-    smallest 2^e with amax / 2^e <= 448 (e4m3 max), clamped to [-127, 127], -127 for amax == 0 -- computed exactly
-    as e4m3_scale_exp in csrc/ptx.cuh (fp32 frexp of amax * (1 / 448))"""
-    m, ex = torch.frexp(amax * torch.tensor(1.0 / 448.0, dtype=torch.float32))
-    e = torch.where(m > 0.5, ex, ex - 1).to(torch.float32)
-    return torch.where(amax > 0, e, torch.full_like(e, -127.0)).clamp(-127, 127)
+    """fp32 exponents e of the power-of-two scales of blocks whose largest magnitudes are ``amax`` (fp32, >= 0): the
+    smallest 2^e with amax / 2^e <= 448 (e4m3 max), clamped to [-127, 127], -127 for amax == 0 -- computed as
+    e4m3_scale_exp in csrc/ptx.cuh, from the bits of amax = m * 2^ex: e = ex - 9 + (m > 0.875)"""
+    b = amax.to(torch.float32).contiguous().view(torch.int32)
+    e = (b >> 23) - 135 + ((b & 0x7FFFFF) > 0x600000).to(torch.int32)
+    return torch.where(b < 0x00800000, -127, e).clamp(-127, 127).to(torch.float32)
 
 
 def mx_quantize_reference(x: torch.Tensor):
@@ -93,12 +93,39 @@ def mx_dequantize(q: torch.Tensor, sf: torch.Tensor, rows: int, cols: int) -> to
     return (v * torch.exp2(t.float() - 127.0).unsqueeze(-1)).reshape(rp, cols)[:rows]
 
 
+GEMM_FLAGS = G.EPI_RELU | G.EPI_SIGMOID | G.EPI_OUT_F32
+
+
+def gemm_mxfp8_eligible(aq, sfa, bq, sfb, M: int, N: int, K: int, out, bias=None, flags: int = 0) -> bool:
+    """What hctr_gemm_mxfp8 reads and writes is there: the epilogue flags it implements (the others read
+    tensors it is not given), q / sf buffers as large as the tensor maps and the scale bulk copies cover
+    (contiguous, 16-byte bases), and an ``out`` / ``bias`` the epilogue can address with its 16-byte
+    vector loads and stores (``gemm.epi_eligible``)."""
+    if flags & ~GEMM_FLAGS or K <= 0 or K % 128:
+        return False
+    mp, np_ = _pad128(M), _pad128(N)
+    for t, need in ((aq, mp * K), (bq, np_ * K), (sfa, mp // 128 * (K // 128) * 512),
+                    (sfb, np_ // 128 * (K // 128) * 512)):
+        if t.element_size() != 1 or not t.is_contiguous() or t.numel() < need or t.data_ptr() % 16:
+            return False
+    want = torch.float32 if flags & G.EPI_OUT_F32 else torch.bfloat16
+    if out.dtype != want or out.dim() != 2 or out.shape[0] < M or out.shape[1] < N:
+        return False
+    if bias is not None and (bias.dtype != torch.float32 or bias.numel() < N):
+        return False
+    return G.epi_eligible(M, N, out, bias)
+
+
 def gemm_mxfp8(aq, sfa, bq, sfb, M: int, N: int, K: int, out=None, bias=None, flags: int = 0, alpha: float = 1.0):
-    """out[M, N] = epilogue(alpha * deq(A)[M, K] @ deq(B)[N, K]^T (+ bias))"""
+    """out[M, N] = epilogue(alpha * deq(A)[M, K] @ deq(B)[N, K]^T (+ bias)); flags: EPI_RELU, EPI_SIGMOID,
+    EPI_OUT_F32.  Raises ValueError, before any launch, on arguments gemm_mxfp8_eligible rejects."""
     f32 = bool(flags & G.EPI_OUT_F32)
     if out is None:
         out = torch.empty(M, N, device=aq.device, dtype=torch.float32 if f32 else torch.bfloat16)
     if aq.is_cuda:
+        if not gemm_mxfp8_eligible(aq, sfa, bq, sfb, M, N, K, out, bias, flags):
+            raise ValueError(f"gemm_mxfp8: M={M} N={N} K={K} flags={flags}: unsupported flags, undersized or "
+                             "misaligned q / sf buffers, or an out / bias the epilogue cannot address")
         rc = lib().hctr_gemm_mxfp8(aq.data_ptr(), sfa.data_ptr(), bq.data_ptr(), sfb.data_ptr(), out.data_ptr(), M, N,
                                    K, out.stride(0), 0 if bias is None else bias.data_ptr(), float(alpha), int(flags),
                                    torch.cuda.current_stream(aq.device).cuda_stream)

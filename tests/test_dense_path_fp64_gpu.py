@@ -427,6 +427,14 @@ def _check_mlp(layer, x):
             ref = torch.relu(ref)
         assert_sum(layer.acts[i], ref, mag, h.shape[1], BF16_R, f"acts[{i}]")
         h = layer.acts[i]
+    check_mlp_bprop(layer, x)
+
+
+def check_mlp_bprop(layer, x):
+    """every GEMM / kernel of one MLP bprop against fp64 on the bf16 activations and weights the layer kept"""
+    n = len(layer.dims_out)
+    kin = layer.k_in
+    xin = layer._x_in
     dy = layer.outputs[0].grad.reshape(layer.rows, -1)
     for i in range(n - 1, -1, -1):
         x_i = xin if i == 0 else layer.acts[i - 1]

@@ -89,6 +89,48 @@ def test_fp8_lookup_equals_fp32_lookup_over_dequantized_table(pitch):
     assert n == 64
 
 
+def test_fp8_lookup_at_the_bottom_of_the_exponent_range():
+    """the boundary of the exactness above (docs/embedding.md): a row at e = -126 whose dequantized values are
+    normal fp32 numbers still looks up bit for bit as the fp32 table; a row with exponent byte 0 (e = -127, nonzero
+    codes) pools to zero in the device fp8 lookup, where the fp32 lookup over the dequantized table and the CPU fp8
+    lookup keep its values"""
+    pitch, n = 64, 4
+    g = torch.Generator().manual_seed(3)
+    x = torch.zeros(n, pitch)
+    x[0] = torch.randn(pitch, generator=g)
+    x[1] = torch.rand(pitch, generator=g) * 2.0 ** -120                 # amax < 448 * 2^-127: byte 0
+    x[1, 0] = 2.0 ** -120
+    codes = torch.randint(0x38, 0x7F, (pitch,), generator=g).to(torch.uint8)   # e4m3 values 1 .. 448
+    codes[0] = 0x7E
+    x[2] = codes.view(torch.float8_e4m3fn).float() * 2.0 ** -126       # amax 448 * 2^-126: e = -126, all normal
+    table = torch.zeros(n * pitch, dtype=torch.float8_e4m3fn, device=DEV)
+    exps = torch.zeros(n, dtype=torch.uint8, device=DEV)
+    bad = torch.zeros(1, dtype=torch.int32, device=DEV)
+    E.quantize_rows(x, torch.arange(n), table, exps, bad)
+    q, e = E.fp8_rows_quantize(x)
+    assert torch.equal(table.view(torch.uint8).view(n, pitch).cpu(), q.view(torch.uint8))
+    assert torch.equal(exps.cpu(), e) and e.tolist() == [e[0].item(), 0, 1, 0]
+    deq = E.fp8_rows_dequantize(q, e)
+    assert bool((deq[2].abs() >= 2.0 ** -126).all()) and bool((deq[1] != 0).any())
+    keys = torch.arange(n, dtype=torch.int64).view(n, 1)
+    lk = E.LookupDesc(table_row_off=0, key_off=0, out_off=0, grad_off=0, hotness=1, key_stride=1, num_shards=1,
+                      shard_idx=0, out_stride=pitch, grad_stride=pitch, combiner=0, ev_size=pitch, rows=n,
+                      nnz_off=-1, weighted=0)
+    outs = []
+    for dev in (DEV, "cpu"):
+        for tab, rexp in ((table.to(dev), exps.to(dev)), (deq.reshape(-1).to(dev), None)):
+            out = torch.full((n, pitch), 7.0, device=dev)
+            E.forward([lk], E.lookups_to_device([lk], dev) if dev == DEV else None, tab, pitch, [keys.to(dev)],
+                      [out], n, 0, key_bytes=8, act_bf16=False, row_exp=rexp)
+            outs.append(out.cpu())
+    o8, o32, c8, c32 = outs
+    for r in (0, 2, 3):
+        assert torch.equal(o8[r], o32[r]), r
+    assert bool((o8[1] == 0).all())
+    assert torch.equal(o32[1], deq[1] * (deq[1].abs() >= 2.0 ** -126))     # the fp32 kernel flushes subnormals
+    assert torch.equal(c8, deq) and torch.equal(c32, deq)
+
+
 def test_fp8_session_predicts_as_fp32_session_on_dequantized_checkpoint_gpu(tmp_path):
     from test_embedding_fp8_serving_cpu import build_serving_test_model, session_predictions_match
     m, paths = build_serving_test_model(tmp_path, DEV)
