@@ -297,10 +297,14 @@ class EmbeddingCollection:
     def __init__(self, cfg: EmbeddingCollectionConfig, batch_per_gpu: int, hotness: Dict[str, int],
                  device, act_dtype, comm, default_opt: OptParamsPy, key_dtype=torch.int32,
                  scaler: float = 1.0, state_dtype=torch.float32, seed: int = 0,
-                 fused: Optional[bool] = None, is_train: bool = True, weighted=(), fp8_quant: bool = False):
+                 fused: Optional[bool] = None, is_train: bool = True, weighted=(), fp8_quant: bool = False,
+                 position_weighted=()):
         """``weighted``: names of the sparse inputs whose keys carry an fp32 weight each (see
         docs/embedding.md): every lookup of such an input pools ``sum_h w_h * T[key_h]`` (mean: divided
         by ``sum_h w_h``, or by 1 when that is 0).
+        ``position_weighted``: names of the sparse inputs whose key h of every bag weighs ``P[0, h]``, a dense
+        parameter bound by ``bind_position_weights``: their lookups pool weighted as above, and the backward
+        adds the weights' gradient into ``P``'s gradient (see docs/embedding.md).
         ``fp8_quant`` (serving collections, ``is_train=False``): every table is stored as e4m3 rows with one
         power-of-two scale per row, quantized by every write (initial fill, checkpoint load); lookups pool the
         dequantized rows in fp32 (see docs/embedding.md)."""
@@ -310,6 +314,8 @@ class EmbeddingCollection:
         self._fp8_bad = {}       # table name -> int32 device flag of a non-finite value met by the quantizer
         self.cfg, self.b, self.device, self.act_dtype = cfg, batch_per_gpu, device, act_dtype
         self.weighted_inputs = frozenset(weighted)
+        self.pw_inputs = frozenset(position_weighted)
+        self._pw_params = {}     # position-weighted input -> (P [1, H] fp32, its gradient), bound after the arena
         # who am I / whom do I talk to: through the backend-neutral interface (core.py; reference core.hpp)
         from ..core import as_core
         self.core = as_core(comm)
@@ -415,6 +421,21 @@ class EmbeddingCollection:
                 if t.name in unique:
                     raise ValueError(f"weighted input {bot}: table {t.name} is listed under CompressionStrategy.Unique, "
                                      "which does not carry weights")
+        for lk in self.cfg.lookups:
+            for t, bot, comb in zip(lk["tables"], lk["bottoms"], lk["combiners"]):
+                if bot not in self.pw_inputs:
+                    continue
+                if comb not in ("sum", "mean", "average"):
+                    raise ValueError(f"position-weighted input {bot}: lookup {lk['top']} of table {t.name} uses the "
+                                     f"{comb!r} combiner; position-weighted inputs pool with sum or mean")
+                if t.name in unique:
+                    raise ValueError(f"position-weighted input {bot}: table {t.name} is listed under "
+                                     "CompressionStrategy.Unique, which does not carry weights")
+                if self.placement[t.name].col_factor > 1:
+                    # each column slice would hold a partial dot product of the weight gradient
+                    raise ValueError(f"position-weighted input {bot}: table {t.name} is split column-wise "
+                                     f"(factor {self.placement[t.name].col_factor}); use a table-wise, row-wise or "
+                                     "data-parallel placement")
 
     def eval_clone(self, batch_per_gpu: int) -> "EmbeddingCollection":
         """Second plan (different batch, no grads) over the SAME tables -- the eval graph."""
@@ -448,7 +469,8 @@ class EmbeddingCollection:
                 gl = {"table": t.name, "bottom": bot, "combiner": comb, "hotness": H,
                       "key_off": koff, "top": len(self.tops), "col": col, "ev": t.ev_size,
                       "out_off": ooff + col, "out_stride": width,
-                      "weighted": bot in getattr(self, "weighted_inputs", ())}
+                      "weighted": bot in getattr(self, "weighted_inputs", ()) or bot in getattr(self, "pw_inputs", ()),
+                      "pw": bot in getattr(self, "pw_inputs", ())}
                 koff += b * H
                 col += t.ev_size * (H if comb == "concat" else 1)
                 ids.append(len(self.glookups))
@@ -460,6 +482,8 @@ class EmbeddingCollection:
         self.key_slab_elems = koff
         # fp32 per-key weights in the layout of the user region of the key slab (weighted inputs only)
         self.has_weights = any(gl["weighted"] for gl in self.glookups)
+        # the weights a batch brings (set_weights); those of position-weighted inputs are written in the step
+        self.has_data_weights = any(gl["weighted"] and not gl["pw"] for gl in self.glookups)
         self.nnz_slab_elems = 0
         self.top_slab_elems = ooff
         # partial blocks for row-sharded lookups (k > 1 on the mp side)
@@ -726,6 +750,13 @@ class EmbeddingCollection:
         z = lambda n, dt: torch.zeros(max(int(n), 1), dtype=dt, device=dev)
         self.key_slab = z(self.key_slab_elems, self.key_dtype)
         self.weight_slab = z(self.user_key_elems, torch.float32) if self.has_weights else None
+        # position-weighted inputs: 1 / 0 at the valid / padding key positions (written with the weights, before
+        # dynamic keys are translated, so a key without a row keeps its place in the mean), and the weight
+        # gradient's per-position dot products, one row per source rank
+        pw = any(gl["pw"] for gl in self.glookups)
+        self.pw_valid = z(self.user_key_elems, torch.float32) if pw else None
+        self.pw_dots = torch.zeros(W, max(self.user_key_elems, 1), dtype=torch.float32, device=dev) \
+            if pw and self.is_train else None
         # the key-side channels: the keys (whose peer-memory dispatch also writes the split lengths), then
         # the weights of weighted lookups, which follow their keys' blocks
         self.key_chans = [_KeyChannel(self.key_slab)]
@@ -804,6 +835,14 @@ class EmbeddingCollection:
             if gl["weighted"]:
                 self.weight_views[gl["bottom"]] = self.weight_slab[gl["key_off"]:gl["key_off"] + b * gl["hotness"]] \
                     .view(b, gl["hotness"])
+        self.valid_views = {gl["bottom"]: self.pw_valid[gl["key_off"]:gl["key_off"] + b * gl["hotness"]].view(
+            b, gl["hotness"]) for gl in self.glookups if gl["pw"]}
+        for grp in self.groups:
+            grp.pw_sel = [j for j, (gi, _) in enumerate(getattr(grp, "lookup_gl", [])) if self.glookups[gi]["pw"]]
+            grp.pw_sel_dev = torch.tensor(grp.pw_sel, dtype=torch.int32, device=dev) if grp.pw_sel else None
+        self._pw_event = None
+        if self._pw_params:
+            self.bind_position_weights(self._pw_params)
         self.top_data, self.top_grad = {}, {}
         for tp in self.tops:
             w = tp["width"]
@@ -954,6 +993,34 @@ class EmbeddingCollection:
         """Copy the fp32 per-key weights of a batch, in the layout of ``set_keys``, into the weight slab."""
         self.weight_slab[:feature_major_weights.numel()].copy_(feature_major_weights.reshape(-1), non_blocking=True)
 
+    def bind_position_weights(self, params):
+        """``params``: {position-weighted input: (P [slot_num, H] fp32, its gradient)}, views of the network's
+        parameter arena.  The step reads P from device memory, so a captured step sees every update of it."""
+        self._pw_params = dict(params)
+        missing = sorted({gl["bottom"] for gl in self.glookups if gl["pw"]} - set(self._pw_params))
+        if missing:
+            raise ValueError(f"position-weighted inputs {missing}: no weight parameter bound")
+        self._pw_regions = []
+        for gl in self.glookups:
+            if gl["pw"]:
+                P = self._pw_params[gl["bottom"]][0]
+                if P.shape[-1] != gl["hotness"]:
+                    raise ValueError(f"position-weighted input {gl['bottom']}: its weights have {P.shape[-1]} "
+                                     f"positions, its lookups read {gl['hotness']} keys per bag")
+                self._pw_regions.append((P.reshape(-1), gl["key_off"], self.b * gl["hotness"], gl["hotness"]))
+        self._pw_regions_dev = E.pw_regions_to_device(self._pw_regions, self.device) if self.native else None
+        targets = {}
+        for gl in self.glookups:
+            if gl["pw"]:
+                targets.setdefault(gl["bottom"], []).append((gl["key_off"], gl["hotness"]))
+        self._pw_plan = E.PwReducePlan([(self._pw_params[n][1].reshape(-1), r) for n, r in targets.items()],
+                                       self.device)
+
+    def _fill_position_weights(self):
+        """P[0, h] into the weight slab at every key position h of the position-weighted inputs (0 at padding keys),
+        from the requester's own keys: ahead of the key exchange and of the translation of dynamic keys"""
+        E.pw_fill(self.key_slab, self.weight_slab, self.pw_valid, self._pw_regions, self._pw_regions_dev)
+
     def forward(self, is_train: bool = True):
         self.forward_begin()
         self.forward_compute()
@@ -961,6 +1028,8 @@ class EmbeddingCollection:
 
     def forward_begin(self):
         """every rank's keys are in place (fused mode: device-side barrier; collective: all-to-all)"""
+        if self.pw_valid is not None:
+            self._fill_position_weights()
         if self.world > 1:
             if self.fused:
                 # forward all-to-all of keys: posted peer stores into the owners' inboxes, then ONE
@@ -1300,7 +1369,13 @@ class EmbeddingCollection:
             tp = self.tops[gl["top"]]
             if forward:
                 keys = self.key_views[gl["bottom"]]
-                if gl["weighted"]:
+                if gl["pw"]:
+                    # (the fill wrote 0 at padding keys; a key without a row keeps its weight in the sum)
+                    sw = self.weight_views[gl["bottom"]].sum(1)
+                    self._pw_sum_w = getattr(self, "_pw_sum_w", {})
+                    self._pw_sum_w[gi] = sw
+                    cnt = torch.where(sw == 0, torch.ones_like(sw), sw)
+                elif gl["weighted"]:
                     w = torch.where(keys >= 0, self.weight_views[gl["bottom"]], torch.zeros((), device=keys.device))
                     sw = w.sum(1)
                     cnt = torch.where(sw == 0, torch.ones_like(sw), sw)
@@ -1317,6 +1392,51 @@ class EmbeddingCollection:
                     else self.top_grad[tp["name"]]
             col = t2d[:, gl["col"]:gl["col"] + gl["ev"]]
             col.copy_((col.float() * self._mean_factor[gi]).to(col.dtype))
+
+    def _top2d(self, gl, which):
+        tp = self.tops[gl["top"]]
+        t = (self.top_data if which == "data" else self.top_grad)[tp["name"]]
+        t2d = t if tp.get("alias") else t.reshape(self.b, -1)
+        return t2d[:, gl["col"]:gl["col"] + gl["ev"]]
+
+    def _pw_mean_terms(self):
+        """The requester's share of the weight gradient of its mean bags: -<pooled, g> / sum_w at every valid key
+        position of a bag whose weights do not sum to 0 (g = dL/dpooled: before the backward rescale)"""
+        self.pw_dots.zero_()
+        mine = self.pw_dots[self.rank]
+        for gi, gl in enumerate(self.glookups):
+            if not gl["pw"] or gl["combiner"] not in ("mean", "average"):
+                continue
+            dot = (self._top2d(gl, "data").float() * self._top2d(gl, "grad").float()).sum(1)
+            sw = self._pw_sum_w[gi]
+            term = torch.where(sw == 0, torch.zeros_like(sw), -dot / torch.where(sw == 0, torch.ones_like(sw), sw))
+            n = self.b * gl["hotness"]
+            mine[gl["key_off"]:gl["key_off"] + n].view(self.b, gl["hotness"]).copy_(
+                self.valid_views[gl["bottom"]] * term.unsqueeze(1))
+
+    def _pw_dots(self, grp):
+        """the owner's dot products <T[row_h], g> of the position-weighted lookups of ``grp`` (before its update)"""
+        if not grp.pw_sel:
+            return
+        s = grp.src
+        dots = list(self.pw_dots.unbind(0)) if len(s.keys) > 1 else [self.pw_dots[self.rank]]
+        E.pw_dots(grp.lookups, grp.lookups_dev, grp.pw_sel, grp.pw_sel_dev, grp.table, grp.pitch, s.keys, s.grads,
+                  self.b, dots, self.rank, nnz_bufs=s.nnz, key_bytes=self._kb, act_bf16=self._abf)
+
+    def _pw_reduce(self):
+        """column sums of the dot products into the gradient of P (the lookups of one input in order); then marks
+        the gradient done (wait_position_weight_grad)"""
+        E.pw_reduce(self.pw_dots, self.b, self._pw_plan)
+        if self.native:
+            self._pw_event = torch.cuda.Event()
+            self._pw_event.record()
+
+    def wait_position_weight_grad(self):
+        """make the current stream wait for the weight gradient of the position-weighted inputs of the last
+        backward (the dense all-reduce and optimizer read it)"""
+        if self._pw_event is not None:
+            torch.cuda.current_stream().wait_event(self._pw_event)
+            self._pw_event = None
 
     def _reduce_partials(self):
         b = self.b
@@ -1358,14 +1478,24 @@ class EmbeddingCollection:
         if not getattr(self, "_index_done", False):
             self.backward_index()
         self._index_done = False
+        pw = self.pw_dots is not None
+        if pw:
+            self._pw_mean_terms()
         self._rescale_mean(forward=False)
         dp_groups = [g for g in self.groups if g.kind == "dp"]
         mp_groups = [g for g in self.groups if g.kind != "dp"]
         side = dp_stream is not None and self.device.type == "cuda" and bool(dp_groups)
+        dp_dots_done = None
         if side:
             cur = torch.cuda.current_stream()
             dp_stream.wait_stream(cur)
             with torch.cuda.stream(dp_stream):
+                for grp in dp_groups:
+                    if pw:
+                        self._pw_dots(grp)
+                if pw:
+                    dp_dots_done = torch.cuda.Event()
+                    dp_dots_done.record()
                 for grp in dp_groups:
                     self._accum_update(grp, lr_t, step_t)
         if self.world > 1:
@@ -1389,6 +1519,12 @@ class EmbeddingCollection:
                 self.comm.all_to_all_v(recv, send, [pk["n_me"]] * self.world, pk["n"])
                 if pk["n_me"]:
                     self.grads_all.index_copy_(1, pk["grad_me"], recv.view(self.world, pk["n_me"]))
+        if pw:
+            for grp in mp_groups + ([] if side else dp_groups):
+                self._pw_dots(grp)
+            if dp_dots_done is not None:
+                torch.cuda.current_stream().wait_event(dp_dots_done)
+            self._pw_reduce()
         for grp in mp_groups:
             self._accum_update(grp, lr_t, step_t)
         if getattr(self, "_uniq", None) is not None:

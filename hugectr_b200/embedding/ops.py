@@ -797,3 +797,137 @@ def bwd_reduce_update(opt: Optimizer_t, lookups, lookups_dev, table, s0, s1, ev_
     if rc:
         raise RuntimeError(f"hctr_emb_bwd_reduce_update failed rc={rc}")
     D._count(3)
+
+
+# ----------------------------------------------------------------------------- position-weighted inputs
+class CPwFillRegion(C.Structure):
+    _fields_ = [("p", C.c_void_p), ("key_off", C.c_longlong), ("n", C.c_longlong), ("hotness", C.c_int),
+                ("pad_", C.c_int)]
+
+
+class CPwReduceCol(C.Structure):
+    _fields_ = [("off", C.c_longlong), ("hotness", C.c_int), ("h", C.c_int)]
+
+
+class CPwReduceTarget(C.Structure):
+    _fields_ = [("dst", C.c_void_p), ("col_begin", C.c_int), ("ncols", C.c_int)]
+
+
+def _pw_lib():
+    l = lib()
+    if not hasattr(l, "_pw_ready"):
+        vp, i, ll = C.c_void_p, C.c_int, C.c_longlong
+        l.hctr_emb_pw_fill.argtypes = [vp, i, vp, vp, vp, i, ll, vp]
+        l.hctr_emb_pw_dot.argtypes = [C.POINTER(CEmbParams), vp, i, vp, ll, i, i, i, i, vp]
+        l.hctr_emb_pw_reduce.argtypes = [vp, ll, i, i, vp, vp, i, vp]
+        for n in ("hctr_emb_pw_fill", "hctr_emb_pw_dot", "hctr_emb_pw_reduce"):
+            getattr(l, n).restype = i
+        sz = (C.c_int * 3)()
+        l.hctr_abi_sizes_pw(sz)
+        if list(sz) != [C.sizeof(CPwFillRegion), C.sizeof(CPwReduceCol), C.sizeof(CPwReduceTarget)]:
+            raise RuntimeError("libhctr_cuda.so position-weight descriptor layouts differ from the python mirrors: "
+                               "rebuild")
+        l._pw_ready = True
+    return l
+
+
+def pw_regions_to_device(regions, device) -> torch.Tensor:
+    """[(P tensor [H] fp32, key_off, n, H)] -> device array of PwFillRegion"""
+    arr = (CPwFillRegion * max(1, len(regions)))()
+    for j, (p, off, n, h) in enumerate(regions):
+        arr[j] = CPwFillRegion(p.data_ptr(), off, n, h, 0)
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).clone().to(device)
+
+
+def pw_fill(keys, weights, valid, regions, regions_dev):
+    """Weights of position-weighted inputs: for every region (P [H], key_off, n, H) of the key slab ``keys``,
+    weights[key_off + i] = P[i % H] and valid[key_off + i] = 1 where the key is >= 0, both 0 at padding keys."""
+    if not regions:
+        return
+    if keys.is_cuda:
+        rc = _pw_lib().hctr_emb_pw_fill(keys.data_ptr(), keys.element_size(), weights.data_ptr(), valid.data_ptr(),
+                                        regions_dev.data_ptr(), len(regions), max(r[2] for r in regions),
+                                        _st(keys.device))
+        if rc:
+            raise RuntimeError(f"hctr_emb_pw_fill failed rc={rc}")
+        D._count()
+        return
+    for p, off, n, h in regions:
+        ok = keys[off:off + n].view(-1, h) >= 0
+        weights[off:off + n].view(-1, h).copy_(torch.where(ok, p.view(1, h), torch.zeros((), dtype=torch.float32)))
+        valid[off:off + n].view(-1, h).copy_(ok.float())
+
+
+def pw_dots(lookups, lookups_dev, sel, sel_dev, table, ev_pitch, key_bufs, grad_bufs, batch, dots, my_rank=0,
+            nnz_bufs=None, key_bytes=4, act_bf16=True):
+    """Weight gradient of position-weighted lookups: for the lookups ``sel`` (indices into ``lookups``) and every
+    owned key h of bag (source rank r, sample s), dots[r][pos] += <T[row_h], g[r, s]> (times 1/nnz for mean),
+    pos the key's element offset.  ``dots``: one fp32 buffer per source rank (rows of one tensor) in the layout
+    of the key slab.  Reads the rows as the forward did, so it runs before the sparse update."""
+    if not sel:
+        return
+    if table.is_cuda:
+        p, kb, gbf = _params(lookups, lookups_dev, table, ev_pitch, key_bufs, batch, my_rank, key_bytes, act_bf16,
+                             nnz_bufs, grad_bufs=grad_bufs)
+        sl = [lookups[j] for j in sel]
+        check_ev_size(max(l.ev_size for l in sl))
+        ev4 = int(vec4_aligned(sl, ev_pitch, [table, *grad_bufs], grad=True))
+        stride = dots[1].data_ptr() - dots[0].data_ptr() if len(dots) > 1 else 0
+        rc = _pw_lib().hctr_emb_pw_dot(C.byref(p), sel_dev.data_ptr(), len(sel), dots[0].data_ptr(), stride // 4,
+                                       kb, gbf, int(table.dtype == torch.bfloat16), ev4, _st(table.device))
+        if rc:
+            raise RuntimeError(f"hctr_emb_pw_dot failed rc={rc}")
+        D._count()
+        return
+    tab = table.view(-1, ev_pitch)
+    for src in range(len(key_bufs)):
+        gbuf = grad_bufs[src].reshape(-1)
+        dbuf = dots[src].reshape(-1)
+        for j in sel:
+            lk = lookups[j]
+            own, rows, nnz = _bag(lk, key_bufs, nnz_bufs, src, batch)
+            g = torch.as_strided(gbuf, (batch, lk.ev_size), (lk.grad_stride, 1), gbuf.storage_offset() + lk.grad_off)
+            dot = (tab[rows][..., :lk.ev_size].float() * g.float().unsqueeze(1)).sum(-1)
+            if lk.combiner == 1:
+                dot = dot / nnz.clamp(min=1).view(-1, 1).float()
+            d = torch.as_strided(dbuf, (batch, lk.hotness), (lk.key_stride, 1), dbuf.storage_offset() + lk.key_off)
+            d.add_(torch.where(own, dot, torch.zeros((), dtype=torch.float32)))
+
+
+class PwReducePlan:
+    """The columns of the dot-product buffer that add into each element of the position weights' gradients:
+    ``targets`` = [(gradient [H] fp32, [(key_off, H) of every lookup of the input, in lookup order])]; element h of
+    a gradient takes position h of each of its lookups' regions, in that order."""
+
+    def __init__(self, targets, device):
+        self.targets = targets
+        self.n = sum(g.numel() for g, _ in targets)
+        self.cols_dev = self.targets_dev = None
+        if device.type == "cuda":
+            cols, tg = [], []
+            for g, regions in targets:
+                for h in range(g.numel()):
+                    tg.append(CPwReduceTarget(g.data_ptr() + 4 * h, len(cols), len(regions)))
+                    cols += [CPwReduceCol(off, H, h) for off, H in regions]
+            as_dev = lambda arr: torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).clone().to(device)
+            self.cols_dev = as_dev((CPwReduceCol * max(1, len(cols)))(*cols))
+            self.targets_dev = as_dev((CPwReduceTarget * max(1, len(tg)))(*tg))
+
+
+def pw_reduce(dots, batch, plan: PwReducePlan):
+    """Every element h of each gradient of ``plan`` += the sum over source ranks r and samples s of
+    dots[r, key_off + s * H + h] of each of its lookups, in a fixed order (``dots``: [ranks, n] fp32)."""
+    if not plan.n:
+        return
+    if dots.is_cuda:
+        rc = _pw_lib().hctr_emb_pw_reduce(dots.data_ptr(), dots.stride(0), batch, dots.shape[0], plan.cols_dev.data_ptr(),
+                                          plan.targets_dev.data_ptr(), plan.n, _st(dots.device))
+        if rc:
+            raise RuntimeError(f"hctr_emb_pw_reduce failed rc={rc}")
+        D._count()
+        return
+    for g, regions in plan.targets:
+        tot = torch.zeros(g.numel(), dtype=torch.float32)
+        for off, H in regions:
+            tot += dots[:, off:off + batch * H].reshape(-1, H).sum(0)
+        g.view(-1).add_(tot)

@@ -184,7 +184,8 @@ def model_to_json(model) -> dict:
                    "dense": {"top": inp.dense_name, "dense_dim": inp.dense_dim},
                    "sparse": [{"top": p.top_name, "type": "DistributedSlot",
                                "nnz_per_slot": p.nnz_per_slot, "is_fixed_length": p.is_fixed_length,
-                               "slot_num": p.slot_num, **({"weighted": True} if p.weighted else {})}
+                               "slot_num": p.slot_num, **({"weighted": True} if p.weighted else {}),
+                               **({"position_weighted": True} if getattr(p, "position_weighted", False) else {})}
                               for p in inp.data_reader_sparse_param_array]})
     for se in model.sparse_embeddings:
         o = se.optimizer or model.opt_params
@@ -247,7 +248,8 @@ def add_from_json(model, graph: dict, include_dense_network: bool = True):
     d = layers[0]
     assert d["type"] == "Data", "first layer of the graph JSON must be Data"
     sparse = [DataReaderSparseParam(s["top"], s["nnz_per_slot"], s["is_fixed_length"], s["slot_num"],
-                                    weighted=bool(s.get("weighted", False)))
+                                    weighted=bool(s.get("weighted", False)),
+                                    position_weighted=bool(s.get("position_weighted", False)))
               for s in d.get("sparse", [])]
     lab = d["label"]
     model.add(Input(label_dims=_as_list(lab["label_dim"]), label_names=_as_list(lab["top"]),

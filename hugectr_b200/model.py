@@ -32,6 +32,11 @@ from .solver import (DataReaderParams, DenseLayer, Input, OptParamsPy, Solver, S
 from .utils import logger
 
 
+def _ones(shape, gen):
+    """initial position weights: 1.0, the unweighted pooling (draws nothing from the arena's generator)"""
+    return torch.ones(shape)
+
+
 class TrainingCallback:
     """Overridable hooks (training_callback_wrapper.hpp:62-86)."""
 
@@ -121,6 +126,11 @@ class Model:
         self.arena.begin_replay()
         self.net_eval = self._build_network(False)
         self.arena.end_replay()
+        # the weights of the position-weighted inputs: dense parameters behind the network's own, so that a model
+        # without such inputs keeps its arena, dense files and optimizer state as they were
+        self.position_weights = {p.top_name: self.arena.add(f"{p.top_name}.position_weight",
+                                                            (p.slot_num, max(p.nnz_per_slot)), _ones)
+                                 for p in inp.data_reader_sparse_param_array if getattr(p, "position_weighted", False)}
         from .enums import AllReduceAlgo
         p2p_ar = (self.world > 1 and self.device.type == "cuda"
                   and s.all_reduce_algo in (AllReduceAlgo.OneShot, AllReduceAlgo.TwoShot)
@@ -129,6 +139,10 @@ class Model:
                             wgrad_alloc=self.comm.symm_alloc if p2p_ar else None)
         self.net_train.finalize()
         self.net_eval.finalize()
+        if self.position_weights:
+            pw = {n: (p.w, p.g) for n, p in self.position_weights.items()}
+            for e in self.ebcs_train + self.ebcs_eval:
+                e.bind_position_weights({n: pw[n] for n in e.pw_inputs})
         self.arena.init_params(s.seed)
         self._setup_losses(loss_names, loss_weights)
         self._create_dense_optimizer()
@@ -194,11 +208,22 @@ class Model:
                                  f"{getattr(se, 'sparse_embedding_name', '')} cannot pool weights "
                                  "(use an EmbeddingCollection lookup)")
 
+    def _check_position_weighted_inputs(self):
+        """Position-weighted inputs are pooled by embedding-collection lookups only."""
+        pw = {p.top_name for p in self.input.data_reader_sparse_param_array if getattr(p, "position_weighted", False)}
+        for se in self.sparse_embeddings:
+            if se.bottom_name in pw:
+                raise ValueError(f"position-weighted input {se.bottom_name}: the legacy SparseEmbedding "
+                                 f"{getattr(se, 'sparse_embedding_name', '')} cannot pool weights "
+                                 "(use an EmbeddingCollection lookup)")
+
     def _build_embeddings(self):
         s = self.solver
         self._check_weighted_inputs()
+        self._check_position_weighted_inputs()
         hot = {p.top_name: max(p.nnz_per_slot) for p in self.input.data_reader_sparse_param_array}
         weighted = {p.top_name for p in self.input.data_reader_sparse_param_array if getattr(p, "weighted", False)}
+        pw = {p.top_name for p in self.input.data_reader_sparse_param_array if getattr(p, "position_weighted", False)}
         self.ebcs_train, self.ebcs_eval = [], []
         state_dtype = torch.float32
         if os.environ.get("HCTR_EMB_STATE_BF16", "0") == "1":
@@ -219,7 +244,8 @@ class Model:
                                     self.act_dtype, self.comm, self.opt_params, self.key_dtype,
                                     scaler=s.scaler if self.mixed else 1.0, state_dtype=state_dtype,
                                     seed=s.seed,
-                                    fused=None if s.fused_embedding_comm else False, weighted=weighted, **kw)
+                                    fused=None if s.fused_embedding_comm else False, weighted=weighted,
+                                    position_weighted=pw, **kw)
             self.ebcs_train.append(e)
             self.ebcs_eval.append(e if self.serving else e.eval_clone(self.b_eval))
         self.legacy_train, self.legacy_eval = [], []
@@ -376,7 +402,7 @@ class Model:
         legs = self.legacy_train if is_train else self.legacy_eval
         if len(ebcs) == 1 and not legs:
             ebcs[0].set_keys(hb.keys)
-            if ebcs[0].has_weights:
+            if ebcs[0].has_data_weights:
                 ebcs[0].set_weights(hb.weights)
         else:
             b = self.b_train if is_train else self.b_eval
@@ -386,7 +412,7 @@ class Model:
                     o = offs[gl["bottom"]]
                     e.key_views[gl["bottom"]].copy_(
                         hb.keys[o:o + b * gl["hotness"]].view(b, gl["hotness"]), non_blocking=nb)
-                    if gl["weighted"]:
+                    if gl["weighted"] and not gl["pw"]:
                         e.weight_views[gl["bottom"]].copy_(
                             hb.weights[o:o + b * gl["hotness"]].view(b, gl["hotness"]), non_blocking=nb)
             for rt in legs:
@@ -514,6 +540,12 @@ class Model:
                 rt.forward(True)
             net.fprop(True)
             net.bprop()
+            if self.position_weights and not frozen_emb:
+                # the embedding backward produces the gradient of the position weights: ahead of the dense step
+                for e in self.ebcs_train:
+                    e.backward(self.lr_t, self.step_t)
+        for e in self.ebcs_train:
+            e.wait_position_weight_grad()
         if not self.dense_frozen:
             if bucketed:
                 self.exchange_wgrad.finish_step()      # all-reduce + optimizer, bucket by bucket
@@ -526,7 +558,7 @@ class Model:
             torch.cuda.current_stream().wait_stream(self._s_emb)
         else:
             for e in self.ebcs_train:
-                if not frozen_emb:
+                if not frozen_emb and not self.position_weights:
                     e.backward(self.lr_t, self.step_t)
             for rt in self.legacy_train:
                 if not self.embedding_frozen.get(rt.name, frozen_emb):
@@ -708,7 +740,7 @@ class Model:
             self._stg = {"label": torch.empty_like(self.net_train.tensors[self.input.label_name].data),
                          "dense": torch.empty_like(self.net_train.tensors[self.input.dense_name].data),
                          "keys": torch.empty_like(self.ebcs_train[0].key_slab)}
-            if self.ebcs_train[0].has_weights:
+            if self.ebcs_train[0].has_data_weights:
                 self._stg["weights"] = torch.empty_like(self.ebcs_train[0].weight_slab)
             self._stg_free = torch.cuda.Event()
             self._stg_free.record()

@@ -304,6 +304,11 @@ def convert(onnx_model_path: str, graph_config: str, dense_model: str, convert_e
             sparse_models: Optional[List[str]] = None, ntp_file: Optional[str] = None,
             graph_name: str = "hugectr", batch_size: int = 2) -> InferenceGraph:
     graph = json.load(open(graph_config))
+    for s in graph["layers"][0].get("sparse", []):
+        if s.get("position_weighted"):
+            # (checked before the dense file is read: the position weights follow the network's parameters in it)
+            raise ValueError(f"position-weighted input {s['top']}: the ONNX export does not carry the position "
+                             "weights")
     ntp = json.load(open(ntp_file)) if ntp_file and os.path.exists(ntp_file) else None
     g = InferenceGraph(graph, load_dense_weights(dense_model), sparse_models or [], convert_embedding, ntp)
     data = graph["layers"][0]

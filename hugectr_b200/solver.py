@@ -190,11 +190,19 @@ def CreateOptimizer(optimizer_type=Optimizer_t.Adam, update_type=Update_t.Global
 # --------------------------------------------------------------------------- data reader params
 class DataReaderSparseParam:
     def __init__(self, top_name: str, nnz_per_slot: Union[int, Sequence[int]],
-                 is_fixed_length: bool, slot_num: int, weighted: bool = False):
+                 is_fixed_length: bool, slot_num: int, weighted: bool = False, position_weighted: bool = False):
         """``weighted``: the reader delivers an fp32 weight with every key of this input, and every
-        embedding lookup of it pools weighted (see docs/embedding.md)."""
+        embedding lookup of it pools weighted (see docs/embedding.md).
+        ``position_weighted``: key h of slot f of every sample weighs ``P[f, h]``, a trainable fp32 parameter
+        ``[slot_num, max(nnz_per_slot)]`` of the dense network that starts at 1.0 (see docs/embedding.md)."""
         self.top_name = top_name
         self.weighted = bool(weighted)
+        if not isinstance(position_weighted, bool):
+            raise ValueError(f"input {top_name}: position_weighted must be a bool, not {position_weighted!r}")
+        if position_weighted and self.weighted:
+            raise ValueError(f"input {top_name}: weighted and position_weighted exclude each other (the weights "
+                             "come either from the reader or from the model)")
+        self.position_weighted = position_weighted
         if isinstance(nnz_per_slot, int):
             self.nnz_per_slot = [nnz_per_slot] * slot_num
         else:
@@ -211,7 +219,8 @@ class DataReaderSparseParam:
                 "nnz_per_slot": self.nnz_per_slot if len(set(self.nnz_per_slot)) > 1
                 else self.nnz_per_slot[0],
                 "is_fixed_length": self.is_fixed_length, "slot_num": self.slot_num,
-                **({"weighted": True} if self.weighted else {})}
+                **({"weighted": True} if self.weighted else {}),
+                **({"position_weighted": True} if self.position_weighted else {})}
 
 
 @dataclass

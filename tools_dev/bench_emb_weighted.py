@@ -1,17 +1,20 @@
-"""Device time of the embedding lookup + fused backward with every input weighted against the same collection
-unweighted, at the DLRM-DCNv2 embedding shapes.
+"""Device time of the embedding lookup + fused backward with every input weighted, and with every input
+position-weighted, against the same collection unweighted, at the DLRM-DCNv2 embedding shapes.
 
-  python tools_dev/bench_emb_weighted.py [--steps 30] [--warmup 5] [--rounds 3] [--ev 128] [--cap-rows 4000000]
+  python tools_dev/bench_emb_weighted.py [--steps 30] [--warmup 5] [--rounds 3] [--ev 128] [--cap-rows 2500000]
+      [--arms unweighted,weighted,position_weighted]
 
 The 26 Criteo-TB tables, batch 6912, the DCNv2 multi-hot sizes (214 keys per sample), power-law keys (alpha
-1.1), AdaGrad, fp32 weights and activations, one GPU.  Tables are capped at --cap-rows rows: both collections
-(fp32 weights and AdaGrad state) live on the card at once, so that the two arms can alternate in one process;
-bench.py's 10M-row cap holds one of them only.  Both collections start from the same tables.  Each round times
+1.1), AdaGrad, fp32 weights and activations, one GPU.  Tables are capped at --cap-rows rows: the collections of all
+arms (fp32 weights and AdaGrad state, about 16.6 GB each at 2.5M rows) live on the card at once, so that the arms can
+alternate in one process; bench.py's 10M-row cap holds one of them only.  All collections start from the same tables.
+The position-weighted arm's step adds the fill of the weights from P, the weight-gradient dot products of every
+looked-up row and their column sums into P's gradient (P stays at 1: the step does not run the dense optimizer).  Each round times
 --steps steps of each arm (forward + backward between CUDA events, median), the arms alternating; the result
 is the median over rounds, printed as one JSON line with the card name and its power limit, the keys per step
 and the extra bytes the weights add per step (one fp32 weight read per key by the lookup and by the backward
 index).  ``--profile`` adds, from one more step of each arm under torch.profiler, the device time per kernel
-name (summed over launches) of both arms.  Without a CUDA device it exits and measures nothing.
+name (summed over launches) of every arm.  Without a CUDA device it exits and measures nothing.
 """
 import argparse
 import json
@@ -36,7 +39,7 @@ def card():
     return name, pl or "unknown"
 
 
-def collection(sizes, hot, ev, weighted, dev):
+def collection(sizes, hot, ev, arm, dev):
     from hugectr_b200.embedding.collection import (EmbeddingCollection, EmbeddingCollectionConfig,
                                                    EmbeddingTableConfig)
     from hugectr_b200.enums import Optimizer_t
@@ -47,8 +50,13 @@ def collection(sizes, hot, ev, weighted, dev):
     names = [f"s{i}" for i in range(len(hot))]
     cfg.embedding_lookup(tabs, names, "emb", ["sum"] * len(hot))
     opt = CreateOptimizer(Optimizer_t.AdaGrad, initial_accu_value=0.0, epsilon=1e-8)
-    return EmbeddingCollection(cfg, BATCH, dict(zip(names, hot)), dev, torch.float32, Comm.single(dev), opt,
-                               seed=1, weighted=names if weighted else ())
+    e = EmbeddingCollection(cfg, BATCH, dict(zip(names, hot)), dev, torch.float32, Comm.single(dev), opt, seed=1,
+                            weighted=names if arm == "weighted" else (),
+                            position_weighted=names if arm == "position_weighted" else ())
+    if arm == "position_weighted":
+        e.bind_position_weights({n: (torch.ones(1, h, device=dev), torch.zeros(1, h, device=dev))
+                                 for n, h in zip(names, hot)})
+    return e
 
 
 def batches(sizes, hot, n, dev):
@@ -69,7 +77,7 @@ def run(e, data, steps, warmup):
     for it in range(warmup + steps):
         keys, w = data[it % len(data)]
         e.set_keys(keys)
-        if e.has_weights:
+        if e.has_data_weights:
             e.set_weights(w)
         ev[0].record()
         e.forward()
@@ -104,7 +112,8 @@ def main(argv):
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--ev", type=int, default=128)
-    ap.add_argument("--cap-rows", type=int, default=4_000_000)
+    ap.add_argument("--cap-rows", type=int, default=2_500_000)
+    ap.add_argument("--arms", default="unweighted,weighted,position_weighted")
     ap.add_argument("--profile", action="store_true")
     a = ap.parse_args(argv)
     if not torch.cuda.is_available():
@@ -115,9 +124,11 @@ def main(argv):
     dev = torch.device("cuda")
     name, plim = card()
     data = batches(sizes, hot, 8, dev)
-    arms = {"unweighted": collection(sizes, hot, a.ev, False, dev), "weighted": collection(sizes, hot, a.ev, True, dev)}
-    for g_w, g_u in zip(arms["weighted"].groups, arms["unweighted"].groups):
-        g_w.table.copy_(g_u.table)
+    arms = {k: collection(sizes, hot, a.ev, k, dev) for k in a.arms.split(",")}
+    first = next(iter(arms.values()))
+    for e in arms.values():
+        for g, g0 in zip(e.groups, first.groups):
+            g.table.copy_(g0.table)
     times = {k: [] for k in arms}
     for _ in range(a.rounds):
         for k, e in arms.items():
@@ -125,17 +136,18 @@ def main(argv):
     med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
     n_keys = BATCH * sum(hot)
     print(json.dumps({"tables": len(hot), "batch": BATCH, "keys_per_step": n_keys, "ev": a.ev, "cap_rows": a.cap_rows,
-                      "optimizer": "AdaGrad", "unweighted_ms": round(med["unweighted"], 4),
-                      "weighted_ms": round(med["weighted"], 4),
-                      "weighted_over_unweighted": round(med["weighted"] / med["unweighted"], 4),
+                      "optimizer": "AdaGrad", **{f"{k}_ms": round(v, 4) for k, v in med.items()},
+                      **{f"{k}_over_unweighted": round(v / med["unweighted"], 4) for k, v in med.items()
+                         if k != "unweighted" and "unweighted" in med},
                       "rounds_ms": {k: [round(x, 4) for x in v] for k, v in times.items()},
                       "weight_bytes_per_step": 2 * n_keys * 4, "row_bytes_per_step_fwd": n_keys * a.ev * 4,
+                      # the weight gradient reads every looked-up row once more
+                      "pw_grad_row_bytes_per_step": n_keys * a.ev * 4,
                       "card": name, "power_limit": plim}), flush=True)
     if a.profile:
         kt = {k: kernel_times(e, data) for k, e in arms.items()}
-        names = sorted(set(kt["unweighted"]) | set(kt["weighted"]),
-                       key=lambda n: -max(kt["unweighted"].get(n, 0), kt["weighted"].get(n, 0)))
-        print(json.dumps({"kernel_us": [[n, kt["unweighted"].get(n, 0), kt["weighted"].get(n, 0)] for n in names[:25]]}),
+        names = sorted(set().union(*kt.values()), key=lambda n: -max(t.get(n, 0) for t in kt.values()))
+        print(json.dumps({"arms": list(kt), "kernel_us": [[n] + [t.get(n, 0) for t in kt.values()] for n in names[:25]]}),
               flush=True)
     return 0
 
